@@ -36,19 +36,7 @@ METRIC = "waveform-samples/sec PASE+ encoder fwd+bwd (B=32,T=32000 per GPU)"
 # SURVEY.md 8(d): algorithmic work per 32000-sample chunk
 FLOP_PER_CHUNK = 25.4e9          # fwd+bwd as the reference computes it
 BYTES_PER_CHUNK = 96.5e6         # ideal-fusion HBM traffic, fp32
-FP32_FFMA_PEAK_TF = 74.4         # 148 SM x 128 lanes x 2 x 1.965 GHz
-
-
-def gemm_traffic(precision):
-    """Mean DRAM bytes per GEMM launch (dram__bytes_read.sum + dram__bytes_write.sum over the
-    GEMM launches of one step) from the committed `ncu --set full` capture of the CURRENT
-    kernels in this precision (profiles/r02_gemm_traffic.json, written by
-    profiles/summarize.py traffic); None when this precision was not captured."""
-    path = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    if not os.path.exists(path):
-        return None
-    ent = json.load(open(path)).get(precision)
-    return None if ent is None else ent["dram_bytes_per_launch"]
+FP32_FFMA_PEAK_TF = 67.0         # H100 SXM data sheet: 132 SM x 128 lanes x 2 x 1.98 GHz
 
 
 def load_peaks():
@@ -57,7 +45,8 @@ def load_peaks():
         d = json.load(open(path))
         return {"hbm_gbs": d["hbm_gbs"], "tf": d["bf16_tflops"],
                 "tf_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+    # H100 SXM data sheet (700 W card): HBM3 bandwidth, dense bf16
+    return {"hbm_gbs": 3350.0, "tf": 989.0, "tf_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
@@ -293,8 +282,7 @@ def time_workers(dev, precision, B, T=T_CHUNK, steps=5, warmup=3, graph=True, st
             "frac": ach / peak, "traffic": None,
             "algorithmic_gflop_per_step": gflop,
             "note": "FLOPs as the reference computes the step (SURVEY.md 8d), counted once per "
-                    "product; peak = sustained bf16 tensor rate (" + pk["src"] + "); "
-                    "per-kernel times of this step: profiles/r02_timeline_workers.md"}
+                    "product; peak = bf16 tensor rate (" + pk["src"] + ")"}
     return {"metric": "waveform-samples/sec PASE+ encoder(3B chunks)+workers+ heads fwd+bwd+adam",
             "roofline": roof,
             "value": B * T / (ms * 1e-3), "unit": "chunk-samples/s", "ms_per_step": ms,
@@ -334,8 +322,8 @@ def _event_time(fn, steps):
 
 def measure_matmul_peaks(dev):
     """Dense tensor-core peaks of THIS GPU as cuBLAS reaches them (torch.matmul, 8192^3, best
-    of 5 bursts of 10 back-to-back GEMMs): TF32 and fp16, next to the driver-measured bf16
-    figure of MEASURED_PEAKS.json.  Denominators for the issued-MMA fractions."""
+    of 5 bursts of 10 back-to-back GEMMs): TF32, fp16 and bf16.  Denominators for the
+    issued-MMA fractions."""
     out = {}
     n = 8192
     prev = torch.backends.cuda.matmul.allow_tf32
@@ -356,7 +344,7 @@ def measure_matmul_peaks(dev):
 
 
 def library_baseline(dev, steps=5):
-    """SURVEY 8(d) / BASELINE.md 4.4: the reference's own module graph on this B200 through
+    """SURVEY 8(d) / BASELINE.md 4.4: the reference's own module graph on this GPU through
     the vendor libraries (cuDNN conv / batch-norm, cuBLAS), `cudnn.benchmark=True` as
     train.py:26 sets it: the oracle restatement with lib_ops on CUDA tensors, fwd + bwd +
     fused Adam on the same synthetic (32,1,32000) batch, once with TF32 allowed (PyTorch's
@@ -424,9 +412,8 @@ def time_encoder_config(dev, stream, precision, B, T, steps=10):
 
 
 def gemm_time_in_replay(step_fn, gemm_flop_per_step, peak_tflops, reps=3):
-    """Sum of the tcgen05 GEMM kernels' device durations inside `reps` replays of the captured
-    step, from torch.profiler's CUDA activity records (same method as tools/gpu/kineto_step.py,
-    profiles/r02_timeline_*.md)."""
+    """Sum of the tensor-core GEMM kernels' device durations inside `reps` replays of the
+    captured step, from torch.profiler's CUDA activity records."""
     from torch.profiler import profile, ProfilerActivity
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -476,6 +463,14 @@ def time_lps_targets(dev, B=B_PER_GPU, T=T_CHUNK, reps=10):
             "cpu_reference_ms_per_step_one_core": cpu_ms_chunk * B,
             "note": "reference path = oracle/targets_oracle.py (torch.stft + savgol deltas) per "
                     "chunk on one host core, as a DataLoader worker runs it"}
+
+
+def dump_outputs(d, arrays):
+    """arrays: name -> tensor (float32 / float64), written as d/<name>.npy"""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), t.cpu().numpy())
 
 
 # ------------------------------------------------------------------ GPU arm ---
@@ -548,10 +543,19 @@ def run_native(args):
     x_host = torch.randn(B_PER_GPU, 1, T_CHUNK, generator=g).pin_memory()
     x_dev = x_host.to(dev)
 
+    last = {}
+
+    def loss_of(y):
+        """the step's loss; keeps the step's output and loss for --dump-outputs (in a captured
+        step these are the graph's static tensors, rewritten by every replay)"""
+        last["output"] = y
+        last["loss"] = y.square().mean()
+        return last["loss"]
+
     def step_resident():
         zero_grads()
         y = model(x_dev)
-        loss = y.square().mean()
+        loss = loss_of(y)
         loss.backward()
         reduce_grads()
         opt.step()
@@ -606,11 +610,11 @@ def run_native(args):
             gopt = torch.optim.Adam(params, lr=1e-4, fused=True, capturable=True) \
                 if args.torch_adam else opt
             if world > 1 and not args.torch_adam and args.overlap:
-                gres = PipelinedDPStep(model, opt, lambda y: y.square().mean(),
+                gres = PipelinedDPStep(model, opt, loss_of,
                                        (B_PER_GPU, 1, T_CHUNK), dev, split=DP_SPLIT,
                                        n_lower=n_lower, stream=side, resident=True)
             else:
-                gres = GraphedEncoderStep(model, gopt, lambda y: y.square().mean(),
+                gres = GraphedEncoderStep(model, gopt, loss_of,
                                           (B_PER_GPU, 1, T_CHUNK), dev, stream=side,
                                           resident=True, **gkw)
             gres.x_static.copy_(x_dev)
@@ -627,6 +631,13 @@ def run_native(args):
     if sampler:
         sampler.stop_flag = True
         sampler.join(timeout=2)
+    if args.dump_outputs and rank == 0:
+        # what the last timed step returned: its loss and encoder output, and the parameters
+        # its Adam update wrote (7.8 M fp32), before any later step touches them
+        dump_outputs(args.dump_outputs, {
+            "loss": last["loss"].detach().double(),
+            "output": last["output"].detach().float(),
+            "params": torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])})
 
     # end-to-end: through the public API with pinned HOST waveforms; the whole step (H2D, fwd,
     # bwd, Adam, D2H of the loss) is captured in one CUDA graph (N>1: two, around the
@@ -713,9 +724,9 @@ def run_native(args):
             "metric": METRIC, "value": value, "unit": "samples/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": step_ms,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": {"fp32": "f32", "3xtf32": "f32 (3xTF32 split on tcgen05, fp32 accumulate: "
+            "dtype": {"fp32": "f32", "3xtf32": "f32 (3xTF32 split on wgmma, fp32 accumulate: "
                       "fp32-equivalent products)",
-                      "3xf16": "f32 (3xF16 split on tcgen05, fp32 accumulate: fp32-equivalent "
+                      "3xf16": "f32 (3xF16 split on wgmma, fp32 accumulate: fp32-equivalent "
                                "products)", "tf32": "tf32", "bf16": "bf16"}[args.precision],
             "data": "synthetic",
             "parity": "oracle pinned to goldens of the unmodified reference (tests/golden); the "
@@ -726,7 +737,7 @@ def run_native(args):
                        "global_batch": B_PER_GPU * world, "seq_len": T_CHUNK,
                        "parallelism": "dp%d" % world, "gemm_precision": args.precision,
                        "cuda_graph": value_graphed,
-                       "l2": "no flush: per-step working set (~1.7 GB activations) >> 126 MB L2",
+                       "l2": "no flush: per-step working set (~1.7 GB activations) >> 50 MB L2",
                        "optimizer": "torch fused Adam" if args.torch_adam else
                        ("pase_adam_flat_dp (one launch, moments sharded over the ranks)"
                         if peer else "pase_adam_flat (one launch, gradients written in place)"),
@@ -748,17 +759,16 @@ def run_native(args):
             "roofline": {
                 "kernel": {"fp32": "pase_gemm_nt + pase_gemm_tn (fp32 FFMA implicit-GEMM conv "
                                    "fwd/dgrad/wgrad)",
-                           "3xtf32": "pase_tc_gemm_nt + pase_tc_gemm_tn (tcgen05 kind::tf32, 3 MMAs "
+                           "3xtf32": "pase_tc_gemm_nt + pase_tc_gemm_tn (wgmma tf32, 3 MMAs "
                                      "per product; FLOPs counted once)",
-                           "3xf16": "pase_tc_gemm_nt + pase_tc_gemm_tn (tcgen05 kind::f16 on fp16 "
+                           "3xf16": "pase_tc_gemm_nt + pase_tc_gemm_tn (wgmma f16 on fp16 "
                                     "hi/lo pairs, 3 MMAs per product; FLOPs counted once)",
-                           "bf16": "pase_tc_gemm_nt + pase_tc_gemm_tn (tcgen05 kind::f16, bf16)",
-                           "tf32": "pase_tc_gemm_nt + pase_tc_gemm_tn (tcgen05 kind::tf32)"}[
+                           "bf16": "pase_tc_gemm_nt + pase_tc_gemm_tn (wgmma bf16)",
+                           "tf32": "pase_tc_gemm_nt + pase_tc_gemm_tn (wgmma tf32)"}[
                     args.precision],
                 "bound": "tensor", "achieved": ach_tf, "peak": peaks["tf_sustained"],
                 "unit": "TFLOP/s", "frac": ach_tf / peaks["tf_sustained"],
-                "traffic": gemm_traffic(args.precision),
-                "peak_source": peaks["src"] + " bf16 sustained (kernel timed inside a long step)",
+                "peak_source": peaks["src"] + " bf16",
                 "gemm_share_of_step": gemm_ms / step_ms if step_ms > 0 else None,
                 "gemm_ms_per_step": gemm_ms, "gemm_gflop_per_step": gemm_flop / 1e9,
                 "frac_of_fp32_ffma_peak": ach_tf / FP32_FFMA_PEAK_TF,
@@ -851,10 +861,9 @@ def main():
                          "ncclAllReduce(avg) of the flat buffer between two graph replays")
     ap.add_argument("--overlap", action="store_true",
                     help="N>1: hide the all-reduce of the large gradient bucket behind the tail "
-                         "of backward (PipelinedDPStep, three graphs + side stream).  Measured "
-                         "at N=2: 3.49 ms/step vs 3.42 for one all-reduce between two graph "
-                         "replays (NVLink moves 31 MB in ~0.05 ms; the extra graph launches, "
-                         "events and SM contention cost more), so the plain form is the default")
+                         "of backward (PipelinedDPStep, three graphs + side stream); the extra "
+                         "graph launches, events and SM contention can cost more than the "
+                         "all-reduce of 31 MB over NVLink, so the plain form is the default")
     ap.add_argument("--no-fuse-heads", action="store_true",
                     help="workers workload: materialise the regression predictions (reference "
                          "protocol) instead of fusing output layer + contextualised MSE")
@@ -873,9 +882,14 @@ def main():
     ap.add_argument("--batch", type=int, default=32, help="chunk triplets per step (workers workload)")
     ap.add_argument("--precision", default=os.environ.get("PASE_B200_PRECISION", "3xf16"),
                     choices=["fp32", "3xtf32", "3xf16", "tf32", "bf16"],
-                    help="GEMM numerics: fp32 FFMA; 3xTF32 / 3xF16 tcgen05 (fp32-equivalent); TF32 "
-                         "tcgen05; bf16 tcgen05 with bf16 activation storage (BASELINE configs[2,4])")
+                    help="GEMM numerics: fp32 FFMA; 3xTF32 / 3xF16 wgmma (fp32-equivalent); TF32 "
+                         "wgmma; bf16 wgmma with bf16 activation storage (BASELINE configs[2,4])")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="encoder workload: after the timed steps, write the last timed step's "
+                         "loss, encoder output and updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "native" or args.workload != "encoder"):
+        raise SystemExit("--dump-outputs: encoder workload of the native implementation only")
     if args.impl == "reference":
         run_reference(args)
     elif args.workload == "workers":

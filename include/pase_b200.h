@@ -1,5 +1,5 @@
 /*
- * pase_b200 -- C-ABI of the B200-native PASE/PASE+ hot path (sm_100a).
+ * pase_b200 -- C-ABI of the native PASE/PASE+ hot path (H100, sm_90a).
  *
  * The reference (santi-pdp/pase) is pure Python/PyTorch and has no FFI; the
  * boundary a maintainer binds is therefore this library, loaded with ctypes
@@ -66,14 +66,14 @@ int pase_gemm_tn(const float* A, long lda, int pitchA, int offA,
                  float alpha, int accumulate, void* stream);
 
 
-/* ---- tensor-core (tcgen05 / TMEM / TMA) GEMMs ------------------------------
- * Same contract as pase_gemm_nt / pase_gemm_tn, computed with tcgen05 UMMA
- * instructions and fp32 accumulation in tensor memory.  `mode` selects the
+/* ---- tensor-core (wgmma / TMA) GEMMs ---------------------------------------
+ * Same contract as pase_gemm_nt / pase_gemm_tn, computed with wgmma
+ * instructions and fp32 accumulation in registers.  `mode` selects the
  * operand element type and the numerics:
  *   0  TF32   : fp32 operands read as tf32, one pass;
  *   1  3xTF32 : fp32 operands pre-split by pase_split_tf32 into exactly
  *               representable hi/lo parts = fp32-equivalent products;
- *   2  BF16   : bf16 operands (kind::f16), one pass at twice the TF32 rate;
+ *   2  BF16   : bf16 operands, one pass at twice the TF32 rate;
  *   3  3xF16  : fp16 operand pairs x = hi + 2^-11 lo' (pase_split_f16 or the
  *               producing kernel) = fp32-equivalent products at half the tensor
  *               time and operand bytes of 3xTF32; operands must fit fp16's

@@ -1,11 +1,11 @@
 """Reference harness -- TEST INFRASTRUCTURE, container-only.
 
-Imports the UNMODIFIED reference (santi-pdp/pase, mounted read-only at
-/root/reference) on CPU so that (a) the CPU restatement in
+Imports the UNMODIFIED reference (a read-only checkout of santi-pdp/pase at
+$PASE_REFERENCE_ROOT) on CPU so that (a) the CPU restatement in
 ``oracle/pase_oracle.py`` can be pinned against the real thing and (b) golden
-vectors can be generated (``tests/golden/make_golden.py``).  /root/reference
-does not exist on the GPU box, so nothing that runs there may import this
-module; it raises ImportError when the reference tree is absent.
+vectors can be generated (``tests/golden/make_golden.py``).  The tests and the
+benchmark never import this module: they run without the reference; it raises
+ImportError when the reference tree is absent.
 
 Shims (SURVEY.md section 8c):
   * ``soundfile``  -- import-only dependency of pase/models/pase.py:15.
@@ -23,11 +23,11 @@ import json
 import contextlib
 import io
 
-REF_ROOT = os.environ.get("PASE_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("PASE_REFERENCE_ROOT", "")
 
 
 def reference_available():
-    return os.path.isdir(os.path.join(REF_ROOT, "pase", "models"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "pase", "models"))
 
 
 def _install_shims():

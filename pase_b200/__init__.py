@@ -1,4 +1,4 @@
-"""pase_b200 -- B200-native (sm_100a) implementation of the PASE/PASE+ hot path.
+"""pase_b200 -- H100-native (sm_90a) implementation of the PASE/PASE+ hot path.
 
 Drop-in for the reference's ``pase.models.frontend.wf_builder`` /
 ``pase.models.pase.pase`` API (see INTEGRATION.md); all compute runs in the

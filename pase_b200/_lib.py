@@ -48,7 +48,7 @@ _lib = None
 
 
 def build(verbose=False):
-    """Compile every CUDA source for sm_100a into csrc/libpase_b200.so."""
+    """Compile every CUDA source for sm_90a into csrc/libpase_b200.so."""
     cmd = ["make", "-C", CSRC, "-j8"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if verbose:

@@ -86,7 +86,9 @@ __device__ __forceinline__ float prelu1(float u, float a) { return u > 0.f ? u :
 //   YT  storage type of y (float / bf16);  DF  operand format of dst:
 //   PASE_FMT_F32 (+ optional tf32-residual twin dst_lo), PASE_FMT_BF16, PASE_FMT_F16X2
 //   (dst = hi, dst_lo = lo').  The dense-skip pool accumulates the value the next layer
-//   reads (i.e. after rounding to bf16 in the bf16 format).
+//   reads (i.e. after rounding to bf16 in the bf16 format); the thread that writes the first
+//   time step of a pooling window sums the whole window in time order, so each window mean
+//   has one writer and comes out the same on every run.
 template <typename YT, int DF, int RUN>
 __global__ void __launch_bounds__(THREADS)
 bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
@@ -107,18 +109,6 @@ bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
   const YT* yn = y + (long)n * y_ss;
   const int pool_len = pool_d > 0 ? pool_T * pool_d : 0;
   const float inv_d = pool_d > 0 ? 1.f / (float)pool_d : 0.f;
-  float4 pacc = make_float4(0.f, 0.f, 0.f, 0.f);
-  int pw = -1;
-  auto flush = [&]() {
-    if (pw >= 0) {
-      float* pp = pool + (long)n * p_ss + (long)pw * p_rs + c;
-      atomicAdd(pp + 0, pacc.x * inv_d);
-      atomicAdd(pp + 1, pacc.y * inv_d);
-      atomicAdd(pp + 2, pacc.z * inv_d);
-      atomicAdd(pp + 3, pacc.w * inv_d);
-    }
-    pacc = make_float4(0.f, 0.f, 0.f, 0.f);
-  };
   const int nvalid = (Tp - tau0) < RUN ? (int)(Tp - tau0) : RUN;
   float4 vals[RUN];
 #pragma unroll
@@ -149,16 +139,25 @@ bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
     } else {
       st4_f16x2(reinterpret_cast<__half*>(dst_v) + o, reinterpret_cast<__half*>(dst_lo_v) + o, a);
     }
-    if (tr >= 0 && tr < pool_len) {
-      const int w = tr / pool_d;
-      if (w != pw) {
-        flush();
-        pw = w;
+    if (tr >= 0 && tr < pool_len && tr % pool_d == 0) {
+      float4 ps = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int k = 0; k < pool_d; ++k) {
+        const float4 w = ld4t(yn + (long)(tr + k) * C + c);
+        float4 b;
+        b.x = prelu1(fmaf(w.x, sc.x, sh.x), al.x);
+        b.y = prelu1(fmaf(w.y, sc.y, sh.y), al.y);
+        b.z = prelu1(fmaf(w.z, sc.z, sh.z), al.z);
+        b.w = prelu1(fmaf(w.w, sc.w, sh.w), al.w);
+        if constexpr (DF == PASE_FMT_BF16) b = rt4t(static_cast<const __nv_bfloat16*>(nullptr), b);
+        ps.x += b.x; ps.y += b.y; ps.z += b.z; ps.w += b.w;
       }
-      pacc.x += a.x; pacc.y += a.y; pacc.z += a.z; pacc.w += a.w;
+      float* pp = pool + (long)n * p_ss + (long)(tr / pool_d) * p_rs + c;
+      atomicAdd(pp + 0, ps.x * inv_d);
+      atomicAdd(pp + 1, ps.y * inv_d);
+      atomicAdd(pp + 2, ps.z * inv_d);
+      atomicAdd(pp + 3, ps.w * inv_d);
     }
   }
-  flush();
 }
 
 // ---- backward pass 1: du + reductions ----
@@ -230,8 +229,12 @@ bn_prelu_bwd_reduce_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                            const float* __restrict__ alpha, BwdSrc s, YT* __restrict__ dst,
                            long d_ss, double* __restrict__ S1, double* __restrict__ S2,
                            double* __restrict__ dalpha, float* __restrict__ amax) {
-  extern __shared__ float red[];      // [3][C] (+ [2] maxima)
-  for (int i = threadIdx.x; i < 3 * C + 2; i += blockDim.x) red[i] = 0.f;
+  // block sums [3][C] in fp64: the order of the threads' additions then only moves bits below
+  // fp32 precision (run-to-run identical statistics); [2] maxima in fp32 after them
+  extern __shared__ double red[];
+  float* redm = reinterpret_cast<float*>(red + 3 * C);
+  for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) red[i] = 0.0;
+  if (threadIdx.x < 2) redm[threadIdx.x] = 0.f;
   __syncthreads();
   const int C4 = C >> 2;
   const int n = blockIdx.y;
@@ -298,9 +301,9 @@ bn_prelu_bwd_reduce_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
   if ((pre && (threadIdx.x & 31) < C4) || (!pre && idx0 < nthreads)) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      atomicAdd(&red[0 * C + c + k], a1[k]);
-      atomicAdd(&red[1 * C + c + k], a2[k]);
-      atomicAdd(&red[2 * C + c + k], a3[k]);
+      atomicAdd(&red[0 * C + c + k], (double)a1[k]);
+      atomicAdd(&red[1 * C + c + k], (double)a2[k]);
+      atomicAdd(&red[2 * C + c + k], (double)a3[k]);
     }
   }
   if (amax != nullptr) {
@@ -310,19 +313,19 @@ bn_prelu_bwd_reduce_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
       mx_xh = fmaxf(mx_xh, __shfl_xor_sync(0xffffffffu, mx_xh, off));
     }
     if ((threadIdx.x & 31) == 0) {
-      atomic_max_pos(&red[3 * C], mx_du);
-      atomic_max_pos(&red[3 * C + 1], mx_xh);
+      atomic_max_pos(&redm[0], mx_du);
+      atomic_max_pos(&redm[1], mx_xh);
     }
   }
   __syncthreads();
   for (int i = threadIdx.x; i < C; i += blockDim.x) {
-    atomicAdd(S1 + i, (double)red[0 * C + i]);
-    atomicAdd(S2 + i, (double)red[1 * C + i]);
-    atomicAdd(dalpha + i, (double)red[2 * C + i]);
+    atomicAdd(S1 + i, red[0 * C + i]);
+    atomicAdd(S2 + i, red[1 * C + i]);
+    atomicAdd(dalpha + i, red[2 * C + i]);
   }
   if (amax != nullptr && threadIdx.x == 0) {
-    atomic_max_pos(amax, red[3 * C]);
-    atomic_max_pos(amax + 1, red[3 * C + 1]);
+    atomic_max_pos(amax, redm[0]);
+    atomic_max_pos(amax + 1, redm[1]);
   }
 }
 
@@ -341,8 +344,10 @@ bn_prelu_bwd_apply_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                           const YT* du, void* dst_v, long d_ss,
                           double* __restrict__ dbias, void* dst_lo_v,
                           const float* __restrict__ amax, float* __restrict__ scale_out) {
-  extern __shared__ float red[];      // [C] + [1]
-  for (int i = threadIdx.x; i < C + 1; i += blockDim.x) red[i] = 0.f;
+  extern __shared__ double red[];     // [C] fp64 sums (see pass 1), then [1] fp32 maximum
+  float* redm = reinterpret_cast<float*>(red + C);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) red[i] = 0.0;
+  if (threadIdx.x == 0) redm[0] = 0.f;
   __syncthreads();
   float gs_scale = 1.f;
   if constexpr (DF == PASE_FMT_F16X2) {
@@ -355,9 +360,9 @@ bn_prelu_bwd_apply_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
     }
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, off));
-    if ((threadIdx.x & 31) == 0) atomic_max_pos(&red[C], b);
+    if ((threadIdx.x & 31) == 0) atomic_max_pos(&redm[0], b);
     __syncthreads();
-    gs_scale = f16_grad_scale(red[C] * 1.0001f);
+    gs_scale = f16_grad_scale(redm[0] * 1.0001f);
     if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
       scale_out[0] = 1.f / gs_scale;
       scale_out[1] = gs_scale;
@@ -424,12 +429,12 @@ bn_prelu_bwd_apply_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
     }
     if (dbias) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) atomicAdd(&red[c + k], acc[k]);
+      for (int k = 0; k < 4; ++k) atomicAdd(&red[c + k], (double)acc[k]);
     }
   }
   if (dbias) {
     __syncthreads();
-    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, (double)red[i]);
+    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, red[i]);
   }
 }
 
@@ -447,8 +452,10 @@ bn_prelu_bwd_apply_src_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                               double inv_count, BwdSrc s, void* dst_v, long d_ss,
                               double* __restrict__ dbias, void* dst_lo_v,
                               const float* __restrict__ amax, float* __restrict__ scale_out) {
-  extern __shared__ float red[];      // [C] + [1]
-  for (int i = threadIdx.x; i < C + 1; i += blockDim.x) red[i] = 0.f;
+  extern __shared__ double red[];     // [C] fp64 sums (see pass 1), then [1] fp32 maximum
+  float* redm = reinterpret_cast<float*>(red + C);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) red[i] = 0.0;
+  if (threadIdx.x == 0) redm[0] = 0.f;
   __syncthreads();
   float gs_scale = 1.f;
   if constexpr (DF == PASE_FMT_F16X2) {
@@ -461,9 +468,9 @@ bn_prelu_bwd_apply_src_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
     }
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, off));
-    if ((threadIdx.x & 31) == 0) atomic_max_pos(&red[C], b);
+    if ((threadIdx.x & 31) == 0) atomic_max_pos(&redm[0], b);
     __syncthreads();
-    gs_scale = f16_grad_scale(red[C] * 1.0001f);
+    gs_scale = f16_grad_scale(redm[0] * 1.0001f);
     if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
       scale_out[0] = 1.f / gs_scale;
       scale_out[1] = gs_scale;
@@ -534,12 +541,12 @@ bn_prelu_bwd_apply_src_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
     }
     if (dbias) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) atomicAdd(&red[c + k], acc[k]);
+      for (int k = 0; k < 4; ++k) atomicAdd(&red[c + k], (double)acc[k]);
     }
   }
   if (dbias) {
     __syncthreads();
-    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, (double)red[i]);
+    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, red[i]);
   }
 }
 
@@ -560,8 +567,8 @@ __global__ void __launch_bounds__(THREADS)
 prelu_bwd_kernel(const float* __restrict__ u, const float* __restrict__ dh,
                  const float* __restrict__ alpha, float* __restrict__ du,
                  double* __restrict__ dalpha, long rows, int C, long ldu, long lddh, long lddu) {
-  extern __shared__ float red[];      // [C]
-  for (int i = threadIdx.x; i < C; i += blockDim.x) red[i] = 0.f;
+  extern __shared__ double red[];     // [C] fp64 sums (order-independent to fp32 precision)
+  for (int i = threadIdx.x; i < C; i += blockDim.x) red[i] = 0.0;
   __syncthreads();
   // thread owns one channel of a strip of rows: coalesced over c
   const int cpb = min(C, (int)blockDim.x);         // channels covered per row pass
@@ -579,10 +586,10 @@ prelu_bwd_kernel(const float* __restrict__ u, const float* __restrict__ dh,
       du[r * lddu + c] = pos ? g : a * g;
       acc += pos ? 0.f : uu * g;
     }
-    atomicAdd(&red[c], acc);
+    atomicAdd(&red[c], (double)acc);
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dalpha + i, (double)red[i]);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dalpha + i, red[i]);
 }
 
 
@@ -590,8 +597,8 @@ prelu_bwd_kernel(const float* __restrict__ u, const float* __restrict__ dh,
 __global__ void __launch_bounds__(THREADS)
 colsum_kernel(const float* __restrict__ X, long ld, long rows, int C, double* __restrict__ acc) {
   pdl_wait();
-  extern __shared__ float red[];      // [C]
-  for (int i = threadIdx.x; i < C; i += blockDim.x) red[i] = 0.f;
+  extern __shared__ double red[];     // [C] fp64 sums (order-independent to fp32 precision)
+  for (int i = threadIdx.x; i < C; i += blockDim.x) red[i] = 0.0;
   __syncthreads();
   const int cpb = min(C, (int)blockDim.x);
   const int rows_per_pass = blockDim.x / cpb;
@@ -610,10 +617,10 @@ colsum_kernel(const float* __restrict__ X, long ld, long rows, int C, double* __
       a3 += X[(r + 3 * step) * ld + c];
     }
     for (; r < rows; r += step) a0 += X[r * ld + c];
-    atomicAdd(&red[c], (a0 + a1) + (a2 + a3));
+    atomicAdd(&red[c], (double)((a0 + a1) + (a2 + a3)));
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(acc + i, (double)red[i]);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(acc + i, red[i]);
 }
 
 __global__ void cast_d2f_kernel(const double* __restrict__ src, float* __restrict__ dst, int n,
@@ -655,10 +662,10 @@ __global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
                                       double* __restrict__ S2) {
   pdl_wait();
   __shared__ float tile[32][33];
-  __shared__ float r1[32], r2[32];
+  __shared__ double r1[32], r2[32];   // fp64: order-independent to fp32 precision
   const int n = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  if (threadIdx.y == 0) { r1[threadIdx.x] = 0.f; r2[threadIdx.x] = 0.f; }
+  if (threadIdx.y == 0) { r1[threadIdx.x] = 0.0; r2[threadIdx.x] = 0.0; }
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const int c = c0 + i, t = t0 + threadIdx.x;
     tile[i][threadIdx.x] = (dout && t < T && c < C) ? dout[((long)n * C + c) * T + t] : 0.f;
@@ -678,12 +685,12 @@ __global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
       a2 += g * xh;
     }
   }
-  atomicAdd(&r1[threadIdx.x], a1);
-  atomicAdd(&r2[threadIdx.x], a2);
+  atomicAdd(&r1[threadIdx.x], (double)a1);
+  atomicAdd(&r2[threadIdx.x], (double)a2);
   __syncthreads();
   if (threadIdx.y == 0 && c < C) {
-    atomicAdd(S1 + c, (double)r1[threadIdx.x]);
-    atomicAdd(S2 + c, (double)r2[threadIdx.x]);
+    atomicAdd(S1 + c, r1[threadIdx.x]);
+    atomicAdd(S2 + c, r2[threadIdx.x]);
   }
 }
 
@@ -898,7 +905,7 @@ int pase_bn_prelu_bwd_reduce(const void* y, int y_bf16, long y_sample_stride, in
     if (gx > cap) gx = cap;
   }
   dim3 grid((unsigned)gx, N);
-  const size_t sm = (3 * C + 2) * sizeof(float);
+  const size_t sm = 3 * C * sizeof(double) + 2 * sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_RED_R(YT, GT, RV)                                                               \
   bn_prelu_bwd_reduce_kernel<YT, GT, RV><<<grid, THREADS, sm, st>>>(                         \
@@ -926,7 +933,7 @@ int pase_bn_prelu_bwd_apply(const void* y, int y_bf16, long y_sample_stride, int
                             void* stream) {
   PASE_CHECK_ARG(y && mean && invstd && S1 && S2 && du && dst,
                  "pase_bn_prelu_bwd_apply: null pointer");
-  PASE_CHECK_ARG(N > 0 && T > 0 && C > 0 && (C % 4) == 0 && C <= 8192,
+  PASE_CHECK_ARG(N > 0 && T > 0 && C > 0 && (C % 4) == 0 && C <= 4096,
                  "pase_bn_prelu_bwd_apply: bad C=%d", C);
   PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2, "pase_bn_prelu_bwd_apply: bad dst_fmt %d", dst_fmt);
   PASE_CHECK_ARG(dst_fmt != PASE_FMT_F16X2 || (dst_lo && amax && scale_out && !y_bf16),
@@ -943,7 +950,7 @@ int pase_bn_prelu_bwd_apply(const void* y, int y_bf16, long y_sample_stride, int
     if (gx > cap) gx = cap;
   }
   dim3 grid((unsigned)gx, N);
-  const size_t sm = (C + 1) * sizeof(float);
+  const size_t sm = C * sizeof(double) + sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_APP_R(YT, DF, RV)                                                                \
   bn_prelu_bwd_apply_kernel<YT, DF, RV><<<grid, THREADS, sm, st>>>(                           \
@@ -973,7 +980,7 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
                                 float* scale_out, void* stream) {
   PASE_CHECK_ARG(y && mean && invstd && scale && shift && alpha && S1 && S2 && srcA && dst,
                  "pase_bn_prelu_bwd_apply_src: null pointer");
-  PASE_CHECK_ARG(N > 0 && T > 0 && C > 0 && (C % 4) == 0 && C <= 8192,
+  PASE_CHECK_ARG(N > 0 && T > 0 && C > 0 && (C % 4) == 0 && C <= 4096,
                  "pase_bn_prelu_bwd_apply_src: bad C=%d", C);
   PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2, "pase_bn_prelu_bwd_apply_src: bad dst_fmt %d",
                  dst_fmt);
@@ -1005,7 +1012,7 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
     if (gx > cap) gx = cap;
   }
   dim3 grid((unsigned)gx, N);
-  const size_t sm = (C + 1) * sizeof(float);
+  const size_t sm = C * sizeof(double) + sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_APS_R(YT, GT, DF, RV)                                                             \
   bn_prelu_bwd_apply_src_kernel<YT, GT, DF, RV><<<grid, THREADS, sm, st>>>(                    \
@@ -1037,14 +1044,14 @@ int pase_prelu_fwd(const float* u, float* h, const float* alpha, long rows, int 
 
 int pase_prelu_bwd(const float* u, const float* dh, const float* alpha, float* du, double* dalpha,
                    long rows, int C, long ldu, long lddh, long lddu, void* stream) {
-  PASE_CHECK_ARG(u && dh && alpha && du && dalpha && rows > 0 && C > 0 && C <= 8192,
+  PASE_CHECK_ARG(u && dh && alpha && du && dalpha && rows > 0 && C > 0 && C <= 6144,
                  "pase_prelu_bwd: bad args");
   const int cpb = C < THREADS ? C : THREADS;
   const int rpp = THREADS / cpb;
   long nb = (rows + rpp - 1) / rpp;
   long cap = (long)pase_num_sms() * 4;
   if (nb > cap) nb = cap;
-  prelu_bwd_kernel<<<(unsigned)nb, THREADS, C * sizeof(float), (cudaStream_t)stream>>>(
+  prelu_bwd_kernel<<<(unsigned)nb, THREADS, C * sizeof(double), (cudaStream_t)stream>>>(
       u, dh, alpha, du, dalpha, rows, C, ldu, lddh, lddu);
   PASE_LAUNCH_CHECK("pase_prelu_bwd");
   return PASE_OK;
@@ -1066,7 +1073,7 @@ int pase_colsum(const float* X, long ld, long rows, int C, double* acc, void* st
     long cap = (long)pase_num_sms() * per_sm;
     if (nb > cap) nb = cap;
     if (nb < 1) nb = 1;
-    PASE_LAUNCH((colsum_kernel), (unsigned)nb, THREADS, Cp * sizeof(float), (cudaStream_t)stream, 
+    PASE_LAUNCH((colsum_kernel), (unsigned)nb, THREADS, Cp * sizeof(double), (cudaStream_t)stream, 
         X + c0, ld, rows, Cp, acc + c0);
     PASE_LAUNCH_CHECK("pase_colsum");
   }

@@ -97,13 +97,16 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr int STAGE_BYTES = TILE_ELEMS * (sizeof(YT) + sizeof(GT));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  float* red = reinterpret_cast<float*>(bars + STAGES);       // [3C + 2] or [C + 1]
+  // block sums in fp64 ([3C] or [C]): the order of the threads' additions then only moves
+  // bits below fp32 precision (run-to-run identical statistics); maxima ([2] or [1]) in fp32
+  double* red = reinterpret_cast<double*>(bars + STAGES);
   const int C = a.C, C4 = C >> 2, T = a.T;
+  float* redm = reinterpret_cast<float*>(red + (APPLY ? C : 3 * C));
   const int tid = threadIdx.x;
   const int q = tid % C4, r0 = tid / C4, rstep = THREADS / C4;
   const int c = q * 4;
-  const int nred = APPLY ? C + 1 : 3 * C + 2;
-  for (int i = tid; i < nred; i += THREADS) red[i] = 0.f;
+  for (int i = tid; i < (APPLY ? C : 3 * C); i += THREADS) red[i] = 0.0;
+  if (tid < 2) redm[tid] = 0.f;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) bar_init(&bars[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -130,9 +133,9 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
     }
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, off));
-    if ((tid & 31) == 0) atomic_max_pos(&red[C], b);
+    if ((tid & 31) == 0) atomic_max_pos(&redm[0], b);
     __syncthreads();
-    gs_scale = f16_grad_scale(red[C] * 1.0001f);
+    gs_scale = f16_grad_scale(redm[0] * 1.0001f);
     if (blockIdx.x == 0 && tid == 0) {
       a.scale_out[0] = 1.f / gs_scale;
       a.scale_out[1] = gs_scale;
@@ -283,15 +286,15 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
   if constexpr (APPLY) {
     if (a.dbias == nullptr) return;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) atomicAdd(&red[c + k], a1[k]);
+    for (int k = 0; k < 4; ++k) atomicAdd(&red[c + k], (double)a1[k]);
     __syncthreads();
-    for (int i = tid; i < C; i += THREADS) atomicAdd(a.dbias + i, (double)red[i]);
+    for (int i = tid; i < C; i += THREADS) atomicAdd(a.dbias + i, red[i]);
   } else {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      atomicAdd(&red[0 * C + c + k], a1[k]);
-      atomicAdd(&red[1 * C + c + k], a2[k]);
-      atomicAdd(&red[2 * C + c + k], a3[k]);
+      atomicAdd(&red[0 * C + c + k], (double)a1[k]);
+      atomicAdd(&red[1 * C + c + k], (double)a2[k]);
+      atomicAdd(&red[2 * C + c + k], (double)a3[k]);
     }
     if (a.amax != nullptr) {
 #pragma unroll
@@ -300,19 +303,19 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
         mx_xh = fmaxf(mx_xh, __shfl_xor_sync(0xffffffffu, mx_xh, off));
       }
       if ((tid & 31) == 0) {
-        atomic_max_pos(&red[3 * C], mx_du);
-        atomic_max_pos(&red[3 * C + 1], mx_xh);
+        atomic_max_pos(&redm[0], mx_du);
+        atomic_max_pos(&redm[1], mx_xh);
       }
     }
     __syncthreads();
     for (int i = tid; i < C; i += THREADS) {
-      atomicAdd(a.S1 + i, (double)red[0 * C + i]);
-      atomicAdd(a.S2 + i, (double)red[1 * C + i]);
-      atomicAdd(a.dalpha + i, (double)red[2 * C + i]);
+      atomicAdd(a.S1 + i, red[0 * C + i]);
+      atomicAdd(a.S2 + i, red[1 * C + i]);
+      atomicAdd(a.dalpha + i, red[2 * C + i]);
     }
     if (a.amax != nullptr && tid == 0) {
-      atomic_max_pos(a.amax, red[3 * C]);
-      atomic_max_pos(a.amax + 1, red[3 * C + 1]);
+      atomic_max_pos(a.amax, redm[0]);
+      atomic_max_pos(a.amax + 1, redm[1]);
     }
   }
 }
@@ -324,12 +327,13 @@ int launch_cfg(const BnStreamArgs& a, cudaStream_t st) {
   g.tps = (a.T + g.TT - 1) / g.TT;
   g.total = (long)a.N * g.tps;
   const size_t smem = (size_t)TC::NS * TC::TE * (sizeof(YT) + sizeof(GT)) +
-                      TC::NS * sizeof(uint64_t) + (size_t)(3 * a.C + 2) * sizeof(float);
+                      TC::NS * sizeof(uint64_t) + (size_t)3 * a.C * sizeof(double) +
+                      2 * sizeof(float);
   auto kern = bn_bwd_stream_kernel<YT, GT, DF, APPLY, TC>;
   static bool attr_done = false;
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(TC::NS * TC::TE * 8 + 64 + (3 * 1024 + 2) * 4));
+                                         (int)(TC::NS * TC::TE * 8 + 64 + 3 * 1024 * 8 + 8));
     if (e != cudaSuccess) {
       pase_set_error("bn_stream: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
       return (int)e;

@@ -1,4 +1,4 @@
-// Shared helpers for the pase_b200 CUDA library (sm_100a).
+// Shared helpers for the pase_b200 CUDA library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -34,7 +34,7 @@ static inline int pase_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -45,10 +45,9 @@ static inline int pase_num_sms() {
 // distribution and the kernel's own prologue overlap the predecessor's tail.  Contract: such a
 // kernel executes pdl_wait() before its first access to global memory (the wait returns once
 // every prerequisite grid has completed and flushed).
-// MEASURED (profiles/r02_history.md): inside the CUDA-graph replay of the encoder step the
-// attribute buys nothing (3.255 vs 3.258 ms with the implicit trigger at block exit) and the
-// early trigger below costs 1.5 % (the dependents' resident, waiting blocks get in the way of
-// the running kernel), so it is OFF unless PASE_B200_PDL=1; with the attribute off pdl_wait()
+// Inside the CUDA-graph replay of the encoder step the attribute hides little launch latency,
+// and the early trigger below lets the dependents' resident, waiting blocks get in the way of
+// the running kernel, so it is OFF unless PASE_B200_PDL=1; with the attribute off pdl_wait()
 // is a no-op.
 static inline bool pase_pdl_enabled() {
   static int v = -1;

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA implicit-GEMM kernels for sm_100a.
+// wgmma / TMA implicit-GEMM kernels for sm_90a.
 //
 //   pase_tc_gemm_nt : C[map(m), n] = alpha * sum_k A[m, k] * B[n, k] + bias[n]
 //       A is addressed through a plain (non-overlapping) 2-D tensor [a_rows x R]:
@@ -6,25 +6,27 @@
 //       matrix of a strided convolution (R = stride * Cin) needs no materialisation
 //       and no overlapping TMA strides.  B is [N x K], K-major.
 //   pase_tc_gemm_tn : C[i, j] += alpha * sum_r A[r, i] * B[r, j]   (weight gradients)
-//       both operands MN-major in shared memory (transpose bits set in the UMMA
-//       instruction descriptor); split over the reduction, fp32 red.add epilogue.
+//       both operands MN-major in global memory; split over the reduction, the splits'
+//       partial tiles summed in a fixed order (run-to-run identical results).  16-bit
+//       operands are read MN-major by wgmma (transpose bits); tf32 wgmma only reads K-major
+//       shared memory, so fp32 tiles are transposed in shared memory first.
 //
-// Numerics (`mode`), fp32 accumulation in TMEM in every mode:
-//   0  TF32    kind::tf32, fp32 operands read as tf32 (10-bit mantissa);
+// Numerics (`mode`), fp32 accumulation in registers in every mode:
+//   0  TF32    .tf32 wgmma, fp32 operands read as tf32 (10-bit mantissa);
 //   1  3xTF32  error-compensated: operands pre-split into exactly representable tf32 "hi"
 //              and "lo" parts, D = Ahi*Bhi + Alo*Bhi + Ahi*Blo -> fp32-equivalent products;
-//   2  BF16    kind::f16 with bf16 operands (one pass at twice the TF32 rate, half the bytes);
+//   2  BF16    .bf16 wgmma (one pass at twice the TF32 rate, half the bytes);
 //   3  3xF16   error-compensated fp16: x = hi + 2^-11 lo', hi = rn_f16(x),
 //              lo' = rn_f16((x - hi) 2^11) (both 11-bit significands -> 22-bit products like
 //              3xTF32, at half the tensor time and half the operand bytes).  The scaled
-//              correction products go to a SECOND TMEM accumulator:
+//              correction products go to a SECOND register accumulator:
 //              D = [Ahi*Bhi] + 2^-11 [Alo'*Bhi + Ahi*Blo'].  Operands must fit fp16's range
 //              (gradients are pre-scaled by a power of two; `alpha_dev` undoes it).
 //
-// Warp roles (576 threads): warps 0-15 = 16 epilogue warps, warp 16 = TMA producer, warp 17 =
-// TMEM owner + MMA issuer (one elected lane).  Epilogue: tcgen05.ld -> fp32 register sums -> bias /
-// row map / BatchNorm column statistics -> staged coalesced stores).  K-major tiles are
-// 128-byte rows with the 128B swizzle; two TMEM accumulator buffers per CTA.
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues), warpgroups 1 and 2
+// = consumers; consumer warpgroup w issues the m64 wgmmas of tile rows [64 (w-1), +64) and runs
+// their epilogue straight from the accumulator registers.  Operand tiles are 128-byte rows with
+// the 128B swizzle.
 #include "common.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -40,13 +42,10 @@ constexpr float F16_LO_SCALE = 1.0f / 2048.0f;       // 2^-11, see pase_split_f1
 template <int MODE>
 struct ModeT {
   static constexpr int ESZ = MODE >= 2 ? 2 : 4;            // operand element size
-  static constexpr bool K16 = MODE >= 2;                   // kind::f16 (else kind::tf32)
   static constexpr bool SPLIT = (MODE == 1 || MODE == 3);  // hi/lo operands, 3 MMAs / product
-  static constexpr int NACC = MODE == 3 ? 2 : 1;           // TMEM accumulators per buffer
-  static constexpr int UMMA_K = 32 / ESZ;                  // 8 (tf32) / 16 (bf16, f16)
+  static constexpr int NACC = MODE == 3 ? 2 : 1;           // register accumulators
   static constexpr int EB = 128 / ESZ;                     // elements per 128-byte row
-  // operand format of the instruction descriptor: kind::tf32 -> 2; kind::f16: f16 0, bf16 1
-  static constexpr uint32_t FMT = MODE <= 1 ? 2u : (MODE == 2 ? 1u : 0u);
+  static constexpr int KIND = MODE <= 1 ? 0 : (MODE == 2 ? 1 : 2);   // tf32 / bf16 / f16
 };
 
 // ------------------------------------------------------------------ PTX helpers ----
@@ -60,6 +59,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
                "r"(bytes)
                : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -112,408 +114,188 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
 __device__ __forceinline__ void tmap_prefetch(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// the producer warpgroup hands registers to the two consumer warpgroups (40 + 2 x 232 per
+// thread x 128 threads <= 64 K): the 3xF16 consumer holds three 64-register accumulators
+__device__ __forceinline__ void regs_producer() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+__device__ __forceinline__ void regs_consumer() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(slot)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// the 256 consumer threads only
+__device__ __forceinline__ void consumer_sync() {
+  asm volatile("bar.sync 1, 256;" ::: "memory");
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-// Warp-convergent MMA issue: every lane of the MMA warp executes the surrounding loop and
-// one elected lane issues.  Keeping the warp converged lets ptxas hold descriptors and TMEM
-// addresses in uniform registers; under `if (lane == 0)` every UTCHMMA is preceded by an
-// ELECT / R2UR.BROADCAST / BRA.U.ANY sequence and the issue thread, not the tensor pipe,
-// bounds the MMA rate (profiles/r01_history.md).
-//   K16: kind::f16 (bf16 / fp16 operands, format in the instruction descriptor), else
-//   kind::tf32.  CG: cta_group (2 = CTA pair, M = 256, issued by the leader only).
-template <bool K16, int CG>
-__device__ __forceinline__ void umma_w(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                       uint32_t idesc, uint32_t accumulate) {
-  if constexpr (!K16 && CG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p, e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@e tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else if constexpr (!K16 && CG == 2) {
-    asm volatile(
-        "{\n\t.reg .pred p, e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@e tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else if constexpr (K16 && CG == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p, e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p, e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@e tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void umma_commit_w(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// ---- CTA-pair (cta_group::2) helpers --------------------------------------------------
-// Two CTAs of a cluster (same TPC) execute ONE tcgen05.mma of M = 256: each holds its own 128
-// rows of A and one half of B's N rows; the leader (cluster rank 0) issues, accumulators land
-// in both CTAs' TMEM.  Operand bytes read from shared memory per flop drop by 25 % (N = 128)
-// against cta_group::1 -- the limiter of the 1-CTA kernel (profiles/r01_history.md).
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local` (an address in this CTA's window) in CTA `rank`
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// 2-SM TMA load: data lands in the executing CTA's shared memory, the transaction bytes are
-// signalled on the mbarrier at `bar_cluster_addr` (the leader CTA's barrier)
-__device__ __forceinline__ void tma2_load_2d(void* dst, const CUtensorMap* map,
-                                             uint32_t bar_cluster_addr, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      ".L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1),
-      "l"(0x1000000000000000ull)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* dst, const CUtensorMap* map,
-                                             uint32_t bar_cluster_addr, int c0, int c1, int c2,
-                                             int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      ".L2::cache_hint [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3), "l"(0x1000000000000000ull)
-      : "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc2(uint32_t* slot) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(slot)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-// commit of all prior MMAs of this thread; arrives on the barrier at the same CTA-relative
-// offset in both CTAs of the pair
-__device__ __forceinline__ void umma2_commit_mc_w(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t.reg .b16 m;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "mov.b16 m, 3;\n\t"
-      "@e tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], m;\n\t}" ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// this warp no longer reads the pipeline stage guarded by `bar` (8 arrivals free it)
+__device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar);
 }
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout).
+// ---- wgmma --------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90 GMMA descriptor): start address, leading and stride
+// byte offsets (all >> 4), layout type 1 = 128B swizzle at bits 62-63.
 //   K-major : rows of 128 B, 8-row atoms of 1024 B -> SBO = 1024 B, LBO unused.
-//   MN-major: 128 B along MN per row, 8 k-rows per 1024 B atom; SBO = 1024 B (next 8 k),
-//             LBO = byte distance between consecutive 128-byte MN blocks.
-//   MN-major fp32/tf32 operands must use the 32-byte-base 128B swizzle (layout type 1,
-//   TMA CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B): atoms of 128 B (MN) x 4 k-rows, SBO = 512 B;
-//   16-bit MN-major operands use the plain 128B swizzle (layout type 2).
-template <int LAYOUT = 2>
+//   MN-major: 128 B (64 16-bit elements) along MN per k-row, 8 k-rows per 1024 B atom:
+//             SBO = 1024 B (next 8 k), LBO = byte distance between 64-element MN blocks.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes,
                                               uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;                      // descriptor version (Blackwell)
-  d |= (uint64_t)LAYOUT << 61;                 // 2 = SWIZZLE_128B, 1 = SWIZZLE_128B_BASE32B
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor bit layout): D = f32 (bit 4), A / B
-// format at bits 7 / 10, transpose bits 15 / 16, N >> 3 at 17, M >> 4 at 24
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn, int b_mn,
-                                                  uint32_t fmt) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_wait0() {
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+// keeps the compiler from touching accumulator registers across the asynchronous wgmma
+template <int NR>
+__device__ __forceinline__ void fence_regs(float (&d)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+template <int K>
+struct KindTag {};
+
+// accumulator register list / operand constraints, then the numbers of the operands after
+// them (descriptors, scale-d, transpose immediates), per accumulator size
+#define PASE_D32 \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, " \
+  "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define PASE_O32 \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), \
+  "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), \
+  "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), \
+  "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), \
+  "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define PASE_AB32 "%32, %33, p, 1, 1"
+#define PASE_SC32 "%34"
+#define PASE_TR32 ", %35, %36"
+#define PASE_D64 \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, " \
+  "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, " \
+  "%34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, " \
+  "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define PASE_O64 \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), \
+  "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), \
+  "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), \
+  "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), \
+  "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), \
+  "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), \
+  "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), \
+  "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+  "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), \
+  "+f"(d[63])
+#define PASE_AB64 "%64, %65, p, 1, 1"
+#define PASE_SC64 "%66"
+#define PASE_TR64 ", %67, %68"
+// m64nNk{8,16} wgmma with fp32 accumulators d (N/2 registers per thread); scale_d = 0
+// overwrites d.  TA / TB: operand MN-major (16-bit kinds only).
+#define PASE_WGMMA(NR, KIND, INSTR, TRANS, ...)                                              \
+  template <int TA, int TB>                                                                 \
+  __device__ __forceinline__ void wgmma_call(float (&d)[NR], uint64_t da, uint64_t db,      \
+                                             uint32_t scale_d, KindTag<KIND>) {             \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " PASE_SC##NR ", 0;\n\t" INSTR " "     \
+                 PASE_D##NR ", " PASE_AB##NR TRANS ";\n\t}"                                   \
+                 : PASE_O##NR                                                                \
+                 : "l"(da), "l"(db), "r"(scale_d) __VA_ARGS__);                              \
+  }
+PASE_WGMMA(32, 0, "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32", "", )
+PASE_WGMMA(32, 1, "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16", PASE_TR32, , "n"(TA), "n"(TB))
+PASE_WGMMA(32, 2, "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16", PASE_TR32, , "n"(TA), "n"(TB))
+PASE_WGMMA(64, 0, "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32", "", )
+PASE_WGMMA(64, 1, "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16", PASE_TR64, , "n"(TA), "n"(TB))
+PASE_WGMMA(64, 2, "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16", PASE_TR64, , "n"(TA), "n"(TB))
+// The wgmmas of one 128-byte k-block: 4 k-steps of 32 B (+2 in the descriptor address when
+// K-major, +kstep_desc in general).
+//   plain : D += A*B;   3xTF32: D += Al*Bh + Ah*Bl + Ah*Bh (one accumulator);
+//   3xF16 : Dc += Al'*Bh + Ah*Bl',  D += Ah*Bh.
+template <int MODE, int TR, int NR, int NC>
+__device__ __forceinline__ void issue_kblock(float (&acc)[NR], float (&corr)[NC], uint64_t dah,
+                                             uint64_t dbh, uint64_t dal, uint64_t dbl,
+                                             uint32_t kstep_desc, bool first) {
+  using MT = ModeT<MODE>;
+  constexpr KindTag<MT::KIND> kt{};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t sc = (first && k == 0) ? 0u : 1u;
+    const uint64_t o = (uint64_t)(k * kstep_desc);
+    if constexpr (MODE == 1) {
+      wgmma_call<TR, TR>(acc, dal + o, dbh + o, sc, kt);
+      wgmma_call<TR, TR>(acc, dah + o, dbl + o, 1u, kt);
+      wgmma_call<TR, TR>(acc, dah + o, dbh + o, 1u, kt);
+    } else if constexpr (MODE == 3) {
+      wgmma_call<TR, TR>(corr, dal + o, dbh + o, sc, kt);
+      wgmma_call<TR, TR>(corr, dah + o, dbl + o, 1u, kt);
+      wgmma_call<TR, TR>(acc, dah + o, dbh + o, sc, kt);
+    } else {
+      wgmma_call<TR, TR>(acc, dah + o, dbh + o, sc, kt);
+    }
+  }
+}
+
+// Fold the finished accumulator(s) of one k-chunk into fp32 register sums with round-to-nearest
+// adds: the split modes flush every K = 128, so rounding inside the tensor core's accumulation
+// cannot drift over long reductions.
+template <int MODE, int NR, int NC>
+__device__ __forceinline__ void fold_chunk(float (&sums)[NR], const float (&acc)[NR],
+                                           const float (&corr)[NC], bool first) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    float v = first ? acc[i] : sums[i] + acc[i];
+    if constexpr (MODE == 3) v = fmaf(corr[i], F16_LO_SCALE, v);
+    sums[i] = v;
+  }
 }
 
 struct RowMap {
   int rows_in, t_valid, rows_out, fold, cols_per_fold;
 };
 
-// transposed butterfly: v[j] per lane (lane = row) -> lane j holds sum over lanes of v[j]
-__device__ __forceinline__ float colsum32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float keep = up ? v[i + off] : v[i];
-      const float send = up ? v[i] : v[i + off];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
-  return v[0];
-}
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// Thread layout shared by all kernels: warps 0..15 = 16 epilogue warps, warp 16 = TMA
-// producer, warp 17 = TMEM owner + MMA issuer.  Epilogue warp w reads TMEM lanes 32*(w%4)..
-// (hardware restriction) and owns column chunk w/4 of the tile, so every warp folds / stores
-// only 32 columns: short per-warp instruction streams, 4 warps per scheduler.
-// The MMA warp has the HIGHEST warp id of its scheduler (17 > 13, 9, 5, 1): the warp
-// arbiter serves the highest eligible warp id first, and the issue loop needs ~15 SASS
-// instructions per tcgen05.mma (profiles/r02_sass.md) against 64 clk of tensor time -- as warp 1
-// it queued behind four busy epilogue warps (tensor pipe 30 % on the epilogue-heavy sinc layer).
-constexpr int N_EPI_WARPS = 16;
-constexpr int WARP_TMA = 16;
-constexpr int WARP_MMA = 17;
-constexpr int NTHREADS_V3 = (2 + N_EPI_WARPS) * 32;
-constexpr int OUT_STG_FLOATS = 32 * 8;                                // 32 rows x 8 cols per pass
-constexpr int OUT_STAGE_BYTES = N_EPI_WARPS * OUT_STG_FLOATS * 4;     // 16 KB
+constexpr int NTHREADS = 384;
 constexpr int SMEM_LIMIT = 232448;                                    // 227 KB opt-in maximum
 constexpr int BAR_BYTES = 256;
 constexpr int MAX_STAGES = 8;
 
-inline int pick_stages(int stage_bytes, int stat_bytes) {
-  int st = (SMEM_LIMIT - 1024 - BAR_BYTES - OUT_STAGE_BYTES - stat_bytes) / stage_bytes;
+inline int pick_stages(int stage_bytes, int extra_bytes) {
+  int st = (SMEM_LIMIT - 1024 - BAR_BYTES - extra_bytes) / stage_bytes;
   return st > MAX_STAGES ? MAX_STAGES : st;
 }
-inline int smem_bytes(int stages, int stage_bytes, int stat_bytes) {
-  return stages * stage_bytes + 1024 + BAR_BYTES + OUT_STAGE_BYTES + stat_bytes;
-}
-
-// Coalesced store of one warp's 32 rows x 32 columns (v[j] = column j of this lane's row).
-// Four passes of 8 columns through a 1 KB swizzled staging tile; after the transpose a
-// lane owns 16 B of a row and 2 lanes cover a full 32 B sector.  `nlim` = first invalid
-// column of this lane's row (0 for rows that must not be written).
-template <bool RED>
-__device__ __forceinline__ void store_chunk(float* stg, const float (&v)[32], int lane,
-                                            float* __restrict__ C, long ldc, long orow, int nlim,
-                                            int nb, bool vec_ok, int accumulate) {
-  const int sw = (lane >> 2) & 1;
-#pragma unroll
-  for (int pass = 0; pass < 4; ++pass) {
-    *reinterpret_cast<float4*>(&stg[lane * 8 + 4 * (0 ^ sw)]) =
-        make_float4(v[pass * 8 + 0], v[pass * 8 + 1], v[pass * 8 + 2], v[pass * 8 + 3]);
-    *reinterpret_cast<float4*>(&stg[lane * 8 + 4 * (1 ^ sw)]) =
-        make_float4(v[pass * 8 + 4], v[pass * 8 + 5], v[pass * 8 + 6], v[pass * 8 + 7]);
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 2; ++it) {
-      const int r = it * 16 + (lane >> 1), h = lane & 1;
-      const float4 val =
-          *reinterpret_cast<const float4*>(&stg[r * 8 + 4 * (h ^ ((r >> 2) & 1))]);
-      const long orow_r = __shfl_sync(0xffffffffu, orow, r);
-      const int nlim_r = __shfl_sync(0xffffffffu, nlim, r);
-      const int n = nb + pass * 8 + h * 4;
-      float* cp = C + orow_r * ldc + n;
-      float x[4] = {val.x, val.y, val.z, val.w};
-      if (n + 3 < nlim_r && vec_ok) {
-        if (RED) {
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(cp), "f"(x[0]),
-                       "f"(x[1]), "f"(x[2]), "f"(x[3])
-                       : "memory");
-        } else {
-          if (accumulate) {
-            const float4 o = *reinterpret_cast<const float4*>(cp);
-            x[0] += o.x; x[1] += o.y; x[2] += o.z; x[3] += o.w;
-          }
-          *reinterpret_cast<float4*>(cp) = make_float4(x[0], x[1], x[2], x[3]);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (n + j < nlim_r) {
-            if (RED) atomicAdd(cp + j, x[j]);
-            else cp[j] = accumulate ? cp[j] + x[j] : x[j];
-          }
-      }
-    }
-    __syncwarp();
-  }
+inline int smem_bytes(int stages, int stage_bytes, int extra_bytes) {
+  return stages * stage_bytes + 1024 + BAR_BYTES + extra_bytes;
 }
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
 }
-
-// 16-bit output (bf16 values, or the fp16 halves of a pair): the same transpose with rows of 16
-// elements (32 B) -- two passes of 16 columns; after the transpose a lane owns 16 B (8 columns)
-// of a row, 2 lanes cover a 32 B sector.  pk[i] = columns 2i, 2i+1 of this lane's row.
-__device__ __forceinline__ void store_chunk_16(float* stg_f, const uint32_t (&pk)[16], int lane,
-                                               uint16_t* __restrict__ C, long ldc, long orow,
-                                               int nlim, int nb, bool vec_ok) {
-  uint4* stg = reinterpret_cast<uint4*>(stg_f);          // 64 chunks of 16 B
-  const int sw = (lane >> 2) & 1;
-#pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
-    const int c = pass * 8;
-    stg[lane * 2 + (0 ^ sw)] = make_uint4(pk[c + 0], pk[c + 1], pk[c + 2], pk[c + 3]);
-    stg[lane * 2 + (1 ^ sw)] = make_uint4(pk[c + 4], pk[c + 5], pk[c + 6], pk[c + 7]);
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 2; ++it) {
-      const int r = it * 16 + (lane >> 1), h = lane & 1;
-      const uint4 val = stg[r * 2 + (h ^ ((r >> 2) & 1))];
-      const long orow_r = __shfl_sync(0xffffffffu, orow, r);
-      const int nlim_r = __shfl_sync(0xffffffffu, nlim, r);
-      const int n = nb + pass * 16 + h * 8;
-      uint16_t* cp = C + orow_r * ldc + n;
-      if (n + 7 < nlim_r && vec_ok) {
-        *reinterpret_cast<uint4*>(cp) = val;
-      } else {
-        const uint32_t w[4] = {val.x, val.y, val.z, val.w};
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (n + j < nlim_r) cp[j] = (uint16_t)(w[j >> 1] >> ((j & 1) * 16));
-      }
-    }
-    __syncwarp();
-  }
+__device__ __forceinline__ uint32_t pack_f16(__half a, __half b) {
+  return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
+}
+// sum over the 8 lanes that share lane % 4 (the 8 accumulator rows g of a warp's m16 slice)
+__device__ __forceinline__ float rowgroup_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  v += __shfl_xor_sync(0xffffffffu, v, 16);
+  return v;
 }
 
-__device__ __forceinline__ void store_chunk_bf16(float* stg_f, const float (&v)[32], int lane,
-                                                 __nv_bfloat16* __restrict__ C, long ldc,
-                                                 long orow, int nlim, int nb, bool vec_ok) {
-  uint32_t pk[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) pk[i] = pack_bf16(v[2 * i], v[2 * i + 1]);
-  store_chunk_16(stg_f, pk, lane, reinterpret_cast<uint16_t*>(C), ldc, orow, nlim, nb, vec_ok);
-}
-
-// one 64-bit shared-memory descriptor = constant bits | (address >> 4)
-template <int LAYOUT>
-__device__ __forceinline__ uint64_t desc_hi_bits(uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return make_desc<LAYOUT>(0, lbo_bytes, sbo_bytes);
-}
-
-// ROWB = bytes per k-block row: 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B; used with BN = 256 so
-// that four pipeline stages still fit in shared memory).
-// Why BN = 256: a 128xNx(32 B) UMMA reads (128 + N) * 32 B of shared memory in N/2 clocks --
-// 128 B/clk at N = 128, i.e. the whole shared-memory bandwidth of the SM before the TMA fills
-// are even counted (measured tensor-pipe activity ~58 %); N = 256 needs 96 B/clk.
-template <int BN, int MODE, int ROWB>
-struct NTCfg {
-  using MT = ModeT<MODE>;
-  static constexpr int BK = ROWB / MT::ESZ;                // elements per k-block
-  static constexpr int A_BYTES = BM * ROWB;
-  static constexpr int B_BYTES = BN * ROWB;
-  static constexpr int STAGE_BYTES = (MT::SPLIT ? 2 : 1) * (A_BYTES + B_BYTES);
-  static constexpr int ACC_COLS = MT::NACC * BN;           // TMEM columns of one buffer
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;           // two accumulator buffers
-  static constexpr int CPW = (BN / 32 + 3) / 4;            // 32-column chunks per epilogue warp
-  static constexpr int EPI_ACTIVE = BN >= 128 ? 16 : 4 * (BN / 32);
-  static constexpr int LAYOUT = ROWB == 128 ? 2 : 4;       // SWIZZLE_128B : SWIZZLE_64B
-  static constexpr int SBO = 8 * ROWB;                     // 8-row core-matrix group
-  static constexpr int KSTEPS = ROWB / 32;                 // UMMA k-steps (32 B each) per block
-  static_assert(TMEM_COLS <= 512, "TMEM budget");
+// Accumulator layout of m64nN (per warp: 16 rows): v[4j + 2h + e] = row g + 8h, column
+// 8j + 2 t4 + e, with g = lane / 4, t4 = lane % 4.
+struct Frag {
+  int m[2];        // the two absolute rows of this thread
+  int n0, t4, g;   // first column of the tile, lane % 4, lane / 4
 };
-
-// The MMAs of one k-block (all lanes converged; elected issue inside umma_w).
-//   plain : D += A*B;   3xTF32: D += Al*Bh + Ah*Bl + Ah*Bh (one accumulator);
-//   3xF16 : Dc (+BN columns) += Al'*Bh + Ah*Bl',  D += Ah*Bh.
-template <int MODE, int CG, int KSTEPS, int KSTEP_DESC>
-__device__ __forceinline__ void issue_kblock(uint32_t d_tmem, uint32_t corr_off, uint64_t dah,
-                                             uint64_t dbh, uint64_t dal, uint64_t dbl,
-                                             uint32_t idesc, uint32_t first) {
-  using MT = ModeT<MODE>;
-#pragma unroll
-  for (int k = 0; k < KSTEPS; ++k) {
-    const uint32_t acc = (k == 0) ? first : 1u;
-    const uint64_t o = (uint64_t)(k * KSTEP_DESC);
-    if constexpr (MODE == 1) {
-      umma_w<MT::K16, CG>(d_tmem, dal + o, dbh + o, idesc, acc);
-      umma_w<MT::K16, CG>(d_tmem, dah + o, dbl + o, idesc, 1);
-      umma_w<MT::K16, CG>(d_tmem, dah + o, dbh + o, idesc, 1);
-    } else if constexpr (MODE == 3) {
-      umma_w<MT::K16, CG>(d_tmem + corr_off, dal + o, dbh + o, idesc, acc);
-      umma_w<MT::K16, CG>(d_tmem + corr_off, dah + o, dbl + o, idesc, 1);
-      umma_w<MT::K16, CG>(d_tmem, dah + o, dbh + o, idesc, acc);
-    } else {
-      umma_w<MT::K16, CG>(d_tmem, dah + o, dbh + o, idesc, acc);
-    }
-  }
-}
-
-// Epilogue: fold one finished TMEM buffer (32 columns at `taddr`) into fp32 register sums.
-template <int MODE>
-__device__ __forceinline__ void fold_chunk(uint32_t taddr, uint32_t corr_off, float (&sums)[32],
-                                           bool first) {
-  uint32_t raw[32];
-  tmem_ld32(taddr, raw);
-  if (first) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) sums[j] = __uint_as_float(raw[j]);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) sums[j] += __uint_as_float(raw[j]);
-  }
-  if constexpr (MODE == 3) {          // scaled correction accumulator
-    tmem_ld32(taddr + corr_off, raw);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) sums[j] = fmaf(__uint_as_float(raw[j]), F16_LO_SCALE, sums[j]);
-  }
-}
 
 struct NTArgs {
   int R;
@@ -527,7 +309,7 @@ struct NTArgs {
   double* colsum;
   double* colsumsq;
   int accumulate, flush_kb, stages, stat_cols;
-  // contextualised-MSE epilogue (fused regression head, tc_gemm_nt2_kernel<.., CTX = true>):
+  // contextualised-MSE epilogue (fused regression head, tc_gemm_nt_kernel<.., CTX = true>):
   // C / cx_lo receive the fp16 pair of s * (prediction - label window) instead of the
   // prediction; cx_loss += sum d^2; cx_db[n] += sum_rows d
   const float* cx_label;           // (B, F, T) fp32
@@ -538,136 +320,178 @@ struct NTArgs {
   double* cx_db;
 };
 
+// Output stage of the NT kernel: alpha / bias, row map and validity, store (fp32 or bf16),
+// BatchNorm column statistics of the fp32 values (into shared-memory column sums).
+template <int NR, bool OUT16>
+__device__ __forceinline__ void nt_output(float (&v)[NR], const NTArgs& a, float alpha,
+                                          const Frag& f, double* s_stats) {
+  const int N = a.N;
+  long orow[2];
+  int nlim[2];                             // columns [0, nlim) of the row are valid
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = f.m[h];
+    orow[h] = 0;
+    nlim[h] = 0;
+    if (m < a.M) {
+      const int g = m / a.rm.rows_in;
+      const int u = m - g * a.rm.rows_in;
+      orow[h] = (long)g * a.rm.rows_out + u;
+      const long lim = (long)(a.rm.t_valid - u * a.rm.fold) * a.rm.cols_per_fold;
+      nlim[h] = lim <= 0 ? 0 : (lim >= N ? N : (int)lim);
+    }
+  }
+  const bool want_stats = a.colsum != nullptr;
+  const bool vec_ok = ((a.ldc & 1) == 0) &&
+                      ((reinterpret_cast<uintptr_t>(a.C) & (OUT16 ? 3u : 7u)) == 0);
+#pragma unroll
+  for (int j = 0; j < NR / 4; ++j) {
+    const int n = f.n0 + 8 * j + 2 * f.t4;
+    const float b0 = (a.bias != nullptr && n < N) ? __ldg(a.bias + n) : 0.f;
+    const float b1 = (a.bias != nullptr && n + 1 < N) ? __ldg(a.bias + n + 1) : 0.f;
+    float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float x0 = fmaf(v[4 * j + 2 * h], alpha, b0);
+      const float x1 = fmaf(v[4 * j + 2 * h + 1], alpha, b1);
+      if constexpr (OUT16) {
+        __nv_bfloat16* cp = reinterpret_cast<__nv_bfloat16*>(a.C) + orow[h] * a.ldc + n;
+        if (n + 1 < nlim[h] && vec_ok) {
+          *reinterpret_cast<uint32_t*>(cp) = pack_bf16(x0, x1);
+        } else {
+          if (n < nlim[h]) cp[0] = __float2bfloat16_rn(x0);
+          if (n + 1 < nlim[h]) cp[1] = __float2bfloat16_rn(x1);
+        }
+      } else {
+        float* cp = reinterpret_cast<float*>(a.C) + orow[h] * a.ldc + n;
+        if (n + 1 < nlim[h] && vec_ok) {
+          float2 o = make_float2(x0, x1);
+          if (a.accumulate) {
+            const float2 p = *reinterpret_cast<const float2*>(cp);
+            o.x += p.x;
+            o.y += p.y;
+          }
+          *reinterpret_cast<float2*>(cp) = o;
+        } else {
+          if (n < nlim[h]) cp[0] = a.accumulate ? cp[0] + x0 : x0;
+          if (n + 1 < nlim[h]) cp[1] = a.accumulate ? cp[1] + x1 : x1;
+        }
+      }
+      if (want_stats) {
+        const float y0 = n < nlim[h] ? x0 : 0.f, y1 = n + 1 < nlim[h] ? x1 : 0.f;
+        s1[0] += y0;
+        s1[1] += y1;
+        s2[0] = fmaf(y0, y0, s2[0]);
+        s2[1] = fmaf(y1, y1, s2[1]);
+      }
+    }
+    if (want_stats) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float c1 = rowgroup_sum(s1[e]), c2 = rowgroup_sum(s2[e]);
+        if (f.g == 0 && n + e < N && (c1 != 0.f || c2 != 0.f)) {
+          atomicAdd(&s_stats[n + e], (double)c1);
+          atomicAdd(&s_stats[a.stat_cols + n + e], (double)c2);
+        }
+      }
+    }
+  }
+}
+
 // Output stage of the fused regression head (losses.py:15-37 + nn.MSELoss fused into the
-// output GEMM of MLPMinion, minions.py:494-524): thread = row (b, t), its 32 columns walk the
+// output GEMM of MLPMinion, minions.py:494-524): row m = (b, t); column n walks the
 // (feature f, context slot j) pairs; label element = label[b][f][t + j - r/2] (zero outside).
-template <int CPW>
-__device__ __forceinline__ void nt_output_ctx(float (&sums)[CPW][32], const NTArgs& a, float alpha,
-                                              int m0, int n0, int cc0, int q, int lane, float* stg,
-                                              double& loss_acc, bool vec_ok) {
-  const int M = a.M, NV = a.cx_nvalid;
-  const int T = a.cx_T, F = a.cx_F, r = a.cx_r;
-  const int m = m0 + q * 32 + lane;
-  const bool row_ok = m < M;
-  const long b = row_ok ? m / T : 0;
-  const int t = row_ok ? (int)(m - b * T) : 0;
+template <int NR>
+__device__ __forceinline__ void nt_output_ctx(const float (&v)[NR], const NTArgs& a, float alpha,
+                                              const Frag& f, double& loss_acc) {
+  const int NV = a.cx_nvalid, T = a.cx_T, F = a.cx_F, r = a.cx_r;
   const float s = __ldg(a.cx_scale + 1);
-  const float* lab_b = a.cx_label + b * F * T;
-  const long orow = row_ok ? m : 0;
-  const int nlim = row_ok ? a.N : 0;             // padding columns are written (as zeros)
+  int t[2];
+  const float* lab[2];
+  bool row_ok[2];
 #pragma unroll
-  for (int h = 0; h < CPW; ++h) {
-    const int nb = n0 + (cc0 + 4 * h) * 32;
-    int f = nb / r, j = nb - f * r;
-    float d2 = 0.f;
-    uint32_t hi[16], lo[16];
+  for (int h = 0; h < 2; ++h) {
+    const int m = f.m[h];
+    row_ok[h] = m < a.M;
+    const long b = row_ok[h] ? m / T : 0;
+    t[h] = row_ok[h] ? (int)(m - b * T) : 0;
+    lab[h] = a.cx_label + b * F * T;
+  }
+  float d2 = 0.f;
 #pragma unroll
-    for (int jn = 0; jn < 32; jn += 2) {
+  for (int j = 0; j < NR / 4; ++j) {
+    const int n = f.n0 + 8 * j + 2 * f.t4;      // n + 1 < a.N (= ldr, a multiple of 128)
+    float cs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
       float d[2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int n = nb + jn + e;
+        const int nn = n + e;
         float dd = 0.f;
-        if (row_ok && n < NV) {
-          const float x = fmaf(sums[h][jn + e], alpha, a.bias ? __ldg(a.bias + n) : 0.f);
-          const int tt = t + j - (r >> 1);
-          const float lab = (tt >= 0 && tt < T) ? __ldg(lab_b + (long)f * T + tt) : 0.f;
-          dd = x - lab;
+        if (row_ok[h] && nn < NV) {
+          const int ff = nn / r, jj = nn - ff * r;
+          const float x = fmaf(v[4 * j + 2 * h + e], alpha, a.bias ? __ldg(a.bias + nn) : 0.f);
+          const int tt = t[h] + jj - (r >> 1);
+          const float lb = (tt >= 0 && tt < T) ? __ldg(lab[h] + (long)ff * T + tt) : 0.f;
+          dd = x - lb;
         }
-        if (++j == r) { j = 0; ++f; }
         d[e] = dd;
-        sums[h][jn + e] = dd;
+        cs[e] += dd;
         d2 = fmaf(dd, dd, d2);
       }
-      __half h0, l0, h1, l1;
-      f16_split(d[0] * s, h0, l0);
-      f16_split(d[1] * s, h1, l1);
-      hi[jn >> 1] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-      lo[jn >> 1] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-    }
-    loss_acc += (double)d2;
-    store_chunk_16(stg, hi, lane, reinterpret_cast<uint16_t*>(a.C), a.ldc, orow, nlim, nb, vec_ok);
-    store_chunk_16(stg, lo, lane, reinterpret_cast<uint16_t*>(a.cx_lo), a.ldc, orow, nlim, nb, vec_ok);
-    const float s1 = colsum32(sums[h], lane);          // bias gradient: column sums of d
-    if (nb + lane < NV && s1 != 0.f) atomicAdd(a.cx_db + nb + lane, (double)s1);
-  }
-}
-
-// Output stage shared by the 1-CTA and CTA-pair NT kernels: alpha / bias, row map and
-// validity, store (fp32 or bf16), BatchNorm column statistics of the fp32 values.
-template <int CPW, bool OUT16>
-__device__ __forceinline__ void nt_output(float (&sums)[CPW][32], const NTArgs& a, float alpha,
-                                          int m0, int n0, int cc0, int q, int lane, float* stg,
-                                          float* s_stats, bool vec_ok) {
-  const int M = a.M, N = a.N;
-  const int m = m0 + q * 32 + lane;
-  long orow = 0;
-  int nlim = 0;                            // columns [0, nlim) of this row are valid
-  if (m < M) {
-    const int g = m / a.rm.rows_in;
-    const int u = m - g * a.rm.rows_in;
-    orow = (long)g * a.rm.rows_out + u;
-    const long lim = (long)(a.rm.t_valid - u * a.rm.fold) * a.rm.cols_per_fold;
-    nlim = lim <= 0 ? 0 : (lim >= N ? N : (int)lim);
-  }
-  const bool want_stats = a.colsum != nullptr;
-#pragma unroll
-  for (int h = 0; h < CPW; ++h) {
-    const int nb = n0 + (cc0 + 4 * h) * 32;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      float x = sums[h][j] * alpha;
-      if (a.bias != nullptr && nb + j < N) x += __ldg(a.bias + nb + j);
-      sums[h][j] = x;
-    }
-    if constexpr (OUT16)
-      store_chunk_bf16(stg, sums[h], lane, reinterpret_cast<__nv_bfloat16*>(a.C), a.ldc, orow,
-                       nlim, nb, vec_ok);
-    else
-      store_chunk<false>(stg, sums[h], lane, reinterpret_cast<float*>(a.C), a.ldc, orow, nlim, nb,
-                         vec_ok, a.accumulate);
-    if (want_stats) {
-      float sq[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        sums[h][j] = (nb + j < nlim) ? sums[h][j] : 0.f;
-        sq[j] = sums[h][j] * sums[h][j];
-      }
-      const float s1 = colsum32(sums[h], lane);
-      const float s2 = colsum32(sq, lane);
-      if (nb + lane < N) {
-        atomicAdd(&s_stats[nb + lane], s1);
-        atomicAdd(&s_stats[a.stat_cols + nb + lane], s2);
+      if (row_ok[h]) {
+        __half h0, l0, h1, l1;
+        f16_split(d[0] * s, h0, l0);
+        f16_split(d[1] * s, h1, l1);
+        const long off = (long)f.m[h] * a.ldc + n;
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(a.C) + off) = pack_f16(h0, h1);
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(a.cx_lo) + off) = pack_f16(l0, l1);
       }
     }
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {               // bias gradient: column sums of d
+      const float c = rowgroup_sum(cs[e]);
+      if (f.g == 0 && n + e < NV && c != 0.f) atomicAdd(a.cx_db + n + e, (double)c);
+    }
   }
+  loss_acc += (double)d2;
 }
 
-__device__ __forceinline__ void flush_stats(const NTArgs& a, const float* s_stats) {
-  asm volatile("bar.sync 1, 512;" ::: "memory");     // the 16 epilogue warps only
-  for (int col = threadIdx.x; col < a.N; col += N_EPI_WARPS * 32) {
-    const float s = s_stats[col], b2 = s_stats[a.stat_cols + col];
-    if (s != 0.f || b2 != 0.f) {
-      atomicAdd(a.colsum + col, (double)s);
-      atomicAdd(a.colsumsq + col, (double)b2);
+__device__ __forceinline__ void flush_stats(const NTArgs& a, const double* s_stats) {
+  consumer_sync();
+  for (int col = threadIdx.x - 128; col < a.N; col += 256) {
+    const double s = s_stats[col], b2 = s_stats[a.stat_cols + col];
+    if (s != 0.0 || b2 != 0.0) {
+      atomicAdd(a.colsum + col, s);
+      atomicAdd(a.colsumsq + col, b2);
     }
   }
 }
 
 // ------------------------------------------------------------------ NT kernel ----
 // Persistent: CTA b processes tiles b, b+grid, ... (n-tile fastest so concurrently running
-// CTAs share A rows in L2).  The MMA warp accumulates `flush_kb` k-blocks into one of two
-// TMEM buffers; the epilogue warps fold each finished buffer into fp32 register sums with
-// round-to-nearest adds (the tensor core's own accumulator rounds toward zero, which drifts
-// over long K) while the MMAs of the next chunk / next tile run.
-template <int BN, int MODE, int ROWB, bool OUT16>
-__global__ void __launch_bounds__(NTHREADS_V3, 1)
+// CTAs share A rows in L2).  Stage = [A.hi | B.hi | A.lo | B.lo], each 128-byte K-major rows.
+// The split modes accumulate `flush_kb` k-blocks in the wgmma accumulators, then fold them into
+// fp32 register sums with round-to-nearest adds.
+template <int BN, int MODE>
+struct NTCfg {
+  using MT = ModeT<MODE>;
+  static constexpr int BK = 128 / MT::ESZ;                 // elements per k-block
+  static constexpr int A_BYTES = BM * 128;
+  static constexpr int B_BYTES = BN * 128;
+  static constexpr int STAGE_BYTES = (MT::SPLIT ? 2 : 1) * (A_BYTES + B_BYTES);
+  static constexpr int NR = BN / 2;                        // accumulator registers per thread
+};
+
+template <int BN, int MODE, bool OUT16, bool CTX>
+__global__ void __launch_bounds__(NTHREADS, 1)
 tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo,
                   const NTArgs a) {
-  using Cfg = NTCfg<BN, MODE, ROWB>;
+  using Cfg = NTCfg<BN, MODE>;
   using MT = ModeT<MODE>;
-  constexpr int BK = Cfg::BK;
+  constexpr int BK = Cfg::BK, NR = Cfg::NR;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -675,13 +499,11 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
   uint8_t* tiles = smem;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* acc_full = empty_bar + MAX_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_out = reinterpret_cast<float*>(smem + stages * Cfg::STAGE_BYTES + BAR_BYTES);
-  float* s_stats = s_out + OUT_STAGE_BYTES / 4;
+  // column sums in fp64: the order of the warps' additions then only moves bits that the
+  // fp32 consumers of the statistics never see (run-to-run identical results)
+  double* s_stats = reinterpret_cast<double*>(smem + stages * Cfg::STAGE_BYTES + BAR_BYTES);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int M = a.M, N = a.N, K = a.K, R = a.R;
   const int n_tiles = (N + BN - 1) / BN, m_tiles = (M + BM - 1) / BM;
   const int total_tiles = n_tiles * m_tiles;
@@ -694,11 +516,7 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], Cfg::EPI_ACTIVE);       // one arrival per active epilogue warp
+      mbar_init(&empty_bar[s], 8);                     // one arrival per consumer warp
     }
     fence_barrier_init();
     tmap_prefetch(&mAhi);
@@ -709,16 +527,13 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
     }
   }
   if (want_stats)
-    for (int i = threadIdx.x; i < 2 * a.stat_cols; i += NTHREADS_V3) s_stats[i] = 0.f;
-  if (warp == WARP_MMA) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
+    for (int i = threadIdx.x; i < 2 * a.stat_cols; i += NTHREADS) s_stats[i] = 0.0;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
 
-  if (warp == WARP_TMA) {
-    if (lane == 0) {
+  if (wg == 0) {
+    regs_producer();
+    if (threadIdx.x == 0) {
       int s = 0;
       uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -747,317 +562,90 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
         }
       }
     }
-    __syncwarp();
-  } else if (warp == WARP_MMA) {
-    // all 32 lanes run the loop (converged); one elected lane issues each MMA / commit
-    constexpr uint32_t idesc = make_idesc(BM, BN, 0, 0, MT::FMT);
-    const uint64_t dconst = desc_hi_bits<Cfg::LAYOUT>(16, Cfg::SBO);
-    const uint32_t tiles_u32 = smem_u32(tiles);
-    const uint32_t tm0 = __shfl_sync(0xffffffffu, tmem_base, 0);
-    uint32_t c = 0;
-    int s = 0;
-    uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      for (int ch = 0; ch < nchunks; ++ch, ++c) {
-        const uint32_t b = c & 1, aph = (c >> 1) & 1;
-        mbar_wait(&acc_empty[b], aph ^ 1, 4);
-        tc_fence_after();
-        const uint32_t d_tmem = tm0 + b * Cfg::ACC_COLS;
-        const int kb_lo = ch * flush_kb;
-        const int kb_hi = (kb_lo + flush_kb < nkb) ? kb_lo + flush_kb : nkb;
-        for (int kb = kb_lo; kb < kb_hi; ++kb) {
-          mbar_wait(&full_bar[s], ph, 2);
-          tc_fence_after();
-          // descriptor = constant bits + (byte address >> 4); k-step of 32 B = +2
-          const uint64_t dah = dconst + ((tiles_u32 + s * Cfg::STAGE_BYTES) >> 4);
-          const uint64_t dbh = dah + (Cfg::A_BYTES >> 4);
-          const uint64_t dal = dbh + (Cfg::B_BYTES >> 4);
-          const uint64_t dbl = dal + (Cfg::A_BYTES >> 4);
-          issue_kblock<MODE, 1, Cfg::KSTEPS, 2>(d_tmem, BN, dah, dbh, dal, dbl, idesc,
-                                                (kb == kb_lo) ? 0u : 1u);
-          umma_commit_w(&empty_bar[s]);          // frees the smem stage once the MMAs retire
-          if (++s == stages) {
-            s = 0;
-            ph ^= 1;
-          }
-        }
-        umma_commit_w(&acc_full[b]);             // this chunk's accumulator is complete
-      }
-    }
-    __syncwarp();
-  } else {
-    // ---------------- epilogue: 16 warps = 4 TMEM lane quarters x 4 column chunks ------------
-    const int e = warp;                          // epilogue warps are warps 0..15
-    const int q = warp & 3;                      // hardware: warp w may access lanes 32*(w%4)..
-    const int cc0 = e >> 2;                      // first 32-column chunk of this warp
-    if (cc0 < BN / 32) {
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-      const bool vec_ok = OUT16 ? (((a.ldc & 7) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 15u) == 0))
-                                : (((a.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 15u) == 0));
-      const float alpha = a.alpha * (a.alpha_dev ? __ldg(a.alpha_dev) : 1.f);
-      float* stg = s_out + e * OUT_STG_FLOATS;
-      uint32_t c = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
-        float sums[Cfg::CPW][32];
-        for (int ch = 0; ch < nchunks; ++ch, ++c) {
-          const uint32_t b = c & 1, aph = (c >> 1) & 1;
-          mbar_wait(&acc_full[b], aph, 3);
-          tc_fence_after();
-#pragma unroll
-          for (int h = 0; h < Cfg::CPW; ++h)
-            fold_chunk<MODE>(lane_addr + b * Cfg::ACC_COLS + (cc0 + 4 * h) * 32, BN, sums[h],
-                             ch == 0);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[b]);        // buffer may be overwritten now
-        }
-        nt_output<Cfg::CPW, OUT16>(sums, a, alpha, m0, n0, cc0, q, lane, stg, s_stats, vec_ok);
-      }
-    }
-    if (want_stats) flush_stats(a, s_stats);
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-}
 
-// ------------------------------------------------------------------ NT kernel, CTA pair ----
-// Same contract as tc_gemm_nt_kernel; a cluster of two CTAs computes a 256 x BN tile with
-// tcgen05.mma.cta_group::2 (default for N % 128 == 0; PASE_B200_TC_2CTA=0 disables it).
-//   * CTA rank r loads A rows [m0 + 128 r, +128) and B rows [n0 + r BN/2, + BN/2) of every
-//     k-block into ITS shared memory at the same CTA-relative offsets; both signal the
-//     transaction bytes on the LEADER's `full` barrier (rank 0), which expects 2 x STAGE_BYTES.
-//   * the leader's MMA warp issues the M = 256 MMAs and commits with a cluster multicast, so
-//     `empty` / `acc_full` flip in both CTAs; each CTA's producer waits on its own `empty`.
-//   * each CTA's 16 epilogue warps drain the CTA's own TMEM (its 128 rows x BN columns) and
-//     release the buffer on the leader's `acc_empty` (count = both CTAs' epilogue warps).
-template <int BN, int MODE>
-struct NT2Cfg {
-  using MT = ModeT<MODE>;
-  static constexpr int ROWB = 128;
-  static constexpr int BK = ROWB / MT::ESZ;
-  static constexpr int A_BYTES = BM * ROWB;
-  static constexpr int BH = BN / 2;                           // B rows held by one CTA
-  static constexpr int B_BYTES = BH * ROWB;
-  static constexpr int STAGE_BYTES = (MT::SPLIT ? 2 : 1) * (A_BYTES + B_BYTES);   // per CTA
-  static constexpr int ACC_COLS = MT::NACC * BN;
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;
-  static constexpr int CPW = (BN / 32 + 3) / 4;
-  static constexpr int EPI_ACTIVE = BN >= 128 ? 16 : 4 * (BN / 32);
-  static constexpr int SBO = 8 * ROWB;
-  static constexpr int KSTEPS = ROWB / 32;
-  static_assert(TMEM_COLS <= 512, "TMEM budget");
-};
-
-template <int BN, int MODE, bool OUT16, bool CTX = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS_V3, 1)
-tc_gemm_nt2_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
-                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo,
-                   const NTArgs a) {
-  using Cfg = NT2Cfg<BN, MODE>;
-  using MT = ModeT<MODE>;
-  constexpr int BK = Cfg::BK;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  const int stages = a.stages;
-  uint8_t* tiles = smem;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* acc_full = empty_bar + MAX_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_out = reinterpret_cast<float*>(smem + stages * Cfg::STAGE_BYTES + BAR_BYTES);
-  float* s_stats = s_out + OUT_STAGE_BYTES / 4;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int M = a.M, N = a.N, K = a.K, R = a.R;
-  const int n_tiles = (N + BN - 1) / BN, m_tiles = (M + 2 * BM - 1) / (2 * BM);
-  const int total_tiles = n_tiles * m_tiles;
-  const int nkb = (K + BK - 1) / BK;
-  int flush_kb = a.flush_kb;
-  if (flush_kb <= 0 || flush_kb > nkb) flush_kb = nkb;
-  const int nchunks = (nkb + flush_kb - 1) / flush_kb;
-  const bool want_stats = a.colsum != nullptr;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < stages; ++s) {
-      mbar_init(&full_bar[s], 1);                      // leader's: one arrive.expect_tx
-      mbar_init(&empty_bar[s], 1);                     // one multicast commit per release
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);                      // one multicast commit per chunk
-      mbar_init(&acc_empty[b], 2 * Cfg::EPI_ACTIVE);   // leader's: both CTAs' epilogue warps
-    }
-    fence_barrier_init();
-    tmap_prefetch(&mAhi);
-    tmap_prefetch(&mBhi);
-    if (MT::SPLIT) {
-      tmap_prefetch(&mAlo);
-      tmap_prefetch(&mBlo);
-    }
-  }
-  if (want_stats)
-    for (int i = threadIdx.x; i < 2 * a.stat_cols; i += NTHREADS_V3) s_stats[i] = 0.f;
-  if (warp == WARP_MMA) tmem_alloc2<Cfg::TMEM_COLS>(tmem_slot);      // same warp in both CTAs
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();            // barriers of both CTAs initialised before any remote signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-
-  if (warp == WARP_TMA) {
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = pair; tile < total_tiles; tile += npairs) {
-        const int m0 = (tile / n_tiles) * (2 * BM) + (int)rank * BM;
-        const int n0 = (tile % n_tiles) * BN + (int)rank * Cfg::BH;
-        int arow = m0, acol = 0;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&empty_bar[s], ph ^ 1, 21);
-          uint8_t* st = tiles + s * Cfg::STAGE_BYTES;
-          const uint32_t fb = mapa_u32(smem_u32(&full_bar[s]), 0);      // the leader's barrier
-          if (leader) mbar_expect_tx(&full_bar[s], 2 * Cfg::STAGE_BYTES);
-          const int kf = kb * BK;
-          tma2_load_2d(st, &mAhi, fb, acol, arow);
-          tma2_load_2d(st + Cfg::A_BYTES, &mBhi, fb, kf, n0);
-          if (MT::SPLIT) {
-            tma2_load_2d(st + Cfg::A_BYTES + Cfg::B_BYTES, &mAlo, fb, acol, arow);
-            tma2_load_2d(st + 2 * Cfg::A_BYTES + Cfg::B_BYTES, &mBlo, fb, kf, n0);
-          }
-          acol += BK;
-          while (acol >= R) {
-            acol -= R;
-            ++arow;
-          }
-          if (++s == stages) {
-            s = 0;
-            ph ^= 1;
-          }
+  regs_consumer();
+  const int cw = wg - 1;                          // rows [64 cw, +64) of every tile
+  const int wq = (threadIdx.x >> 5) & 3;
+  Frag f;
+  f.g = lane >> 2;
+  f.t4 = lane & 3;
+  const float alpha = a.alpha * (a.alpha_dev ? __ldg(a.alpha_dev) : 1.f);
+  const uint32_t tiles_u32 = smem_u32(tiles);
+  const uint64_t dconst = make_desc(0, 16, 1024);
+  float acc[NR];
+  float corr[MT::NACC == 2 ? NR : 1];
+  float sums[MT::SPLIT ? NR : 1];
+  double cx_loss = 0.0;
+  int s = 0;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
+    for (int ch = 0; ch < nchunks; ++ch) {
+      const int kb_lo = ch * flush_kb;
+      const int kb_hi = (kb_lo + flush_kb < nkb) ? kb_lo + flush_kb : nkb;
+      for (int kb = kb_lo; kb < kb_hi; ++kb) {
+        mbar_wait(&full_bar[s], ph, 2);
+        const uint32_t st = tiles_u32 + s * Cfg::STAGE_BYTES;
+        const uint64_t dah = dconst + ((st + cw * 64 * 128) >> 4);
+        const uint64_t dbh = dconst + ((st + Cfg::A_BYTES) >> 4);
+        const uint64_t dal = dconst + ((st + Cfg::A_BYTES + Cfg::B_BYTES + cw * 64 * 128) >> 4);
+        const uint64_t dbl = dconst + ((st + 2 * Cfg::A_BYTES + Cfg::B_BYTES) >> 4);
+        wgmma_fence();
+        issue_kblock<MODE, 0>(acc, corr, dah, dbh, dal, dbl, 2, kb == kb_lo);
+        wgmma_commit();
+        // drained per k-block: with 3 stages of 64 KB (3xF16), holding a stage for one more
+        // k-block (wait_group 1) starves the producer; it measured 5 % slower on an H100
+        wgmma_wait0();
+        fence_regs(acc);
+        fence_regs(corr);
+        release_stage(&empty_bar[s], lane);
+        if (++s == stages) {
+          s = 0;
+          ph ^= 1;
         }
       }
+      if constexpr (MT::SPLIT) fold_chunk<MODE>(sums, acc, corr, ch == 0);
     }
-    __syncwarp();
-  } else if (warp == WARP_MMA) {
-    if (leader) {
-      // converged warp, elected issue (see umma_w); M = 256 across the pair
-      constexpr uint32_t idesc = make_idesc(2 * BM, BN, 0, 0, MT::FMT);
-      const uint64_t dconst = desc_hi_bits<2>(16, Cfg::SBO);
-      const uint32_t tiles_u32 = smem_u32(tiles);
-      const uint32_t tm0 = __shfl_sync(0xffffffffu, tmem_base, 0);
-      uint32_t c = 0;
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = pair; tile < total_tiles; tile += npairs) {
-        for (int ch = 0; ch < nchunks; ++ch, ++c) {
-          const uint32_t b = c & 1, aph = (c >> 1) & 1;
-          mbar_wait(&acc_empty[b], aph ^ 1, 24);
-          tc_fence_after();
-          const uint32_t d_tmem = tm0 + b * Cfg::ACC_COLS;
-          const int kb_lo = ch * flush_kb;
-          const int kb_hi = (kb_lo + flush_kb < nkb) ? kb_lo + flush_kb : nkb;
-          for (int kb = kb_lo; kb < kb_hi; ++kb) {
-            mbar_wait(&full_bar[s], ph, 22);
-            tc_fence_after();
-            const uint64_t dah = dconst + ((tiles_u32 + s * Cfg::STAGE_BYTES) >> 4);
-            const uint64_t dbh = dah + (Cfg::A_BYTES >> 4);
-            const uint64_t dal = dbh + (Cfg::B_BYTES >> 4);
-            const uint64_t dbl = dal + (Cfg::A_BYTES >> 4);
-            issue_kblock<MODE, 2, Cfg::KSTEPS, 2>(d_tmem, BN, dah, dbh, dal, dbl, idesc,
-                                                  (kb == kb_lo) ? 0u : 1u);
-            umma2_commit_mc_w(&empty_bar[s]);        // frees the stage in both CTAs
-            if (++s == stages) {
-              s = 0;
-              ph ^= 1;
-            }
-          }
-          umma2_commit_mc_w(&acc_full[b]);           // accumulator chunk complete in both CTAs
-        }
-      }
+    f.m[0] = m0 + cw * 64 + wq * 16 + f.g;
+    f.m[1] = f.m[0] + 8;
+    f.n0 = n0;
+    if constexpr (CTX) {
+      if constexpr (MT::SPLIT) nt_output_ctx<NR>(sums, a, alpha, f, cx_loss);
+      else nt_output_ctx<NR>(acc, a, alpha, f, cx_loss);
+    } else {
+      if constexpr (MT::SPLIT) nt_output<NR, OUT16>(sums, a, alpha, f, s_stats);
+      else nt_output<NR, OUT16>(acc, a, alpha, f, s_stats);
     }
-    __syncwarp();
-  } else {
-    // ---------------- epilogue: this CTA's 128 rows x BN columns ----------------
-    const int e = warp;                          // epilogue warps are warps 0..15
-    const int q = warp & 3;
-    const int cc0 = e >> 2;
-    if (cc0 < BN / 32) {
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-      const bool vec_ok = OUT16 ? (((a.ldc & 7) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 15u) == 0))
-                                : (((a.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 15u) == 0));
-      const float alpha = a.alpha * (a.alpha_dev ? __ldg(a.alpha_dev) : 1.f);
-      float* stg = s_out + e * OUT_STG_FLOATS;
-      double cx_loss = 0.0;
-      const uint32_t acc_empty0 = mapa_u32(smem_u32(&acc_empty[0]), 0);
-      uint32_t c = 0;
-      for (int tile = pair; tile < total_tiles; tile += npairs) {
-        const int m0 = (tile / n_tiles) * (2 * BM) + (int)rank * BM;
-        const int n0 = (tile % n_tiles) * BN;
-        float sums[Cfg::CPW][32];
-        for (int ch = 0; ch < nchunks; ++ch, ++c) {
-          const uint32_t b = c & 1, aph = (c >> 1) & 1;
-          mbar_wait(&acc_full[b], aph, 23);
-          tc_fence_after();
-#pragma unroll
-          for (int h = 0; h < Cfg::CPW; ++h)
-            fold_chunk<MODE>(lane_addr + b * Cfg::ACC_COLS + (cc0 + 4 * h) * 32, BN, sums[h],
-                             ch == 0);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_remote(acc_empty0 + b * 8);
-        }
-        if constexpr (CTX)
-          nt_output_ctx<Cfg::CPW>(sums, a, alpha, m0, n0, cc0, q, lane, stg, cx_loss, vec_ok);
-        else
-          nt_output<Cfg::CPW, OUT16>(sums, a, alpha, m0, n0, cc0, q, lane, stg, s_stats, vec_ok);
-      }
-      if constexpr (CTX) {
-        cx_loss = warp_sum_d(cx_loss);
-        if (lane == 0 && cx_loss != 0.0) atomicAdd(a.cx_loss, cx_loss);
-      }
-    }
-    if (want_stats) flush_stats(a, s_stats);
-    tc_fence_before();
   }
-  __syncthreads();
-  cluster_sync_all();            // neither CTA frees TMEM / exits while the pair still uses it
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc2<Cfg::TMEM_COLS>(tmem_base);
+  if constexpr (CTX) {
+    cx_loss = warp_sum_d(cx_loss);
+    if (lane == 0 && cx_loss != 0.0) atomicAdd(a.cx_loss, cx_loss);
   }
+  if (want_stats) flush_stats(a, s_stats);
 }
 
 // ------------------------------------------------------------------ TN kernel ----
 // C[i,j] += alpha * sum_r A[r,i] B[r,j].  A: 4-D tensor (128 B inner, rows-per-group, column
 // blocks, groups); B addressed through the folded-row trick: (r, j) -> row u + j/R of group g,
-// column j % R.  One stage = KR reduction rows (4 UMMA k-steps): 32 rows of fp32, 64 of 16-bit.
+// column j % R.  One stage = KR reduction rows (4 wgmma k-steps): 32 rows of fp32, 64 of 16-bit,
+// stored as MN blocks of [KR rows x 128 B].
+//   16-bit: wgmma reads the MN-major blocks directly (128B swizzle, LBO = next MN block).
+//   fp32  : the consumers transpose each stage into K-major 128B-swizzled tiles [MN x 128 B]
+//           (tf32 wgmma has no MN-major form) and run the NT k-block on them.
 template <int BN, int MODE>
 struct TNCfg {
   using MT = ModeT<MODE>;
   static constexpr int EB = MT::EB;                        // elements per 128-byte MN block
-  static constexpr int KR = 4 * MT::UMMA_K;                // reduction rows per stage
+  static constexpr int KR = 4 * 32 / MT::ESZ;              // reduction rows per stage
   static constexpr int A_BYTES = KR * BM * MT::ESZ;        // BM/EB MN-blocks of [KR rows x 128 B]
   static constexpr int B_BYTES = KR * BN * MT::ESZ;
   static constexpr int STAGE_BYTES = (MT::SPLIT ? 2 : 1) * (A_BYTES + B_BYTES);
-  static constexpr int ACC_COLS = MT::NACC * BN;
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;
-  static constexpr int EPI_ACTIVE = 4 * (BN / 32);
-  // MN-major descriptors: fp32 -> 128B swizzle with 32-byte base (4 k-rows per atom);
-  // 16-bit -> plain 128B swizzle (8 k-rows per atom)
-  static constexpr int LAYOUT = MT::ESZ == 4 ? 1 : 2;
-  static constexpr int SBO = MT::ESZ == 4 ? 512 : 1024;
+  static constexpr bool TRANSPOSE = MT::ESZ == 4;
+  static constexpr int T_BYTES = TRANSPOSE ? STAGE_BYTES : 0;   // K-major copy of one stage
   static constexpr int LBO = KR * 128;                     // next MN block
-  static constexpr int KSTEP_DESC = (MT::UMMA_K * 128) >> 4;   // UMMA_K k-rows of 128 B
-  static_assert(TMEM_COLS <= 512, "TMEM budget");
+  static constexpr int NR = BN / 2;
 };
 
 struct TNArgs {
@@ -1067,31 +655,94 @@ struct TNArgs {
   int I, J, groups, rows_per_group;
   float alpha;
   const float* alpha_dev;
-  int chunks_per_split, flush_ch, stages, b_blocked;
-  int lbo, sbo;                    // MN-major descriptor strides (TNCfg defaults)
+  int chunks_per_split, flush_ch, stages, b_blocked, accumulate;
+  float* ws;                       // several splits: [split][tile][BM x BN] partial tiles
 };
 
+// fp32 stage operand [rows/32 blocks of (32 k-rows x 32 elements)] -> K-major 128B-swizzled
+// [rows x 32 k] (row i, k at byte i*128 + ((k/4 ^ i%8) * 16) + (k%4) * 4)
+template <int ROWS>
+__device__ __forceinline__ void transpose_tile(const float* __restrict__ src, float* __restrict__ dst,
+                                               int ctid) {
+#pragma unroll 4
+  for (int e = ctid; e < 32 * ROWS; e += 256) {
+    const int k = e / ROWS, i = e % ROWS;
+    dst[i * 32 + ((((k >> 2) ^ (i & 7))) << 2) + (k & 3)] = src[(i >> 5) * 1024 + k * 32 + (i & 31)];
+  }
+}
+
+// alpha * (this warp's 16 tile rows starting at r0).  One split: straight into C (C = x, or
+// C += x when accumulating; every element has exactly one writer).  Several splits: into this
+// split's partial tile in the workspace, which tn_reduce_splits_kernel sums in split order, so
+// the result does not depend on the order in which the splits finish.
+template <int BN, int NR>
+__device__ __forceinline__ void tn_output(const float (&v)[NR], const TNArgs& a, int r0, int i0,
+                                          int j0, int lane) {
+  const float alpha = a.alpha * (a.alpha_dev ? __ldg(a.alpha_dev) : 1.f);
+  const bool vec_ok = ((a.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 7u) == 0);
+  const int g = lane >> 2, t4 = lane & 3;
+  float* tile = a.ws == nullptr ? nullptr
+      : a.ws + (((long)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * (BM * BN);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + g + 8 * h, i = i0 + r;
+    if (tile == nullptr && i >= a.I) continue;
+    float* crow = a.C + (long)i * a.ldc;
+#pragma unroll
+    for (int j = 0; j < NR / 4; ++j) {
+      const int col = 8 * j + 2 * t4, n = j0 + col;
+      const float x0 = v[4 * j + 2 * h] * alpha, x1 = v[4 * j + 2 * h + 1] * alpha;
+      if (tile != nullptr) {
+        *reinterpret_cast<float2*>(tile + r * BN + col) = make_float2(x0, x1);
+      } else if (n + 1 < a.J && vec_ok) {
+        float2 o = make_float2(x0, x1);
+        if (a.accumulate) {
+          const float2 p = *reinterpret_cast<const float2*>(crow + n);
+          o.x += p.x;
+          o.y += p.y;
+        }
+        *reinterpret_cast<float2*>(crow + n) = o;
+      } else {
+        if (n < a.J) crow[n] = a.accumulate ? crow[n] + x0 : x0;
+        if (n + 1 < a.J) crow[n + 1] = a.accumulate ? crow[n + 1] + x1 : x1;
+      }
+    }
+  }
+}
+
+// C[i, j] (+)= sum over the splits, in split order, of the partial tiles holding (i, j)
+__global__ void tn_reduce_splits_kernel(const float* __restrict__ ws, int splits, int tiles_j,
+                                        int bn, long tiles, float* __restrict__ C, long ldc, int I,
+                                        int J, int accumulate) {
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long)I * J) return;
+  const int i = (int)(idx / J), j = (int)(idx % J);
+  const long tile_elems = (long)BM * bn;
+  const float* p = ws + ((long)(i / BM) * tiles_j + j / bn) * tile_elems + (i % BM) * bn + j % bn;
+  float sum = 0.f;
+  for (int z = 0; z < splits; ++z) sum += p[z * tiles * tile_elems];
+  float* c = C + (long)i * ldc + j;
+  *c = accumulate ? *c + sum : sum;
+}
+
 template <int BN, int MODE>
-__global__ void __launch_bounds__(NTHREADS_V3, 1)
+__global__ void __launch_bounds__(NTHREADS, 1)
 tc_gemm_tn_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo,
                   const TNArgs a) {
   using Cfg = TNCfg<BN, MODE>;
   using MT = ModeT<MODE>;
-  constexpr int KR = Cfg::KR, EB = Cfg::EB;
+  constexpr int KR = Cfg::KR, EB = Cfg::EB, NR = Cfg::NR;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   const int stages = a.stages;
   uint8_t* tiles = smem;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * Cfg::STAGE_BYTES);
+  uint8_t* ttile = smem + stages * Cfg::STAGE_BYTES;                 // transposed stage (fp32)
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ttile + Cfg::T_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* acc_full = empty_bar + MAX_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_out = reinterpret_cast<float*>(smem + stages * Cfg::STAGE_BYTES + BAR_BYTES);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int R = a.R;
   const int j0 = blockIdx.x * BN, i0 = blockIdx.y * BM;
   const int cpg = (a.rows_per_group + KR - 1) / KR;           // chunks per group
@@ -1100,45 +751,30 @@ tc_gemm_tn_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
   long c_end = c_begin + a.chunks_per_split;
   if (c_end > total_chunks) c_end = total_chunks;
   const int nch = (int)(c_end - c_begin);
+  if (nch <= 0) return;                // uniform across the CTA
   int flush_ch = a.flush_ch;
-  if (flush_ch <= 0 || flush_ch > nch) flush_ch = nch > 0 ? nch : 1;
+  if (flush_ch <= 0 || flush_ch > nch) flush_ch = nch;
   const int nflush = (nch + flush_ch - 1) / flush_ch;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], Cfg::EPI_ACTIVE);
+      mbar_init(&empty_bar[s], 8);
     }
     fence_barrier_init();
     tmap_prefetch(&mAhi);
     tmap_prefetch(&mBhi);
   }
-  if (warp == WARP_MMA) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
-  if (nch <= 0) {                      // uniform across the CTA
-    __syncthreads();
-    if (warp == WARP_MMA) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-    return;
-  }
   const int jq = j0 / R, jc = j0 % R;  // folded-row offset / column of this B tile
 
-  if (warp == WARP_TMA) {
-    if (lane == 0) {
-      int s = -1;
-      uint32_t ph = 1;
+  if (wg == 0) {
+    regs_producer();
+    if (threadIdx.x == 0) {
+      int s = 0;
+      uint32_t ph = 0;
       for (int it = 0; it < nch; ++it) {
-        if (++s == stages || it == 0) {
-          s = 0;
-          ph ^= 1;
-        }
         mbar_wait(&empty_bar[s], ph ^ 1, 11);
         const long ch = c_begin + it;
         const int g = (int)(ch / cpg);
@@ -1168,278 +804,76 @@ tc_gemm_tn_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
               tma_load_4d(b_lo + nb * KR * 128, &mBlo, &full_bar[s], 0, u0 + qq, cc / EB, g);
           }
         }
-      }
-    }
-    __syncwarp();
-  } else if (warp == WARP_MMA) {
-    // converged warp, elected issue (see umma_w)
-    constexpr uint32_t idesc = make_idesc(BM, BN, 1, 1, MT::FMT);
-    const uint64_t dconst = desc_hi_bits<Cfg::LAYOUT>((uint32_t)a.lbo, (uint32_t)a.sbo);
-    const uint32_t tiles_u32 = smem_u32(tiles);
-    const uint32_t tm0 = __shfl_sync(0xffffffffu, tmem_base, 0);
-    int s = 0;
-    uint32_t ph = 0;
-    for (int f = 0; f < nflush; ++f) {
-      const uint32_t b = f & 1, aph = (f >> 1) & 1;
-      mbar_wait(&acc_empty[b], aph ^ 1, 14);
-      tc_fence_after();
-      const uint32_t d_tmem = tm0 + b * Cfg::ACC_COLS;
-      const int it_lo = f * flush_ch;
-      const int it_hi = (it_lo + flush_ch < nch) ? it_lo + flush_ch : nch;
-      for (int it = it_lo; it < it_hi; ++it) {
-        mbar_wait(&full_bar[s], ph, 12);
-        tc_fence_after();
-        const uint64_t dah = dconst + ((tiles_u32 + s * Cfg::STAGE_BYTES) >> 4);
-        const uint64_t dbh = dah + (Cfg::A_BYTES >> 4);
-        const uint64_t dal = dbh + (Cfg::B_BYTES >> 4);
-        const uint64_t dbl = dal + (Cfg::A_BYTES >> 4);
-        issue_kblock<MODE, 1, 4, Cfg::KSTEP_DESC>(d_tmem, BN, dah, dbh, dal, dbl, idesc,
-                                                  (it == it_lo) ? 0u : 1u);
-        umma_commit_w(&empty_bar[s]);
         if (++s == stages) {
           s = 0;
           ph ^= 1;
         }
       }
-      umma_commit_w(&acc_full[b]);
     }
-    __syncwarp();
-  } else {
-    const int e = warp;                          // epilogue warps are warps 0..15
-    const int q = warp & 3;
-    const int cc = e >> 2;
-    if (cc < BN / 32) {
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(cc * 32);
-      float sums[32];
-      for (int f = 0; f < nflush; ++f) {
-        const uint32_t b = f & 1, aph = (f >> 1) & 1;
-        mbar_wait(&acc_full[b], aph, 13);
-        tc_fence_after();
-        fold_chunk<MODE>(taddr + b * Cfg::ACC_COLS, BN, sums, f == 0);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[b]);
-      }
-      const int i = i0 + q * 32 + lane;
-      const bool vec_ok = ((a.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 15u) == 0);
-      const float alpha = a.alpha * (a.alpha_dev ? __ldg(a.alpha_dev) : 1.f);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) sums[j] *= alpha;
-      store_chunk<true>(s_out + e * OUT_STG_FLOATS, sums, lane, a.C, a.ldc, (long)i,
-                        i < a.I ? a.J : 0, j0 + cc * 32, vec_ok, 0);
-    }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-}
 
-// ------------------------------------------------------------------ TN kernel, CTA pair ----
-// Same contract as tc_gemm_tn_kernel for I >= 256: a cluster of two CTAs computes a 256 (I) x
-// BN (J) tile with tcgen05.mma.cta_group::2.  CTA rank r loads the A columns [i0 + 128 r,
-// +128) (BM/EB MN-blocks) and ONE half of B's BN columns ([j0 + r BN/2, + BN/2)) of every
-// reduction chunk; barriers as in tc_gemm_nt2_kernel (transaction bytes on the leader's
-// `full`, multicast commits, the leader's `acc_empty` counts both CTAs' epilogue warps).
-// Operand bytes read from shared memory per MMA: 6 KB instead of 8 KB per SM, and 25 % fewer
-// bytes through TMA / L2 per flop.
-template <int BN, int MODE>
-struct TN2Cfg {
-  using MT = ModeT<MODE>;
-  static constexpr int EB = MT::EB;
-  static constexpr int KR = 4 * MT::UMMA_K;
-  static constexpr int BH = BN / 2;                        // B columns held by one CTA
-  static constexpr int A_BYTES = KR * BM * MT::ESZ;
-  static constexpr int B_BYTES = KR * BH * MT::ESZ;
-  static constexpr int STAGE_BYTES = (MT::SPLIT ? 2 : 1) * (A_BYTES + B_BYTES);   // per CTA
-  static constexpr int ACC_COLS = MT::NACC * BN;
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;
-  static constexpr int EPI_ACTIVE = 4 * (BN / 32);
-  static constexpr int LAYOUT = MT::ESZ == 4 ? 1 : 2;
-  static constexpr int SBO = MT::ESZ == 4 ? 512 : 1024;
-  static constexpr int LBO = KR * 128;
-  static constexpr int KSTEP_DESC = (MT::UMMA_K * 128) >> 4;
-  static_assert(TMEM_COLS <= 512, "TMEM budget");
-  static_assert(BH % EB == 0, "each CTA's B half must be whole 128-byte MN blocks");
-};
-
-template <int BN, int MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS_V3, 1)
-tc_gemm_tn2_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
-                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo,
-                   const TNArgs a) {
-  using Cfg = TN2Cfg<BN, MODE>;
-  using MT = ModeT<MODE>;
-  constexpr int KR = Cfg::KR, EB = Cfg::EB;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  const int stages = a.stages;
-  uint8_t* tiles = smem;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* acc_full = empty_bar + MAX_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_out = reinterpret_cast<float*>(smem + stages * Cfg::STAGE_BYTES + BAR_BYTES);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int R = a.R;
-  const int j0 = (blockIdx.x >> 1) * BN, i0 = blockIdx.y * (2 * BM) + (int)rank * BM;
-  const int cpg = (a.rows_per_group + KR - 1) / KR;           // chunks per group
-  const long total_chunks = (long)a.groups * cpg;
-  const long c_begin = (long)blockIdx.z * a.chunks_per_split;
-  long c_end = c_begin + a.chunks_per_split;
-  if (c_end > total_chunks) c_end = total_chunks;
-  const int nch = (int)(c_end - c_begin);                    // identical in both CTAs
-  int flush_ch = a.flush_ch;
-  if (flush_ch <= 0 || flush_ch > nch) flush_ch = nch > 0 ? nch : 1;
-  const int nflush = (nch + flush_ch - 1) / flush_ch;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < stages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 2 * Cfg::EPI_ACTIVE);
-    }
-    fence_barrier_init();
-    tmap_prefetch(&mAhi);
-    tmap_prefetch(&mBhi);
-  }
-  if (warp == WARP_MMA) tmem_alloc2<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  // this CTA's half of the B tile: columns [j0 + rank*BH, +BH)
-  const int jb = j0 + (int)rank * Cfg::BH;
-  const int jq = jb / R, jc = jb % R;
-
-  if (nch > 0) {
-    if (warp == WARP_TMA) {
-      if (lane == 0) {
-        int s = -1;
-        uint32_t ph = 1;
-        for (int it = 0; it < nch; ++it) {
-          if (++s == stages || it == 0) {
-            s = 0;
-            ph ^= 1;
-          }
-          mbar_wait(&empty_bar[s], ph ^ 1, 31);
-          const long ch = c_begin + it;
-          const int g = (int)(ch / cpg);
-          const int u0 = (int)(ch - (long)g * cpg) * KR;
-          uint8_t* st = tiles + s * Cfg::STAGE_BYTES;
-          const uint32_t fb = mapa_u32(smem_u32(&full_bar[s]), 0);
-          if (leader) mbar_expect_tx(&full_bar[s], 2 * Cfg::STAGE_BYTES);
-          uint8_t* a_hi = st;
-          uint8_t* b_hi = st + Cfg::A_BYTES;
-          uint8_t* a_lo = b_hi + Cfg::B_BYTES;
-          uint8_t* b_lo = a_lo + Cfg::A_BYTES;
-          tma2_load_4d(a_hi, &mAhi, fb, 0, u0, i0 / EB, g);
-          if (MT::SPLIT) tma2_load_4d(a_lo, &mAlo, fb, 0, u0, i0 / EB, g);
-#pragma unroll
-          for (int nb = 0; nb < Cfg::BH / EB; ++nb) {
-            // EB consecutive columns never straddle a folded row (R % EB == 0)
-            const int col = jc + nb * EB;
-            const int qq = jq + col / R, cc = col % R;
-            tma2_load_4d(b_hi + nb * KR * 128, &mBhi, fb, 0, u0 + qq, cc / EB, g);
-            if (MT::SPLIT) tma2_load_4d(b_lo + nb * KR * 128, &mBlo, fb, 0, u0 + qq, cc / EB, g);
-          }
+  regs_consumer();
+  const int cw = wg - 1;
+  const int wq = (threadIdx.x >> 5) & 3;
+  const int ctid = threadIdx.x - 128;
+  // K-major (transposed fp32) or MN-major (16-bit) descriptors; WG cw's 64 A rows start
+  // 64 * 128 B into the K-major tile, one MN block (KR * 128 B) into the MN-major stage
+  const uint64_t dconst = Cfg::TRANSPOSE ? make_desc(0, 16, 1024) : make_desc(0, Cfg::LBO, 1024);
+  const uint32_t kstep = Cfg::TRANSPOSE ? 2u : (uint32_t)((16 * 128) >> 4);
+  float acc[NR];
+  float corr[MT::NACC == 2 ? NR : 1];
+  float sums[MT::SPLIT ? NR : 1];
+  int s = 0;
+  uint32_t ph = 0;
+  for (int fl = 0; fl < nflush; ++fl) {
+    const int it_lo = fl * flush_ch;
+    const int it_hi = (it_lo + flush_ch < nch) ? it_lo + flush_ch : nch;
+    for (int it = it_lo; it < it_hi; ++it) {
+      mbar_wait(&full_bar[s], ph, 12);
+      uint32_t base;
+      if constexpr (Cfg::TRANSPOSE) {
+        consumer_sync();               // both warpgroups' previous wgmmas have retired
+        const float* st = reinterpret_cast<const float*>(tiles + s * Cfg::STAGE_BYTES);
+        float* tt = reinterpret_cast<float*>(ttile);
+        transpose_tile<BM>(st, tt, ctid);
+        transpose_tile<BN>(st + Cfg::A_BYTES / 4, tt + Cfg::A_BYTES / 4, ctid);
+        if constexpr (MT::SPLIT) {
+          const int o = (Cfg::A_BYTES + Cfg::B_BYTES) / 4;
+          transpose_tile<BM>(st + o, tt + o, ctid);
+          transpose_tile<BN>(st + o + Cfg::A_BYTES / 4, tt + o + Cfg::A_BYTES / 4, ctid);
         }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        consumer_sync();
+        release_stage(&empty_bar[s], lane);
+        base = smem_u32(ttile);
+      } else {
+        base = smem_u32(tiles + s * Cfg::STAGE_BYTES);
       }
-      __syncwarp();
-    } else if (warp == WARP_MMA) {
-      if (leader) {
-        constexpr uint32_t idesc = make_idesc(2 * BM, BN, 1, 1, MT::FMT);
-        const uint64_t dconst = desc_hi_bits<Cfg::LAYOUT>((uint32_t)a.lbo, (uint32_t)a.sbo);
-        const uint32_t tiles_u32 = smem_u32(tiles);
-        const uint32_t tm0 = __shfl_sync(0xffffffffu, tmem_base, 0);
-        int s = 0;
-        uint32_t ph = 0;
-        for (int f = 0; f < nflush; ++f) {
-          const uint32_t b = f & 1, aph = (f >> 1) & 1;
-          mbar_wait(&acc_empty[b], aph ^ 1, 34);
-          tc_fence_after();
-          const uint32_t d_tmem = tm0 + b * Cfg::ACC_COLS;
-          const int it_lo = f * flush_ch;
-          const int it_hi = (it_lo + flush_ch < nch) ? it_lo + flush_ch : nch;
-          for (int it = it_lo; it < it_hi; ++it) {
-            mbar_wait(&full_bar[s], ph, 32);
-            tc_fence_after();
-            const uint64_t dah = dconst + ((tiles_u32 + s * Cfg::STAGE_BYTES) >> 4);
-            const uint64_t dbh = dah + (Cfg::A_BYTES >> 4);
-            const uint64_t dal = dbh + (Cfg::B_BYTES >> 4);
-            const uint64_t dbl = dal + (Cfg::A_BYTES >> 4);
-            issue_kblock<MODE, 2, 4, Cfg::KSTEP_DESC>(d_tmem, BN, dah, dbh, dal, dbl, idesc,
-                                                      (it == it_lo) ? 0u : 1u);
-            umma2_commit_mc_w(&empty_bar[s]);
-            if (++s == stages) {
-              s = 0;
-              ph ^= 1;
-            }
-          }
-          umma2_commit_mc_w(&acc_full[b]);
-        }
+      const uint32_t a_off = Cfg::TRANSPOSE ? cw * 64 * 128 : cw * Cfg::LBO;
+      const uint64_t dah = dconst + ((base + a_off) >> 4);
+      const uint64_t dbh = dconst + ((base + Cfg::A_BYTES) >> 4);
+      const uint64_t dal = dconst + ((base + Cfg::A_BYTES + Cfg::B_BYTES + a_off) >> 4);
+      const uint64_t dbl = dconst + ((base + 2 * Cfg::A_BYTES + Cfg::B_BYTES) >> 4);
+      wgmma_fence();
+      issue_kblock<MODE, Cfg::TRANSPOSE ? 0 : 1>(acc, corr, dah, dbh, dal, dbl, kstep, it == it_lo);
+      wgmma_commit();
+      wgmma_wait0();
+      fence_regs(acc);
+      fence_regs(corr);
+      if constexpr (!Cfg::TRANSPOSE) release_stage(&empty_bar[s], lane);
+      if (++s == stages) {
+        s = 0;
+        ph ^= 1;
       }
-      __syncwarp();
-    } else {
-      const int e = warp;                          // epilogue warps are warps 0..15
-      const int q = warp & 3;
-      const int cc = e >> 2;
-      if (cc < BN / 32) {
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(cc * 32);
-        const uint32_t acc_empty0 = mapa_u32(smem_u32(&acc_empty[0]), 0);
-        float sums[32];
-        for (int f = 0; f < nflush; ++f) {
-          const uint32_t b = f & 1, aph = (f >> 1) & 1;
-          mbar_wait(&acc_full[b], aph, 33);
-          tc_fence_after();
-          fold_chunk<MODE>(taddr + b * Cfg::ACC_COLS, BN, sums, f == 0);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_remote(acc_empty0 + b * 8);
-        }
-        const int i = i0 + q * 32 + lane;
-        const bool vec_ok = ((a.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.C) & 15u) == 0);
-        const float alpha = a.alpha * (a.alpha_dev ? __ldg(a.alpha_dev) : 1.f);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) sums[j] *= alpha;
-        store_chunk<true>(s_out + e * OUT_STG_FLOATS, sums, lane, a.C, a.ldc, (long)i,
-                          i < a.I ? a.J : 0, j0 + cc * 32, vec_ok, 0);
-      }
-      tc_fence_before();
     }
+    if constexpr (MT::SPLIT) fold_chunk<MODE>(sums, acc, corr, fl == 0);
   }
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc2<Cfg::TMEM_COLS>(tmem_base);
-  }
+  if constexpr (MT::SPLIT) tn_output<BN, NR>(sums, a, cw * 64 + wq * 16, i0, j0, lane);
+  else tn_output<BN, NR>(acc, a, cw * 64 + wq * 16, i0, j0, lane);
 }
 
 // ------------------------------------------------------------------ host side ----
-static bool pase_tc_use_2cta() {
-  static int v = -1;
-  if (v < 0) {
-    // CTA-pair kernel (tcgen05 cta_group::2): on by default (NT 2.41 -> 2.16 ms per PASE+
-    // step, profiles/r01_history.md); PASE_B200_TC_2CTA=0 selects the 1-CTA kernel
-    const char* e = getenv("PASE_B200_TC_2CTA");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
-
 // A timed-out mbarrier wait traps the kernel; the (tag, block, thread) it recorded in the
 // mapped host diagnostics word is appended to the error message of the failing call.
 static unsigned int* h_tc_diag = nullptr;
@@ -1527,20 +961,20 @@ int make_map(CUtensorMap* map, const void* base, int mode, int rank, const uint6
     }                                                                      \
   } while (0)
 
-template <int BN, int MODE, int ROWB, bool OUT16>
+template <int BN, int MODE, bool OUT16, bool CTX>
 int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
               const CUtensorMap& bl, NTArgs a, cudaStream_t st) {
-  using Cfg = NTCfg<BN, MODE, ROWB>;
+  using Cfg = NTCfg<BN, MODE>;
   static bool attr = false;
   a.stat_cols = a.colsum ? ((a.N + 31) / 32) * 32 : 0;
-  a.stages = pick_stages(Cfg::STAGE_BYTES, 2 * a.stat_cols * 4);
-  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, 2 * a.stat_cols * 4);
+  a.stages = pick_stages(Cfg::STAGE_BYTES, 2 * a.stat_cols * 8);
+  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, 2 * a.stat_cols * 8);
   if (a.stages < 2) {
     pase_set_error("pase_tc_gemm_nt: not enough shared memory for 2 pipeline stages");
     return PASE_ERR_UNSUPPORTED;
   }
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt_kernel<BN, MODE, ROWB, OUT16>,
+    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt_kernel<BN, MODE, OUT16, CTX>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
       pase_set_error("pase_tc_gemm_nt: smem attribute: %s", cudaGetErrorString(e));
@@ -1550,63 +984,36 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
   }
   const long tiles = (long)((a.N + BN - 1) / BN) * ((a.M + BM - 1) / BM);
   const int grid = (int)(tiles < pase_num_sms() ? tiles : pase_num_sms());
-  PASE_LAUNCH((tc_gemm_nt_kernel<BN, MODE, ROWB, OUT16>), grid, NTHREADS_V3, smem, st, ah, al, bh, bl, a);
-  PASE_TC_LAUNCH_CHECK("pase_tc_gemm_nt");
+  PASE_LAUNCH((tc_gemm_nt_kernel<BN, MODE, OUT16, CTX>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
+  PASE_TC_LAUNCH_CHECK(CTX ? "pase_tc_gemm_nt_ctxmse" : "pase_tc_gemm_nt");
   return PASE_OK;
 }
 
-template <int BN, int MODE, bool OUT16>
-int launch_nt2(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
-               const CUtensorMap& bl, NTArgs a, cudaStream_t st) {
-  using Cfg = NT2Cfg<BN, MODE>;
-  static bool attr = false;
-  a.stat_cols = a.colsum ? ((a.N + 31) / 32) * 32 : 0;
-  a.stages = pick_stages(Cfg::STAGE_BYTES, 2 * a.stat_cols * 4);
-  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, 2 * a.stat_cols * 4);
-  if (a.stages < 2) {
-    pase_set_error("pase_tc_gemm_nt (2-CTA): not enough shared memory for 2 pipeline stages");
-    return PASE_ERR_UNSUPPORTED;
+// Partial tiles of the split weight-gradient GEMM: room for 4 CTAs per SM of BM x 128 fp32,
+// allocated once per device on first use (never freed: captured CUDA graphs keep using it).
+static float* tn_workspace(cudaStream_t st) {
+  static float* ws[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) {
+    pase_set_error("pase_tc_gemm_tn: device index %d", dev);
+    return nullptr;
   }
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt2_kernel<BN, MODE, OUT16>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-    if (e != cudaSuccess) {
-      pase_set_error("pase_tc_gemm_nt (2-CTA): smem attribute: %s", cudaGetErrorString(e));
-      return (int)e;
-    }
-    attr = true;
+  if (ws[dev] != nullptr) return ws[dev];
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  cudaStreamIsCapturing(st, &cs);
+  if (cs != cudaStreamCaptureStatusNone) {
+    pase_set_error("pase_tc_gemm_tn: first split-K call on this device inside a stream capture "
+                   "(run one step before capturing)");
+    return nullptr;
   }
-  const long tiles = (long)((a.N + BN - 1) / BN) * ((a.M + 2 * BM - 1) / (2 * BM));
-  const long max_pairs = pase_num_sms() / 2;
-  const int grid = 2 * (int)(tiles < max_pairs ? tiles : max_pairs);   // cluster dims (2,1,1)
-  PASE_LAUNCH((tc_gemm_nt2_kernel<BN, MODE, OUT16>), grid, NTHREADS_V3, smem, st, ah, al, bh, bl, a);
-  PASE_TC_LAUNCH_CHECK("pase_tc_gemm_nt(2cta)");
-  return PASE_OK;
-}
-
-// fused regression head: 3xF16 pair kernel with the contextualised-MSE epilogue
-int launch_nt2_ctx(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
-                   const CUtensorMap& bl, NTArgs a, cudaStream_t st) {
-  using Cfg = NT2Cfg<128, 3>;
-  static bool attr = false;
-  a.stat_cols = 0;
-  a.stages = pick_stages(Cfg::STAGE_BYTES, 0);
-  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, 0);
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt2_kernel<128, 3, true, true>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-    if (e != cudaSuccess) {
-      pase_set_error("pase_tc_gemm_nt_ctxmse: smem attribute: %s", cudaGetErrorString(e));
-      return (int)e;
-    }
-    attr = true;
+  cudaError_t e = cudaMalloc(&ws[dev], (size_t)4 * pase_num_sms() * BM * 128 * sizeof(float));
+  if (e != cudaSuccess) {
+    ws[dev] = nullptr;
+    pase_set_error("pase_tc_gemm_tn: workspace allocation: %s", cudaGetErrorString(e));
+    return nullptr;
   }
-  const long tiles = (long)((a.N + 127) / 128) * ((a.M + 2 * BM - 1) / (2 * BM));
-  const long max_pairs = pase_num_sms() / 2;
-  const int grid = 2 * (int)(tiles < max_pairs ? tiles : max_pairs);
-  PASE_LAUNCH((tc_gemm_nt2_kernel<128, 3, true, true>), grid, NTHREADS_V3, smem, st, ah, al, bh, bl, a);
-  PASE_TC_LAUNCH_CHECK("pase_tc_gemm_nt_ctxmse");
-  return PASE_OK;
+  return ws[dev];
 }
 
 template <int BN, int MODE>
@@ -1614,19 +1021,8 @@ int launch_tn(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
               const CUtensorMap& bl, TNArgs a, cudaStream_t st) {
   using Cfg = TNCfg<BN, MODE>;
   static bool attr = false;
-  a.stages = pick_stages(Cfg::STAGE_BYTES, 0);
-  a.lbo = Cfg::LBO;
-  a.sbo = Cfg::SBO;
-  if (MODE >= 2) {                 // bring-up aid: PASE_B200_TN16_DESC="lbo,sbo" (bytes)
-    static int o_lbo = -1, o_sbo = -1;
-    if (o_lbo == -1) {
-      o_lbo = 0;
-      const char* e = getenv("PASE_B200_TN16_DESC");
-      if (e) sscanf(e, "%d,%d", &o_lbo, &o_sbo);
-    }
-    if (o_lbo > 0) { a.lbo = o_lbo; a.sbo = o_sbo; }
-  }
-  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, 0);
+  a.stages = pick_stages(Cfg::STAGE_BYTES, Cfg::T_BYTES);
+  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, Cfg::T_BYTES);
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(tc_gemm_tn_kernel<BN, MODE>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
@@ -1659,54 +1055,19 @@ int launch_tn(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
   long cps = (total + splits - 1) / splits;
   splits = (total + cps - 1) / cps;
   a.chunks_per_split = (int)cps;
+  a.ws = nullptr;
+  if (splits > 1) {      // splits * tiles <= 4 * sms CTAs (loop above): fits the workspace
+    if ((a.ws = tn_workspace(st)) == nullptr) return PASE_ERR_UNSUPPORTED;
+  }
   dim3 grid(tj, ti, (unsigned)splits);
-  PASE_LAUNCH((tc_gemm_tn_kernel<BN, MODE>), grid, NTHREADS_V3, smem, st, ah, al, bh, bl, a);
+  PASE_LAUNCH((tc_gemm_tn_kernel<BN, MODE>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
   PASE_TC_LAUNCH_CHECK("pase_tc_gemm_tn");
-  return PASE_OK;
-}
-
-template <int BN, int MODE>
-int launch_tn2(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
-               const CUtensorMap& bl, TNArgs a, cudaStream_t st) {
-  using Cfg = TN2Cfg<BN, MODE>;
-  static bool attr = false;
-  a.stages = pick_stages(Cfg::STAGE_BYTES, 0);
-  a.lbo = Cfg::LBO;
-  a.sbo = Cfg::SBO;
-  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, 0);
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_gemm_tn2_kernel<BN, MODE>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-    if (e != cudaSuccess) {
-      pase_set_error("pase_tc_gemm_tn (2-CTA): smem attribute: %s", cudaGetErrorString(e));
-      return (int)e;
-    }
-    attr = true;
+  if (splits > 1) {
+    const long n = (long)a.I * a.J;
+    tn_reduce_splits_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+        a.ws, (int)splits, tj, BN, tiles, a.C, a.ldc, a.I, a.J, a.accumulate);
+    PASE_TC_LAUNCH_CHECK("pase_tc_gemm_tn (split reduction)");
   }
-  const int ti = (a.I + 2 * BM - 1) / (2 * BM), tj = (a.J + BN - 1) / BN;
-  const int cpg = (a.rows_per_group + Cfg::KR - 1) / Cfg::KR;
-  const long total = (long)a.groups * cpg;
-  // one CTA pair per (tile, split): fill whole waves of the SM pairs (see launch_tn)
-  const long tiles = (long)ti * tj;
-  const int pairs = pase_num_sms() / 2;
-  long best = 1;
-  double best_eff = -1.0;
-  for (long sp = 1; sp <= total && sp * tiles <= 4L * pairs; ++sp) {
-    const long cps_try = (total + sp - 1) / sp;
-    if (cps_try < 8 && sp > 1) break;
-    const long ctas = tiles * ((total + cps_try - 1) / cps_try);
-    const long waves = (ctas + pairs - 1) / pairs;
-    const double cost = (double)waves * (double)(cps_try + 6);
-    const double eff = 1.0 / cost;
-    if (eff > best_eff) { best_eff = eff; best = sp; }
-  }
-  long splits = best;
-  long cps = (total + splits - 1) / splits;
-  splits = (total + cps - 1) / cps;
-  a.chunks_per_split = (int)cps;
-  dim3 grid(2 * tj, ti, (unsigned)splits);               // cluster (2,1,1) along x
-  PASE_LAUNCH((tc_gemm_tn2_kernel<BN, MODE>), grid, NTHREADS_V3, smem, st, ah, al, bh, bl, a);
-  PASE_TC_LAUNCH_CHECK("pase_tc_gemm_tn(2cta)");
   return PASE_OK;
 }
 
@@ -1757,8 +1118,8 @@ __global__ void split_tf32_kernel(const float* __restrict__ x, float* __restrict
 extern "C" {
 
 int pase_split_tf32(const float* x, float* hi, float* lo, long n, void* stream) {
-  // hi may be NULL: kind::tf32 ignores the low 13 mantissa bits of its fp32 operands
-  // (verified on B200, tools/tf32_probe.py), so the original array serves as "hi".
+  // hi may be NULL: tf32 wgmma ignores the low 13 mantissa bits of its fp32 operands, so the
+  // original array serves as "hi".
   PASE_CHECK_ARG(x && lo && n > 0, "pase_split_tf32: bad args");
   PASE_CHECK_ARG(aligned16(x) && aligned16(lo) && (hi == nullptr || aligned16(hi)),
                  "pase_split_tf32: alignment");
@@ -1797,43 +1158,25 @@ int pase_tc_gemm_nt(const void* Ahi, const void* Alo, long a_rows, int R, const 
   PASE_CHECK_ARG(colsum == nullptr || N <= 4096, "pase_tc_gemm_nt: stats need N <= 4096");
   PASE_CHECK_ARG(colsum == nullptr || !accumulate, "pase_tc_gemm_nt: stats + accumulate");
   PASE_CHECK_ARG(!c_bf16 || !accumulate, "pase_tc_gemm_nt: bf16 output cannot accumulate");
-  // 256-wide tiles (64-byte k-blocks, see NTCfg) raise the MMA rate per flop by ~1.2x but
-  // halve the tile count (wave quantisation) and double the epilogue per warp: measured on
-  // the PASE+ shapes they only pay off for long reductions (profiles/r01_history.md);
-  // not available with the two-accumulator 3xF16 mode (TMEM budget)
-  const bool wide = N >= 256 && (N % 256) == 0 && K >= 4096 && mode != 3;
-  // bf16 (one pass at the full f16 rate) is bound by operand bytes per flop, not by the tensor
-  // pipe: a CTA pair on a 256 x 256 tile loads 32 KB per k-block for twice the flops of the
-  // 24 KB a 256 x 128 pair tile needs (PASE_B200_BF16_WIDE=0 disables)
-  static int bf16_wide = -1;
-  if (bf16_wide < 0) {
-    const char* e = getenv("PASE_B200_BF16_WIDE");
-    bf16_wide = (e && e[0] == '0') ? 0 : 1;
-  }
-  const bool pair256 = mode == 2 && bf16_wide && N >= 256 && (N % 256) == 0 && pase_tc_use_2cta();
-  const int BN = N <= 64 ? 64 : ((wide || pair256) ? 256 : 128);
-  const int rowb = (BN == 256 && !pair256) ? 64 : 128;
-  const int bk = rowb / esz;
-  // split modes: fold the TMEM accumulator into fp32 register sums every K = 128.  The
-  // accumulator rounds toward zero (a bias of ~0.5 ulp per accumulate step): over K <= 512
-  // that stays below 1e-6 relative, so short reductions (sinc layer, block-1 dgrad) keep
-  // one chunk and a third of the epilogue work
-  const int flush_kb = (split && K > 512) ? (128 / bk > 0 ? 128 / bk : 1) : 0;
+  const int BN = N <= 64 ? 64 : 128;
+  const int bk = eb;
+  // split modes: fold the accumulators into fp32 register sums every K = 128; over K <= 512
+  // the tensor core's own accumulation stays below 1e-6 relative, so short reductions (sinc
+  // layer, block-1 dgrad) keep one chunk
+  const int flush_kb = (split && K > 512) ? 128 / bk : 0;
   CUtensorMap ah, al, bh, bl;
-  const bool pair2 = pair256 || (BN == 128 && (N % 128) == 0 && pase_tc_use_2cta());
   uint64_t adims[2] = {(uint64_t)R, (uint64_t)a_rows};
   uint64_t astr[1] = {(uint64_t)R * esz};
   uint32_t abox[2] = {(uint32_t)bk, (uint32_t)BM};
   uint64_t bdims[2] = {(uint64_t)K, (uint64_t)N};
   uint64_t bstr[1] = {(uint64_t)ldb * esz};
-  uint32_t bbox[2] = {(uint32_t)bk, (uint32_t)(pair2 ? BN / 2 : BN)};   // pair: half per CTA
-  const CUtensorMapSwizzle swz = rowb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  uint32_t bbox[2] = {(uint32_t)bk, (uint32_t)BN};
   int rc;
-  if ((rc = make_map(&ah, Ahi, mode, 2, adims, astr, abox, "A.hi", swz)) != 0) return rc;
-  if ((rc = make_map(&bh, Bhi, mode, 2, bdims, bstr, bbox, "B.hi", swz)) != 0) return rc;
+  if ((rc = make_map(&ah, Ahi, mode, 2, adims, astr, abox, "A.hi")) != 0) return rc;
+  if ((rc = make_map(&bh, Bhi, mode, 2, bdims, bstr, bbox, "B.hi")) != 0) return rc;
   if (split) {
-    if ((rc = make_map(&al, Alo, mode, 2, adims, astr, abox, "A.lo", swz)) != 0) return rc;
-    if ((rc = make_map(&bl, Blo, mode, 2, bdims, bstr, bbox, "B.lo", swz)) != 0) return rc;
+    if ((rc = make_map(&al, Alo, mode, 2, adims, astr, abox, "A.lo")) != 0) return rc;
+    if ((rc = make_map(&bl, Blo, mode, 2, bdims, bstr, bbox, "B.lo")) != 0) return rc;
   } else {
     al = ah;
     bl = bh;
@@ -1847,35 +1190,20 @@ int pase_tc_gemm_nt(const void* Ahi, const void* Alo, long a_rows, int R, const 
   a.cx_label = nullptr; a.cx_F = a.cx_T = a.cx_r = a.cx_nvalid = 0; a.cx_scale = nullptr;
   a.cx_lo = nullptr; a.cx_loss = nullptr; a.cx_db = nullptr;
   cudaStream_t st = (cudaStream_t)stream;
-#define PASE_NT_MODES(FN, ...)                                                           \
-  switch (mode * 2 + (c_bf16 ? 1 : 0)) {                                                 \
-    case 0: return FN(0, false, __VA_ARGS__);                                            \
-    case 1: return FN(0, true, __VA_ARGS__);                                             \
-    case 2: return FN(1, false, __VA_ARGS__);                                            \
-    case 3: return FN(1, true, __VA_ARGS__);                                             \
-    case 4: return FN(2, false, __VA_ARGS__);                                            \
-    case 5: return FN(2, true, __VA_ARGS__);                                             \
-    case 6: return FN(3, false, __VA_ARGS__);                                            \
-    default: return FN(3, true, __VA_ARGS__);                                            \
+#define PASE_NT(BNV)                                                                       \
+  switch (mode * 2 + (c_bf16 ? 1 : 0)) {                                                   \
+    case 0: return launch_nt<BNV, 0, false, false>(ah, al, bh, bl, a, st);                 \
+    case 1: return launch_nt<BNV, 0, true, false>(ah, al, bh, bl, a, st);                  \
+    case 2: return launch_nt<BNV, 1, false, false>(ah, al, bh, bl, a, st);                 \
+    case 3: return launch_nt<BNV, 1, true, false>(ah, al, bh, bl, a, st);                  \
+    case 4: return launch_nt<BNV, 2, false, false>(ah, al, bh, bl, a, st);                 \
+    case 5: return launch_nt<BNV, 2, true, false>(ah, al, bh, bl, a, st);                  \
+    case 6: return launch_nt<BNV, 3, false, false>(ah, al, bh, bl, a, st);                 \
+    default: return launch_nt<BNV, 3, true, false>(ah, al, bh, bl, a, st);                 \
   }
-#define PASE_NT2(MODEV, O16, BNV) launch_nt2<BNV, MODEV, O16>(ah, al, bh, bl, a, st)
-#define PASE_NT1(MODEV, O16, BNV, RB) launch_nt<BNV, MODEV, RB, O16>(ah, al, bh, bl, a, st)
-  if (pair256) return c_bf16 ? launch_nt2<256, 2, true>(ah, al, bh, bl, a, st)
-                             : launch_nt2<256, 2, false>(ah, al, bh, bl, a, st);
-  if (pair2) { PASE_NT_MODES(PASE_NT2, 128) }
-  if (BN == 64) { PASE_NT_MODES(PASE_NT1, 64, 128) }
-  if (BN == 128) { PASE_NT_MODES(PASE_NT1, 128, 128) }
-  switch (mode * 2 + (c_bf16 ? 1 : 0)) {       // BN == 256 (never mode 3)
-    case 0: return PASE_NT1(0, false, 256, 64);
-    case 1: return PASE_NT1(0, true, 256, 64);
-    case 2: return PASE_NT1(1, false, 256, 64);
-    case 3: return PASE_NT1(1, true, 256, 64);
-    case 4: return PASE_NT1(2, false, 256, 64);
-    default: return PASE_NT1(2, true, 256, 64);
-  }
-#undef PASE_NT1
-#undef PASE_NT2
-#undef PASE_NT_MODES
+  if (BN == 64) { PASE_NT(64) }
+  PASE_NT(128)
+#undef PASE_NT
 }
 
 // Fused output layer of a regression head (MLPMinion W + ContextualizedLoss MSE,
@@ -1895,7 +1223,6 @@ int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
                  "pase_tc_gemm_nt_ctxmse: operand alignment (R=%d K=%d ldb=%ld)", R, K, ldb);
   PASE_CHECK_ARG((ldr % 128) == 0 && ldr >= N && aligned16(Rhi) && aligned16(Rlo),
                  "pase_tc_gemm_nt_ctxmse: ldr=%ld must be a multiple of 128 and >= N", ldr);
-  PASE_CHECK_ARG(pase_tc_use_2cta(), "pase_tc_gemm_nt_ctxmse needs the CTA-pair kernels");
   pase_tc_init_diag();
   const int mode = 3, esz = 2, bk = 64;
   CUtensorMap ah, al, bh, bl;
@@ -1904,7 +1231,7 @@ int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
   uint32_t abox[2] = {(uint32_t)bk, (uint32_t)BM};
   uint64_t bdims[2] = {(uint64_t)K, (uint64_t)N};          // rows >= N: zero-filled by TMA
   uint64_t bstr[1] = {(uint64_t)ldb * esz};
-  uint32_t bbox[2] = {(uint32_t)bk, 64};
+  uint32_t bbox[2] = {(uint32_t)bk, 128};
   int rc;
   if ((rc = make_map(&ah, Ahi, mode, 2, adims, astr, abox, "ctx A.hi")) != 0) return rc;
   if ((rc = make_map(&al, Alo, mode, 2, adims, astr, abox, "ctx A.lo")) != 0) return rc;
@@ -1919,7 +1246,7 @@ int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
   a.stages = 0; a.stat_cols = 0;
   a.cx_label = label; a.cx_F = F; a.cx_T = T; a.cx_r = r; a.cx_nvalid = N; a.cx_scale = scale;
   a.cx_lo = Rlo; a.cx_loss = loss_acc; a.cx_db = db_acc;
-  return launch_nt2_ctx(ah, al, bh, bl, a, (cudaStream_t)stream);
+  return launch_nt<128, 3, false, true>(ah, al, bh, bl, a, (cudaStream_t)stream);
 }
 
 // A: groups x [rows_per_group x lda] starting `offA` rows into each group of pitch `pitchA`
@@ -1941,14 +1268,6 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
                  "pase_tc_gemm_tn: need R%%%d==0, lda*%d%%16==0, I%%4==0, J%%%d==0 (R=%d lda=%ld "
                  "I=%d J=%d)", eb, esz, eb, R, lda, I, J);
   cudaStream_t st = (cudaStream_t)stream;
-  if (!accumulate) {
-    cudaError_t e =
-        cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)J * sizeof(float), (size_t)I, st);
-    if (e != cudaSuccess) {
-      pase_set_error("pase_tc_gemm_tn: memset failed: %s", cudaGetErrorString(e));
-      return (int)e;
-    }
-  }
   const int BN = J <= 64 ? 64 : 128;
   const int kr = 4 * (32 / esz);                 // reduction rows per stage
   const int flush_ch = split ? (128 / kr > 0 ? 128 / kr : 1) : 0;   // fold every 128 rows
@@ -1962,15 +1281,7 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
   // B group g covers folded rows [g*pitchB, ...): rows beyond the allocation are zero-filled
   long rows_in_group = b_rows_total - (long)(groups - 1) * pitchB;
   if (rows_in_group > pitchB + (J + R - 1) / R + 1) rows_in_group = pitchB + (J + R - 1) / R + 1;
-  // CTA pair (M = 256) for tall outputs in the 16-bit modes; every CTA then loads ONE half
-  // of the B tile, block by block (PASE_B200_TN_2CTA=0 disables, =2 also enables fp32 modes)
-  static int tn2 = -1;
-  if (tn2 < 0) {
-    const char* e = getenv("PASE_B200_TN_2CTA");
-    tn2 = e ? atoi(e) : 1;
-  }
-  const bool pair = BN == 128 && I >= 256 && tn2 > 0 && (mode >= 2 || tn2 >= 2) && pase_tc_use_2cta();
-  const int b_blocked = !pair && (R % BN) == 0;
+  const int b_blocked = (R % BN) == 0;
   uint64_t bdims[4] = {(uint64_t)eb, (uint64_t)rows_in_group, (uint64_t)(R / eb),
                        (uint64_t)groups};
   uint64_t bstr[3] = {(uint64_t)R * esz, 128, (uint64_t)pitchB * R * esz};
@@ -1979,8 +1290,8 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
   // columns (they only feed output rows >= I, which are never stored); the caller must
   // keep 128 bytes of slack after the last row of A.
   int rc;
-  const CUtensorMapSwizzle sw = esz == 4 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
-                                         : CU_TENSOR_MAP_SWIZZLE_128B;
+  // fp32 stages are transposed in shared memory by the consumers: plain row-major boxes
+  const CUtensorMapSwizzle sw = esz == 4 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
   const char* Ah_off = reinterpret_cast<const char*>(Ahi) + (long)offA * lda * esz;
   if ((rc = make_map(&ah, Ah_off, mode, 4, adims, astr, abox, "tn A.hi", sw)) != 0) return rc;
   if ((rc = make_map(&bh, Bhi, mode, 4, bdims, bstr, bbox, "tn B.hi", sw)) != 0) return rc;
@@ -1996,6 +1307,7 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
   a.R = R; a.C = C; a.ldc = ldc; a.I = I; a.J = J; a.groups = groups;
   a.rows_per_group = rows_per_group; a.alpha = alpha; a.alpha_dev = alpha_dev;
   a.chunks_per_split = 0; a.flush_ch = flush_ch; a.stages = 0; a.b_blocked = b_blocked;
+  a.accumulate = accumulate; a.ws = nullptr;
 #define PASE_TN(BNV)                                                      \
   switch (mode) {                                                         \
     case 0: return launch_tn<BNV, 0>(ah, al, bh, bl, a, st);              \
@@ -2004,14 +1316,6 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
     default: return launch_tn<BNV, 3>(ah, al, bh, bl, a, st);             \
   }
   if (BN == 64) { PASE_TN(64) }
-  if (pair) {
-    switch (mode) {
-      case 0: return launch_tn2<128, 0>(ah, al, bh, bl, a, st);
-      case 1: return launch_tn2<128, 1>(ah, al, bh, bl, a, st);
-      case 2: return launch_tn2<128, 2>(ah, al, bh, bl, a, st);
-      default: return launch_tn2<128, 3>(ah, al, bh, bl, a, st);
-    }
-  }
   PASE_TN(128)
 #undef PASE_TN
 }

@@ -1,4 +1,4 @@
-"""B200-native WaveFe encoder engine: geometry, HBM buffer plan and the
+"""H100-native WaveFe encoder engine: geometry, HBM buffer plan and the
 forward/backward orchestration over the C-ABI kernels.
 
 Formulation (DESIGN.md section 3).  Activations are channel-last (n, t, c).
@@ -295,7 +295,7 @@ class EncoderPlan(object):
         format directly (apad, xq, dyz) are registered at construction; everything else is an
         fp32 tensor converted here (`fresh=False` reuses this step's earlier conversion):
           tf32   : the tensor itself;
-          3xtf32 : activations: the tensor is "hi" (kind::tf32 truncates), lo = rn(x-trunc(x));
+          3xtf32 : activations: the tensor is "hi" (tf32 tensor cores truncate), lo = rn(x-trunc(x));
                    weights: explicit hi = rn(x), lo = rn(x - hi) (no coherent bias);
           bf16   : bf16 copy;    3xf16 : fp16 (hi, lo') pair, gradients pre-scaled by a power
                    of two (alpha = {1/s, s} on the device)."""

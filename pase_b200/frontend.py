@@ -1,7 +1,7 @@
 """Drop-in for ``pase.models.frontend`` (wf_builder / WaveFe, frontend.py:18-40,
 116-279): same constructor kwargs, same ``state_dict`` keys and shapes, same
 ``forward(batch, device=None, mode=None)`` contract -- but forward and backward
-run in the sm_100a kernels of ``pase_b200/csrc`` through ``pase_b200.encoder``.
+run in the sm_90a kernels of ``pase_b200/csrc`` through ``pase_b200.encoder``.
 
 The ``nn.Conv1d`` / ``nn.BatchNorm1d`` / ``nn.PReLU`` / ``nn.Linear`` objects
 below are PARAMETER CONTAINERS only (they give the reference's key names and
@@ -19,7 +19,7 @@ import torch.nn as nn
 from .modules import Model, format_frontend_chunk, format_frontend_output
 from . import encoder as _enc
 
-# "3xtf32": tcgen05 tensor cores with error-compensated TF32 (fp32-equivalent, meets the
+# "3xtf32": wgmma tensor cores with error-compensated TF32 (fp32-equivalent, meets the
 # fp32 parity bar); "fp32": FFMA kernels; "tf32": single-pass TF32 (L2-equivalent only).
 # Shapes the tensor-core kernels cannot take (channel counts not multiples of 32) fall back
 # to the FFMA kernels per GEMM -- still on the GPU, never to a CPU path.
@@ -143,8 +143,8 @@ class WaveFe(Model):
         if cfg["norm_out"]:
             self.norm_out = nn.BatchNorm1d(emb, affine=False)
         self._plans = OrderedDict()
-        # GEMM numerics (encoder.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (tcgen05,
-        # fp32-equivalent), "tf32" (tcgen05), "bf16" (tcgen05, bf16 operands and activations)
+        # GEMM numerics (encoder.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (wgmma,
+        # fp32-equivalent), "tf32" (wgmma), "bf16" (wgmma, bf16 operands and activations)
         self.precision = os.environ.get("PASE_B200_PRECISION", DEFAULT_PRECISION)
         self._sinc_n = self._sinc_win = None
         self.last_output_ntc = None
@@ -205,7 +205,7 @@ class WaveFe(Model):
         if x.dim() != 3 or x.shape[1] != 1:
             raise ValueError("WaveFe expects (N,1,T) waveforms, got %s" % (tuple(x.shape),))
         if not x.is_cuda:
-            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_100a) only; got a %s tensor. "
+            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; got a %s tensor. "
                                "There is no CPU path." % x.device)
         x = x.contiguous().float()
         self._sinc_consts(x.device)

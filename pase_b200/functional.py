@@ -11,7 +11,7 @@ import torch
 
 from . import ops
 
-# GEMM numerics of the heads (same meaning as WaveFe.precision): "3xf16" / "3xtf32" (tcgen05,
+# GEMM numerics of the heads (same meaning as WaveFe.precision): "3xf16" / "3xtf32" (wgmma,
 # fp32-equivalent products), "tf32", "bf16" (bf16 operands, fp32 everything else), or "fp32"
 # (FFMA kernels).
 PRECISION = os.environ.get("PASE_B200_PRECISION", "3xf16")
@@ -87,7 +87,7 @@ def to_operand(flat, n, mode, kind="act"):
 
 def gemm_nt(A, lda, a_used, B, ldb, b_used, C, ldc, M, N, K, bias, rows_in=None, t_valid=None,
             rows_out=None, a_kind="act"):
-    """C[map(m),n] = sum_k A[m*lda+k] B[n*ldb+k] + bias[n]; dispatches tcgen05 / FFMA.
+    """C[map(m),n] = sum_k A[m*lda+k] B[n*ldb+k] + bias[n]; dispatches wgmma / FFMA.
     Optional row map (rows_in, t_valid, rows_out) as in pase_gemm_nt.  A / B may be fp32 flat
     views or already-converted Operands."""
     mode = _MODES[PRECISION]

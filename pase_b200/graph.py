@@ -143,9 +143,9 @@ class PipelinedDPStep(object):
                    activations, ~40 % of the backward time -- runs on the main stream
         eager      NCCL all-reduce of the LOWER bucket (blocks 0..split-1: ~1 MB)
         graph B    one pase_adam_flat launch, D2H of the loss
-    Collectives are never captured (capturing NCCL hung in this image, profiles/r01_history.md);
-    they are ordered against the graph replays with events.  ``optimizer`` must be a FlatAdam
-    whose FIRST parameters are exactly the encoder's blocks < split (see ``order_params``)."""
+    Collectives are never captured; they are ordered against the graph replays with events.
+    ``optimizer`` must be a FlatAdam whose FIRST parameters are exactly the encoder's blocks
+    < split (see ``order_params``)."""
 
     @staticmethod
     def order_params(model, split):

@@ -1,5 +1,5 @@
-"""Generates tests/golden/*.pt from the UNMODIFIED reference (container only:
-needs /root/reference).  Run:  python tests/golden/make_golden.py
+"""Generates tests/golden/*.pt from the UNMODIFIED reference (needs a checkout of
+santi-pdp/pase).  Run:  PASE_REFERENCE_ROOT=<checkout> python tests/golden/make_golden.py
 
 Every case: deterministic parameters (detweights.fill_state_dict) are loaded
 into the reference module, seeded inputs are pushed through the reference's own
@@ -34,6 +34,13 @@ MINI_NORNN_CFG = {
     "strides": [1, 10, 2, 1, 2, 1, 2, 2],
     "fmaps": [8, 8, 16, 16, 24, 24, 32, 32],
     "emb_dim": 20, "norm_out": True,
+}
+# checkpoint-format fixtures only (small files)
+SAVER_CFG = {
+    "kwidths": [31, 5, 3, 3, 3, 3, 3, 3],
+    "strides": [1, 10, 2, 1, 2, 1, 2, 2],
+    "fmaps": [8, 8, 8, 8, 8, 8, 8, 8],
+    "emb_dim": 8, "norm_out": True,
 }
 MINI_WORKERS = {
     "regr": [
@@ -96,6 +103,82 @@ def encoder_case(name, cfg, N, T, training, seed, with_grads=True):
     out["frame_counts"] = torch.tensor(lens)
     torch.save(out, os.path.join(HERE, name + ".pt"))
     print(name, tuple(y.shape), lens)
+
+
+def _file_bytes(path):
+    with open(path, "rb") as f:
+        return torch.tensor(list(f.read()), dtype=torch.uint8)
+
+
+def boundary_case():
+    """boundary.pt: what the reference's own training-step code and checkpoint code produce,
+    for tests/test_reference_boundary.py.
+      sched/*: backprop_scheduler('base') with one Adam per worker + one for the frontend
+               (trainer.py:86-143, 229-244) driving the reference pase model of
+               pase_mini_workers_1600 for two steps: per-step losses and the final weights
+               (tensors above FULL_MAX elements as a strided sample plus their L2 norm).
+      saver/*: files the reference Saver writes for a SAVER_CFG frontend (four saves,
+               max_ckpts=2, prefix 'PASE-'), and those of Model.save(dir, 5)."""
+    import copy
+    import tempfile
+    rh.import_reference()
+    from pase.models.WorkerScheduler.worker_scheduler import backprop_scheduler
+    from pase.models.modules import Saver as RefSaver
+    out = {}
+    seed, B, T = 8, 2, 1600
+    wcfg = json.loads(json.dumps(MINI_WORKERS))
+    model = rh.build_ref_pase(dict(MINI_CFG), copy.deepcopy(wcfg)).train()
+    model.load_state_dict(fill_state_dict(model.state_dict(), seed))
+    batch = {k: seeded_randn((B, 1, T), seed + 10 + i, 0.5)
+             for i, k in enumerate(["chunk", "chunk_ctxt", "chunk_rand", "cchunk"])}
+    with torch.no_grad():
+        model.eval()
+        Tq = model.frontend(batch["chunk"]).shape[2]
+        model.train()
+    for i, w in enumerate(wcfg["regr"]):
+        if w["name"] != "cchunk":
+            batch[w["name"]] = seeded_randn((B, w["num_outputs"], Tq), seed + 100 + i)
+    sched = backprop_scheduler(model, mode="base")
+    fe_opt = torch.optim.Adam(model.frontend.parameters(), lr=5e-4)
+    cls_opt = {w.name: torch.optim.Adam(w.parameters(), lr=4e-4)
+               for w in model.classification_workers}
+    regr_opt = {w.name: torch.optim.Adam(w.parameters(), lr=4e-4)
+                for w in model.regression_workers}
+    for it in range(2):
+        random.seed(seed + it)
+        h, chunk, preds, labels = model.forward(dict(batch), 1, "cpu")
+        losses, _ = sched(preds, labels, cls_opt, regr_opt, fe_opt, device="cpu")
+        for k, v in losses.items():
+            out["sched/loss%d/%s" % (it, k)] = torch.tensor(float(v.detach()), dtype=torch.float64)
+    for k, v in model.state_dict().items():
+        if v.numel() <= FULL_MAX:
+            out["sched/state/" + k] = v.detach().clone()
+        else:
+            out["sched/ssample/" + k] = sample_view(v.detach())
+            out["sched/snorm/" + k] = v.detach().double().norm()
+
+    fe = rh.build_ref_frontend(dict(SAVER_CFG))
+    fe.load_state_dict(fill_state_dict(fe.state_dict(), 7))
+    opt = torch.optim.Adam(fe.parameters(), lr=1e-3)
+    with tempfile.TemporaryDirectory() as d:
+        d1 = os.path.join(d, "saver")
+        rs = RefSaver(fe, d1, max_ckpts=2, optimizer=opt, prefix="PASE-")
+        import contextlib
+        import io
+        with contextlib.redirect_stdout(io.StringIO()):
+            for step in (10, 20, 30, 40):
+                rs.save("FE_e%d" % (step // 10), step)
+            d3 = os.path.join(d, "model_api")
+            fe.save(d3, 5)
+        out["saver/listing"] = json.dumps(sorted(os.listdir(d1)))
+        for name in sorted(os.listdir(d1)):
+            out["saver/file/" + name] = _file_bytes(os.path.join(d1, name))
+        out["saver/model_name"] = fe.name
+        for name in sorted(os.listdir(d3)):
+            out["saver/model_file/" + name] = _file_bytes(os.path.join(d3, name))
+    out["saver/pasep_total_params"] = rh.build_ref_frontend("cfg/frontend/PASE+.cfg").get_total_params()
+    torch.save(out, os.path.join(HERE, "boundary.pt"))
+    print("boundary", os.path.getsize(os.path.join(HERE, "boundary.pt")))
 
 
 def frame_count_table():
@@ -194,3 +277,4 @@ if __name__ == "__main__":
     pase_case("pase_mini_workers_1600", MINI_CFG, MINI_WORKERS, 2, 1600, 8)
     pase_case("pase_plus_workers_3200", "cfg/frontend/PASE+.cfg",
               "cfg/workers/workers+.cfg", 2, 3200, 9)
+    boundary_case()

@@ -1,7 +1,8 @@
 """Data parallelism on real GPUs (2 ranks, NCCL over NVLink): the flat-buffer all-reduce
 averages the per-rank gradients, and the pipelined step (all-reduce hidden behind the tail
-of backward, three CUDA graphs) equals the plain eager step.  Needs >= 2 GPUs:
-    gpurun --gpus 2 -- python -m pytest tests/test_dp_nccl_gpu.py -m gpu
+of backward, three CUDA graphs) equals the plain eager step.  Needs >= 2 GPUs (skips
+otherwise):
+    python -m pytest tests/test_dp_nccl_gpu.py -m gpu
 """
 import os
 import socket
@@ -106,7 +107,7 @@ def _worker(rank, world, port, out):
     dist.destroy_process_group()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_flat_allreduce_and_pipelined_step_two_gpus(tmp_path):
     import torch.multiprocessing as mp
     mp.spawn(_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=True)
@@ -208,7 +209,7 @@ def _peer_worker(rank, world, port, out):
     dist.destroy_process_group()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_peer_memory_dp_update_two_gpus(tmp_path):
     import torch.multiprocessing as mp
     mp.spawn(_peer_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=True)

@@ -34,7 +34,7 @@ def _native(cfg, seed, training, precision="fp32"):
 WIDE = [c for c in CASES if "mini" not in c]       # channel counts multiples of 64
 
 
-# "fp32": FFMA kernels; "3xtf32" / "3xf16": tcgen05 tensor cores with error-compensated
+# "fp32": FFMA kernels; "3xtf32" / "3xf16": wgmma tensor cores with error-compensated
 # TF32 / fp16 products (fp32-equivalent) -- all three must meet the fp32 parity bar.
 @pytest.mark.parametrize("precision", ["fp32", "3xtf32", "3xf16"])
 @pytest.mark.parametrize("name", CASES)
@@ -65,10 +65,8 @@ def test_encoder_matches_reference_golden(name, precision):
     # enc_pasep_train_4001 is bistable on top of that: one pre-activation of block 2/3 lies
     # within the run-to-run noise of the BatchNorm statistics (fp64 atomics, order-dependent in
     # the last bit) of zero.  When its gate flips, the gradients of blocks 0-2 move to exactly
-    # 7.19e-3 / 6.00e-3 / 6.95e-3 / 4.83e-3 (low_hz_, norm.weight, block-1 and block-2 weights)
-    # from the golden, otherwise they sit at 2e-6; blocks 4+ never move.  Measured in 1-3 of 6
-    # repetitions with every BatchNorm-backward variant of this repo (staged, register-resident,
-    # stored du; tools/gpu/debug_4001.py) -- with N=3 one gate is 0.5 % of a gradient norm.
+    # ~7e-3 (low_hz_, norm.weight, block-1 and block-2 weights) from the golden, otherwise
+    # they sit at 2e-6; blocks 4+ never move -- with N=3 one gate is 0.5 % of a gradient norm.
     l2_tol = 1.2e-2 if name == "enc_pasep_train_4001" else 5e-3
     assert check_grads(grads, gold, 2e-3, 2e-4,
                        l2_keys=() if precision == "fp32" else ("",), l2_tol=l2_tol) > 10

@@ -1,4 +1,4 @@
-"""tcgen05 / TMA GEMM kernels against the exact spec (the product of the operands as the
+"""wgmma / TMA GEMM kernels against the exact spec (the product of the operands as the
 tensor core reads them, accumulated in fp64).  Modes 1 (3xTF32) and 3 (3xF16) must be
 fp32-equivalent; mode 0 (TF32) and mode 2 (bf16) are exact products of rounded operands, so
 they too are checked tightly against the spec evaluated on the SAME rounded operands."""
@@ -90,7 +90,7 @@ def test_tc_gemm_nt(M, N, K, Rr, rows_in, t_valid, rows_out, fold, bias, stats, 
     torch.cuda.synchronize()
     scale = float((A.abs().mean() * B.abs().mean() * K ** 0.5))
     # split modes: fp32-equivalent; single-pass modes: exact products, fp32 accumulation in
-    # TMEM (round-toward-zero drift over K)
+    # the tensor core (rounding drift over K)
     tol = (2e-6 if mode in (1, 3) else 2e-5) * max(scale, 1e-3) * 8
     out_c, out_d = cpu[7], dev[7].cpu()
     err = float((out_c - out_d).abs().max())
@@ -106,7 +106,7 @@ def test_tc_gemm_nt(M, N, K, Rr, rows_in, t_valid, rows_out, fold, bias, stats, 
 @pytest.mark.parametrize("mode", [2, 3, 1])
 @pytest.mark.parametrize("M,N,K,Rr,rows_in,t_valid,rows_out,fold", [
     (1000, 64, 1280, 640, 103, 100, 100, 1),        # BN=64, 1-CTA
-    (700, 128, 704, 128, 70, 64, 64, 1),            # CTA pair
+    (700, 128, 704, 128, 70, 64, 64, 1),            # BN=128
     (520, 4096, 320, 64, 130, 8200, 129, 64),       # folded sinc (fold 64), wide N, stats
     (300, 256, 5632, 1024, 300, 300, 300, 1),       # 256-wide tiles (mode 2) / pair (mode 3)
 ])

@@ -1,12 +1,8 @@
 #!/usr/bin/env python
 """Per-launch table of the tensor-core GEMMs of one PASE+ encoder step (B=32, T=32000):
 shape, time (CUDA events around each launch, eager), fp32-equivalent TFLOP/s.  Meant for
-A/B runs of kernel variants selected by environment switches, e.g.
-
-    PASE_B200_TC_2CTA=0 python tools/gemm_table.py > gpurun_out/gemms_1cta.md
-    PASE_B200_TC_2CTA=1 python tools/gemm_table.py > gpurun_out/gemms_pair.md
-
-(the switches are read once per process by the library).  Needs a B200; `--precision`
+A/B runs of kernel variants selected by PASE_B200_* environment switches (read once per
+process by the library).  Needs a GPU; `--precision`
 as in bench.py.  Not part of the library; measurement helper only.
 """
 import argparse

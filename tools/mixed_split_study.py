@@ -1,7 +1,6 @@
 #!/usr/bin/env python
-"""CPU study for the next GEMM precision scheme (profiles/r01_history.md, "what is left"):
-keep the main product in TF32 and do the two error-compensation products of 3xTF32 in bf16
-(`kind::f16`, twice the tensor rate), i.e.
+"""CPU study for a GEMM precision scheme: keep the main product in TF32 and do the two
+error-compensation products of 3xTF32 in bf16 (twice the tensor rate), i.e.
 
     D = trunc_tf32(a) * rn_tf32(b)                       (tf32 pass, as today)
       + bf16(a - trunc_tf32(a)) * bf16(b)                (bf16 pass)

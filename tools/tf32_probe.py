@@ -1,4 +1,4 @@
-"""GPU probe: does kind::tf32 truncate or round its fp32 inputs?  (decides whether the
+"""GPU probe: does the tf32 tensor-core GEMM truncate or round its fp32 inputs?  (decides whether the
 'hi' operand of the 3xTF32 scheme could be the original array).  Prints one line."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -17,7 +17,7 @@ outs = []
 for a, b in ((A, B), (At, Bt)):
     C = torch.zeros(M * N).cuda()
     _lib.call("pase_tc_gemm_nt", a.cuda(), None, (M * K + 64) // K, K, b.cuda(), None, K, C, N, M, N, K,
-              1.0, None, M, M, M, 1, None, None, 0, 0)
+              1.0, None, None, M, M, M, 1, None, None, 0, 0, 0)
     outs.append(C.cpu())
 ref_t = (At[:M * K].view(M, K).double() @ Bt.view(N, K).double().t()).float().reshape(-1)
 ref_f = (A[:M * K].view(M, K).double() @ B.view(N, K).double().t()).float().reshape(-1)
