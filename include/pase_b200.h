@@ -97,6 +97,9 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
                     const void* Bhi, const void* Blo, int R, int pitchB, long b_rows_total,
                     float* C, long ldc, int I, int J, int groups, int rows_per_group,
                     float alpha, const float* alpha_dev, int accumulate, int mode, void* stream);
+/* How pase_tc_gemm_tn splits the reduction of this shape on the current device (host only):
+ * out2 = {splits, chunks_per_split}; a chunk is 32 reduction rows in modes 0/1, 64 in 2/3. */
+int pase_tc_gemm_tn_plan(int I, int J, int groups, int rows_per_group, int mode, int* out2);
 
 /* ---- operand-format conversions for GEMM modes 2 / 3 (small tensors) -------- */
 /* dst (bf16) = rn(x) */

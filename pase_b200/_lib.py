@@ -124,3 +124,14 @@ def device_info():
     if rc != 0:
         raise RuntimeError("pase_device_info failed: " + last_error())
     return {"sms": out[0], "cc": (out[1], out[2]), "smem_optin": out[3]}
+
+
+def tc_gemm_tn_plan(I, J, groups, rows_per_group, mode):
+    """(splits, chunks_per_split) of pase_tc_gemm_tn for this shape on the current device."""
+    out = (ctypes.c_int * 2)()
+    L = lib()
+    rc = L.pase_tc_gemm_tn_plan(I, J, groups, rows_per_group, mode,
+                                ctypes.cast(out, ctypes.c_void_p))
+    if rc != 0:
+        raise RuntimeError("pase_tc_gemm_tn_plan failed: " + last_error())
+    return out[0], out[1]

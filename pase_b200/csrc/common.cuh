@@ -39,6 +39,19 @@ static inline int pase_num_sms() {
   return sms;
 }
 
+// ---- split-K weight gradients (splitk.cu) ----
+// A split GEMM writes split z's partial tile t (128 x bn fp32, bn <= 128) at
+// ws + (z * tiles + t) * 128 * bn; pase_splitk_reduce sums the splits in split order into C
+// (C = sum, or C += sum when accumulating).  The workspace holds pase_splitk_ws_tiles() tiles
+// of PASE_SPLITK_TILE floats, so a launch needs splits * tiles <= pase_splitk_ws_tiles().
+// One workspace per device, shared by every split GEMM: calls must be ordered on one stream.
+#define PASE_SPLITK_WAVES 4
+#define PASE_SPLITK_TILE (128 * 128)
+long pase_splitk_ws_tiles();
+float* pase_splitk_workspace(cudaStream_t st, const char* who);
+int pase_splitk_reduce(const float* ws, int splits, int tiles_j, int bn, long tiles, float* C,
+                       long ldc, int I, int J, int accumulate, cudaStream_t st, const char* who);
+
 // ---- programmatic dependent launch (PDL) ----
 // Kernels launched through PASE_LAUNCH may be scheduled while the previous kernel of the stream
 // is still draining (graph capture turns this into a programmatic edge): launch latency, block

@@ -4,7 +4,8 @@
 //             forward conv / transposed conv / dgrad / linear layers.  A may be an
 //             overlapping-row view of a padded channel-last activation (lda < K).
 //   gemm_tn : C[i,j] += alpha * sum_r A[rowA(r)*lda+i] * B[rowB(r)*ldb+j]
-//             weight gradients (split over the reduction, fp32 red.add epilogue).
+//             weight gradients (split over the reduction; the splits' partial tiles are
+//             summed in split order, so the result does not depend on thread scheduling).
 //
 // 128 x BN x 16 CTA tile, 256 threads, 8 x (BN/16) register tile per thread,
 // global->register prefetch of the next k-slab overlapped with the FFMA loop.
@@ -217,7 +218,7 @@ template <int BN>
 __global__ void __launch_bounds__(NT, 2)
 gemm_tn_kernel(const float* __restrict__ A, long lda, const float* __restrict__ B, long ldb,
                float* __restrict__ C, long ldc, int I, int J, RedMap rm, float alpha,
-               long rows_per_split) {
+               long rows_per_split, int accumulate, float* __restrict__ ws) {
   constexpr int TN = BN / 16;
   constexpr int BQ = BN / 64;            // float4 per thread per 16-row slab: BN*16/4/256
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -313,15 +314,25 @@ gemm_tn_kernel(const float* __restrict__ A, long lda, const float* __restrict__ 
     }
   }
 
+  // one split: straight into C (every element has exactly one writer).  Several splits: into
+  // this split's partial tile, summed in split order by pase_splitk_reduce
+  float* tile = ws == nullptr ? nullptr
+      : ws + (((long)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * (BM * BN);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const int ii = i0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
-    if (ii >= I) continue;
+    const int r = i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4);
+    if (i0 + r >= I) continue;
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
-      const int jj = j0 + (j < 4 ? tx * 4 + j : (BN / 2) + tx * 4 + (j - 4));
-      if (jj >= J) continue;
-      atomicAdd(C + (long)ii * ldc + jj, acc[i][j] * alpha);
+      const int c = j < 4 ? tx * 4 + j : (BN / 2) + tx * 4 + (j - 4);
+      if (j0 + c >= J) continue;
+      const float v = acc[i][j] * alpha;
+      if (tile != nullptr) {
+        tile[r * BN + c] = v;
+      } else {
+        float* p = C + (long)(i0 + r) * ldc + j0 + c;
+        *p = accumulate ? *p + v : v;
+      }
     }
   }
 }
@@ -346,7 +357,7 @@ int launch_nt(const float* A, long lda, const float* B, long ldb, float* C, long
 
 template <int BN>
 int launch_tn(const float* A, long lda, const float* B, long ldb, float* C, long ldc, int I,
-              int J, RedMap rm, float alpha, cudaStream_t st) {
+              int J, RedMap rm, float alpha, int accumulate, cudaStream_t st) {
   static bool attr_set = false;
   const size_t smem = sizeof(SmemTN<BN>);
   if (!attr_set) {
@@ -355,17 +366,28 @@ int launch_tn(const float* A, long lda, const float* B, long ldb, float* C, long
     attr_set = true;
   }
   const int ti = (I + BM - 1) / BM, tj = (J + BN - 1) / BN;
+  const long tiles = (long)ti * tj;
   const int target = 3 * pase_num_sms();
-  long splits = (target + ti * tj - 1) / (ti * tj);
+  long splits = (target + tiles - 1) / tiles;
   long max_splits = (rm.total_rows + 4 * BK - 1) / (4 * BK);
   if (splits > max_splits) splits = max_splits;
+  // the partial tiles must fit the workspace: ceil(3 sms / tiles) * tiles exceeds it for
+  // 2 sms < tiles < 3 sms
+  if (splits * tiles > pase_splitk_ws_tiles()) splits = pase_splitk_ws_tiles() / tiles;
   if (splits < 1) splits = 1;
   long rps = (rm.total_rows + splits - 1) / splits;
   rps = ((rps + BK - 1) / BK) * BK;
-  splits = (rm.total_rows + rps - 1) / rps;
+  splits = (rm.total_rows + rps - 1) / rps;     // no empty split
+  float* ws = nullptr;
+  if (splits > 1 && (ws = pase_splitk_workspace(st, "pase_gemm_tn")) == nullptr)
+    return PASE_ERR_UNSUPPORTED;
   dim3 grid(tj, ti, (unsigned)splits);
-  gemm_tn_kernel<BN><<<grid, NT, smem, st>>>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, rps);
+  gemm_tn_kernel<BN><<<grid, NT, smem, st>>>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, rps,
+                                            accumulate, ws);
   PASE_LAUNCH_CHECK("pase_gemm_tn");
+  if (splits > 1)
+    return pase_splitk_reduce(ws, (int)splits, tj, BN, tiles, C, ldc, I, J, accumulate, st,
+                              "pase_gemm_tn");
   return PASE_OK;
 }
 
@@ -408,15 +430,7 @@ extern "C" int pase_gemm_tn(const float* A, long lda, int pitchA, int offA, cons
                  lda, ldb, I, J);
   PASE_CHECK_ARG(aligned16(A) && aligned16(B), "pase_gemm_tn: A/B must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  if (!accumulate) {
-    cudaError_t e = cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)J * sizeof(float),
-                                      (size_t)I, st);
-    if (e != cudaSuccess) {
-      pase_set_error("pase_gemm_tn: memset failed: %s", cudaGetErrorString(e));
-      return (int)e;
-    }
-  }
   RedMap rm{rows_per_group, pitchA, offA, pitchB, offB, (long)groups * rows_per_group};
-  if (J <= 64) return launch_tn<64>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, st);
-  return launch_tn<128>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, st);
+  if (J <= 64) return launch_tn<64>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, accumulate, st);
+  return launch_tn<128>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, accumulate, st);
 }

@@ -656,7 +656,7 @@ struct TNArgs {
   float alpha;
   const float* alpha_dev;
   int chunks_per_split, flush_ch, stages, b_blocked, accumulate;
-  float* ws;                       // several splits: [split][tile][BM x BN] partial tiles
+  float* ws;                       // several splits: [split][tile][BM x BN] partial tiles (splitk.cu)
 };
 
 // fp32 stage operand [rows/32 blocks of (32 k-rows x 32 elements)] -> K-major 128B-swizzled
@@ -673,7 +673,7 @@ __device__ __forceinline__ void transpose_tile(const float* __restrict__ src, fl
 
 // alpha * (this warp's 16 tile rows starting at r0).  One split: straight into C (C = x, or
 // C += x when accumulating; every element has exactly one writer).  Several splits: into this
-// split's partial tile in the workspace, which tn_reduce_splits_kernel sums in split order, so
+// split's partial tile in the workspace, which pase_splitk_reduce sums in split order, so
 // the result does not depend on the order in which the splits finish.
 template <int BN, int NR>
 __device__ __forceinline__ void tn_output(const float (&v)[NR], const TNArgs& a, int r0, int i0,
@@ -708,21 +708,6 @@ __device__ __forceinline__ void tn_output(const float (&v)[NR], const TNArgs& a,
       }
     }
   }
-}
-
-// C[i, j] (+)= sum over the splits, in split order, of the partial tiles holding (i, j)
-__global__ void tn_reduce_splits_kernel(const float* __restrict__ ws, int splits, int tiles_j,
-                                        int bn, long tiles, float* __restrict__ C, long ldc, int I,
-                                        int J, int accumulate) {
-  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (long)I * J) return;
-  const int i = (int)(idx / J), j = (int)(idx % J);
-  const long tile_elems = (long)BM * bn;
-  const float* p = ws + ((long)(i / BM) * tiles_j + j / bn) * tile_elems + (i % BM) * bn + j % bn;
-  float sum = 0.f;
-  for (int z = 0; z < splits; ++z) sum += p[z * tiles * tile_elems];
-  float* c = C + (long)i * ldc + j;
-  *c = accumulate ? *c + sum : sum;
 }
 
 template <int BN, int MODE>
@@ -989,36 +974,41 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
   return PASE_OK;
 }
 
-// Partial tiles of the split weight-gradient GEMM: room for 4 CTAs per SM of BM x 128 fp32,
-// allocated once per device on first use (never freed: captured CUDA graphs keep using it).
-static float* tn_workspace(cudaStream_t st) {
-  static float* ws[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) {
-    pase_set_error("pase_tc_gemm_tn: device index %d", dev);
-    return nullptr;
+// How pase_tc_gemm_tn splits its reduction: the split count and the chunks (stages of KR
+// rows) per split.  The CTA count should fill whole waves of the SMs (one CTA per SM): among
+// 1..PASE_SPLITK_WAVES waves pick the split with the best fill, keeping chains >= 8 chunks.
+struct TNPlan {
+  int bn;
+  long tiles_j, tiles, splits, chunks_per_split;
+};
+TNPlan tn_split_plan(int I, int J, int groups, int rows_per_group, int mode) {
+  TNPlan p;
+  const int kr = 4 * 32 / (mode >= 2 ? 2 : 4);
+  p.bn = J <= 64 ? 64 : 128;
+  p.tiles_j = (J + p.bn - 1) / p.bn;
+  p.tiles = (long)((I + BM - 1) / BM) * p.tiles_j;
+  const long total = (long)groups * ((rows_per_group + kr - 1) / kr);
+  const int sms = pase_num_sms();
+  long best = 1;
+  double best_eff = -1.0;
+  for (long sp = 1; sp <= total && sp * p.tiles <= pase_splitk_ws_tiles(); ++sp) {
+    const long cps_try = (total + sp - 1) / sp;
+    if (cps_try < 8 && sp > 1) break;
+    const long ctas = p.tiles * ((total + cps_try - 1) / cps_try);
+    const long waves = (ctas + sms - 1) / sms;
+    // time ~ waves * chunks-per-cta: lower is better
+    const double cost = (double)waves * (double)(cps_try + 6);
+    const double eff = 1.0 / cost;
+    if (eff > best_eff) { best_eff = eff; best = sp; }
   }
-  if (ws[dev] != nullptr) return ws[dev];
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(st, &cs);
-  if (cs != cudaStreamCaptureStatusNone) {
-    pase_set_error("pase_tc_gemm_tn: first split-K call on this device inside a stream capture "
-                   "(run one step before capturing)");
-    return nullptr;
-  }
-  cudaError_t e = cudaMalloc(&ws[dev], (size_t)4 * pase_num_sms() * BM * 128 * sizeof(float));
-  if (e != cudaSuccess) {
-    ws[dev] = nullptr;
-    pase_set_error("pase_tc_gemm_tn: workspace allocation: %s", cudaGetErrorString(e));
-    return nullptr;
-  }
-  return ws[dev];
+  p.chunks_per_split = (total + best - 1) / best;
+  p.splits = (total + p.chunks_per_split - 1) / p.chunks_per_split;   // no empty split
+  return p;
 }
 
 template <int BN, int MODE>
 int launch_tn(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
-              const CUtensorMap& bl, TNArgs a, cudaStream_t st) {
+              const CUtensorMap& bl, TNArgs a, int mode, cudaStream_t st) {
   using Cfg = TNCfg<BN, MODE>;
   static bool attr = false;
   a.stages = pick_stages(Cfg::STAGE_BYTES, Cfg::T_BYTES);
@@ -1032,42 +1022,19 @@ int launch_tn(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
     }
     attr = true;
   }
-  const int ti = (a.I + BM - 1) / BM, tj = (a.J + BN - 1) / BN;
-  const int cpg = (a.rows_per_group + Cfg::KR - 1) / Cfg::KR;
-  const long total = (long)a.groups * cpg;
-  // split the reduction so that the CTA count fills whole waves of the SMs (one CTA per SM):
-  // among 1..4 waves pick the split with the best fill, keeping chains >= 8 chunks
-  const long tiles = (long)ti * tj;
-  const int sms = pase_num_sms();
-  long best = 1;
-  double best_eff = -1.0;
-  for (long sp = 1; sp <= total && sp * tiles <= 4L * sms; ++sp) {
-    const long cps_try = (total + sp - 1) / sp;
-    if (cps_try < 8 && sp > 1) break;
-    const long ctas = tiles * ((total + cps_try - 1) / cps_try);
-    const long waves = (ctas + sms - 1) / sms;
-    // time ~ waves * chunks-per-cta: lower is better
-    const double cost = (double)waves * (double)(cps_try + 6);
-    const double eff = 1.0 / cost;
-    if (eff > best_eff) { best_eff = eff; best = sp; }
-  }
-  long splits = best;
-  long cps = (total + splits - 1) / splits;
-  splits = (total + cps - 1) / cps;
-  a.chunks_per_split = (int)cps;
+  const TNPlan p = tn_split_plan(a.I, a.J, a.groups, a.rows_per_group, mode);
+  a.chunks_per_split = (int)p.chunks_per_split;
   a.ws = nullptr;
-  if (splits > 1) {      // splits * tiles <= 4 * sms CTAs (loop above): fits the workspace
-    if ((a.ws = tn_workspace(st)) == nullptr) return PASE_ERR_UNSUPPORTED;
+  if (p.splits > 1) {    // splits * tiles <= pase_splitk_ws_tiles() (tn_split_plan)
+    if ((a.ws = pase_splitk_workspace(st, "pase_tc_gemm_tn")) == nullptr)
+      return PASE_ERR_UNSUPPORTED;
   }
-  dim3 grid(tj, ti, (unsigned)splits);
+  dim3 grid((unsigned)p.tiles_j, (unsigned)(p.tiles / p.tiles_j), (unsigned)p.splits);
   PASE_LAUNCH((tc_gemm_tn_kernel<BN, MODE>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
   PASE_TC_LAUNCH_CHECK("pase_tc_gemm_tn");
-  if (splits > 1) {
-    const long n = (long)a.I * a.J;
-    tn_reduce_splits_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-        a.ws, (int)splits, tj, BN, tiles, a.C, a.ldc, a.I, a.J, a.accumulate);
-    PASE_TC_LAUNCH_CHECK("pase_tc_gemm_tn (split reduction)");
-  }
+  if (p.splits > 1)
+    return pase_splitk_reduce(a.ws, (int)p.splits, (int)p.tiles_j, BN, p.tiles, a.C, a.ldc, a.I,
+                              a.J, a.accumulate, st, "pase_tc_gemm_tn");
   return PASE_OK;
 }
 
@@ -1310,14 +1277,24 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
   a.accumulate = accumulate; a.ws = nullptr;
 #define PASE_TN(BNV)                                                      \
   switch (mode) {                                                         \
-    case 0: return launch_tn<BNV, 0>(ah, al, bh, bl, a, st);              \
-    case 1: return launch_tn<BNV, 1>(ah, al, bh, bl, a, st);              \
-    case 2: return launch_tn<BNV, 2>(ah, al, bh, bl, a, st);              \
-    default: return launch_tn<BNV, 3>(ah, al, bh, bl, a, st);             \
+    case 0: return launch_tn<BNV, 0>(ah, al, bh, bl, a, 0, st);           \
+    case 1: return launch_tn<BNV, 1>(ah, al, bh, bl, a, 1, st);           \
+    case 2: return launch_tn<BNV, 2>(ah, al, bh, bl, a, 2, st);           \
+    default: return launch_tn<BNV, 3>(ah, al, bh, bl, a, 3, st);          \
   }
   if (BN == 64) { PASE_TN(64) }
   PASE_TN(128)
 #undef PASE_TN
+}
+
+int pase_tc_gemm_tn_plan(int I, int J, int groups, int rows_per_group, int mode, int* out2) {
+  PASE_CHECK_ARG(out2 && I > 0 && J > 0 && groups > 0 && rows_per_group > 0 && mode >= 0 &&
+                     mode <= 3,
+                 "pase_tc_gemm_tn_plan: bad args");
+  const TNPlan p = tn_split_plan(I, J, groups, rows_per_group, mode);
+  out2[0] = (int)p.splits;
+  out2[1] = (int)p.chunks_per_split;
+  return PASE_OK;
 }
 
 }  // extern "C"

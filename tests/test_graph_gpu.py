@@ -53,10 +53,12 @@ def test_graphed_step_matches_eager(split):
         # the capture itself does not execute; replays do
         l1 = gs.step()
         l2 = gs.step()
-        assert abs(l1 - eager_losses[3]) <= 5e-4 * abs(eager_losses[3]) + 1e-6
-        assert abs(l2 - eager_losses[4]) <= 5e-4 * abs(eager_losses[4]) + 1e-6
+        # the same kernels in the same order, and no sum depends on thread scheduling: the
+        # replayed steps reproduce the eager steps bit for bit
+        assert l1 == eager_losses[3] and l2 == eager_losses[4], (l1, l2, eager_losses[3:])
         assert abs(eager_losses[4] - eager_losses[3]) > 1e-3 * abs(eager_losses[3])   # loss moves
         for (k, pe), (_, pg) in zip(me.named_parameters(), mg.named_parameters()):
-            assert rel_l2(pg.detach().cpu(), pe.detach().cpu()) < 2e-3, k
+            assert torch.equal(pg.detach(), pe.detach()), \
+                (k, rel_l2(pg.detach().cpu(), pe.detach().cpu()))
     finally:
         torch.cuda.set_stream(torch.cuda.default_stream())

@@ -17,6 +17,36 @@ def test_pase_workers_match_reference_golden(name):
     check_case(gold, meta, model, batch, "cuda", rtol=1e-3, atol=1e-5)
 
 
+@pytest.mark.parametrize("precision", ["fp32", "3xf16"])
+def test_pase_workers_step_is_reproducible(precision):
+    """Two identical forward + backward passes of the PASE+ encoder with its worker heads give
+    the same loss and the same gradient bits (no sum in the step depends on scheduling)."""
+    import random
+    from pase_b200.pase import total_loss
+    from pase_b200 import functional as Fn
+    prev = Fn.PRECISION
+    Fn.set_precision(precision)
+    try:
+        gold, meta, model, batch = build_case("pase_plus_workers_3200", "cuda")
+        model.frontend.precision = precision
+        runs = []
+        for _ in range(2):
+            random.seed(meta["seed"])
+            torch.manual_seed(meta["seed"])
+            model.zero_grad(set_to_none=True)
+            h, chunk, preds, labels = model(batch, 1, "cuda")
+            tot, _ = total_loss(model, preds, labels)
+            tot.backward()
+            runs.append((tot.detach().clone(),
+                         {k: p.grad.clone() for k, p in model.named_parameters()}))
+    finally:
+        Fn.set_precision(prev)
+    (t1, g1), (t2, g2) = runs
+    assert torch.equal(t1, t2), (float(t1), float(t2))
+    for k in g1:
+        assert torch.equal(g1[k], g2[k]), k
+
+
 def test_mlp_minion_accepts_reference_layout_tensors():
     """A (B,C,T) tensor that did not come from the encoder goes through the NCT->rows kernel."""
     torch.manual_seed(0)

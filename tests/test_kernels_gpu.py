@@ -62,6 +62,11 @@ def test_gemm_nt(M, N, K, lda, rows_in, t_valid, rows_out, fold, bias, stats, ac
     (256, 256, 2, 500, 256, 500, 0, 4, 520, 0, 0),
     (100, 1920, 1, 77, 100, 77, 0, 1920, 77, 0, 1),
     (512, 64, 4, 33, 512, 40, 5, 64, 33, 0, 0),
+    (128, 704, 4, 1600, 128, 1610, 5, 704, 1605, 3, 1),     # ~66 splits, accumulate
+    (100, 60, 3, 900, 100, 905, 2, 60, 903, 1, 0),          # BN=64 tile, tails, splits
+    # 16 x 17 = 272 tiles: ceil(3 SMs / tiles) = 2 splits would overflow the 4 x SMs-tile
+    # workspace on a 132-SM H100; the launcher keeps splits x tiles within it
+    (2048, 2176, 2, 128, 2048, 130, 1, 2176, 129, 0, 0),
 ])
 def test_gemm_tn(I, J, groups, rpg, lda, pitchA, offA, ldb, pitchB, offB, acc):
     A = R(groups * pitchA * lda + I + 8, seed=5)
@@ -69,6 +74,130 @@ def test_gemm_tn(I, J, groups, rpg, lda, pitchA, offA, ldb, pitchB, offB, acc):
     C = R(I * J, seed=7)
     run_both("pase_gemm_tn", [A, lda, pitchA, offA, B, ldb, pitchB, offB, C, J, I, J, groups, rpg,
                               0.25, acc], rtol=2e-4, atol=2e-5)
+
+
+# ---- run-to-run reproducibility: the same computation twice on identical inputs ----
+def _twice(name, args, outs):
+    """Run `name` twice on fresh device copies of args; -> the two lists of outputs."""
+    res = []
+    for _ in range(2):
+        dev = [a.cuda() if isinstance(a, torch.Tensor) else a for a in args]
+        _lib.call(name, *dev)
+        res.append([dev[i] for i in outs])
+    torch.cuda.synchronize()
+    return res
+
+
+def _same_fp64(a, b):
+    """fp64 accumulators: equal to 1e-14, and equal once rounded to fp32 (what consumers use)."""
+    assert float((a - b).abs().max()) <= 1e-14 * float(a.abs().max())
+    assert torch.equal(a.float(), b.float())
+
+
+def test_gemm_tn_is_reproducible():
+    I, J, groups, rpg, lda, pitchA, offA, ldb, pitchB = 128, 704, 4, 1600, 128, 1610, 5, 704, 1605
+    A = R(groups * pitchA * lda + I + 8, seed=61)
+    B = R(groups * pitchB * ldb + J + 8, seed=62)
+    (c1,), (c2,) = _twice("pase_gemm_tn", [A, lda, pitchA, offA, B, ldb, pitchB, 0,
+                                           torch.zeros(I * J), J, I, J, groups, rpg, 1.0, 0], [8])
+    assert torch.equal(c1, c2)
+
+
+def test_bn_prelu_bwd_and_colsum_are_reproducible():
+    N, T, C, padL, padR, pool_d = 4, 1603, 128, 5, 5, 8
+    Tp = T + padL + padR
+    y = R(N * T * C, seed=63)
+    mean, invstd = R(C, seed=64, scale=0.1), R(C, seed=65).abs() + 0.5
+    scale, shift, alpha = R(C, seed=66), R(C, seed=67), R(C, seed=68, scale=0.3)
+    pool_T = T // pool_d
+    args = [y, 0, T * C, N, T, C, mean, invstd, scale, shift, alpha, R(N * Tp * C, seed=69), 0,
+            Tp * C, C, padL, padR, None, 0, 0, 0, R(N * pool_T * C, seed=70), pool_T * C, C,
+            pool_d, pool_T, torch.zeros(N * T * C), T * C] + \
+        [torch.zeros(C, dtype=torch.float64) for _ in range(3)] + [torch.zeros(2)]
+    r1, r2 = _twice("pase_bn_prelu_bwd_reduce", args, [26, 28, 29, 30, 31])
+    assert torch.equal(r1[0], r2[0]) and torch.equal(r1[4], r2[4])
+    for a, b in zip(r1[1:4], r2[1:4]):
+        _same_fp64(a, b)
+    outs = []
+    for du, s1, s2 in ((r1[0], r1[1], r1[2]), (r2[0], r2[1], r2[2])):
+        dy = torch.zeros_like(du)
+        db = torch.zeros(C, dtype=torch.float64, device="cuda")
+        _lib.call("pase_bn_prelu_bwd_apply", y.cuda(), 0, T * C, N, T, C, mean.cuda(),
+                  invstd.cuda(), R(C, seed=71).cuda(), s1, s2, float(N * T), du, dy, None, 0,
+                  T * C, db, None, None)
+        outs.append((dy, db))
+    torch.cuda.synchronize()
+    assert torch.equal(outs[0][0], outs[1][0])
+    _same_fp64(outs[0][1], outs[1][1])
+    rows = 20000
+    (s1,), (s2,) = _twice("pase_colsum", [R(rows * 520, seed=72), 520, rows, 517,
+                                          torch.zeros(517, dtype=torch.float64)], [4])
+    _same_fp64(s1, s2)
+
+
+# ---- small helpers of the 3xF16 gradient scaling and of the flat-gradient packing ----
+def test_bound_scale_bit_exact():
+    """{1/s, s} with s the power of two placing 1.0001 x (a0 a1 + a2 + a3) below 2^14,
+    including bounds that are exact powers of two, zero and tiny / huge bounds."""
+    for a4 in ([2.0, 4.0, 0.0, 0.0], [0.5, 0.5, 0.0, 0.0], [1.0, 2.0 ** -20, 0.0, 0.0],
+               [2.0 ** 14, 1.0, 0.0, 0.0], [1.0, 1.0, 2.0 ** 15, 2.0 ** 15], [3.0, 5.0, 1.0, 0.5],
+               [0.0, 0.0, 0.0, 0.0], [1e-20, 1e-10, 0.0, 0.0], [1e19, 1e19, 0.0, 0.0],
+               [0.1, 0.3, 7.0, 1e-3]):
+        cpu, dev = run_both("pase_bound_scale", [torch.tensor(a4), torch.zeros(2)], rtol=0, atol=0)
+        assert torch.equal(cpu[1], dev[1].cpu()), (a4, cpu[1], dev[1])
+
+
+@pytest.mark.parametrize("rows,cols,ld", [(1, 1, 1), (300, 37, 40), (1000, 1001, 1003),
+                                          (64, 4, 4), (5000, 99, 128)])
+def test_rownorm_max(rows, cols, ld):
+    """max_r ||X[r, :cols]|| over rows spanning 20 decades, with in-row spikes; cols not a
+    multiple of 4 and ld > cols (the padding holds large values that must be ignored)."""
+    g = torch.Generator().manual_seed(rows + cols)
+    X = torch.randn(rows, ld, generator=g)
+    X *= 10.0 ** torch.randint(-10, 10, (rows, 1), generator=g).float()
+    X[::7, 0] *= 1e4
+    X[:, cols:] = 1e30
+    for prior in (0.0, float(X[:, :cols].double().norm(dim=1).max()) * 2):
+        amax = torch.tensor([prior])
+        cpu, dev = run_both("pase_rownorm_max", [X.reshape(-1), ld, rows, cols, amax],
+                            rtol=1e-5, atol=0)
+        if prior:
+            assert float(dev[4][0]) == float(amax[0])
+
+
+@pytest.mark.parametrize("njobs", [7, 128])
+def test_scatter_copy(njobs):
+    """Strided 2-D copies of several shapes in one launch (128 = the table's capacity); the
+    guard elements between destinations stay untouched."""
+    g = torch.Generator().manual_seed(njobs)
+    shapes = [(1, 1, 1, 1), (3, 5, 7, 6), (17, 33, 40, 35), (64, 100, 100, 100),
+              (2, 1000, 1003, 1001), (1, 4097, 4097, 4097), (9, 2, 2, 9)]
+    while len(shapes) < njobs:
+        r, c = (int(v) for v in torch.randint(1, 40, (2,), generator=g))
+        shapes.append((r, c, c + int(torch.randint(0, 4, (1,), generator=g)),
+                       c + int(torch.randint(0, 4, (1,), generator=g))))
+    so, do, s_off, d_off = 0, 0, [], []
+    for (r, c, sl, dl) in shapes:
+        s_off.append(so)
+        d_off.append(do + 3)                       # 3 guard elements before every destination
+        so += (r - 1) * sl + c + 5
+        do += 3 + (r - 1) * dl + c + 3
+    src = torch.randn(so, generator=g)
+    dst = torch.full((do,), -7.0)
+    ref = dst.clone()
+    srcd, dstd = src.cuda(), dst.cuda()
+    total = sum(r * c for (r, c, _, _) in shapes)
+
+    def table(s, d):
+        return torch.tensor([[s.data_ptr() + 4 * so_, d.data_ptr() + 4 * do_, r, c, sl, dl]
+                             for (r, c, sl, dl), so_, do_ in zip(shapes, s_off, d_off)],
+                            dtype=torch.int64).reshape(-1)
+    emul_ops.pase_scatter_copy(table(src, ref), njobs, total)
+    _lib.call("pase_scatter_copy", table(srcd, dstd).cuda(), njobs, total)
+    torch.cuda.synchronize()
+    out = dstd.cpu()
+    assert torch.equal(out, ref)
+    assert int((out == -7.0).sum()) == do - total
 
 
 def test_weight_layouts():
