@@ -253,6 +253,23 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
                                 void* dst, void* dst_lo, int dst_fmt, long dst_sample_stride,
                                 double* dbias_acc, const float* amax, float* scale_out,
                                 void* stream);
+/* The three backward entry points above read and write y, srcA, srcB, pool, dst, dst_lo and du
+ * in quads of channels: fp32 operands must be 16-byte aligned, 16-bit ones 8-byte aligned,
+ * every row and sample stride a multiple of 4 elements, a/b_row_stride >= C and
+ * pool_T * pool_d <= T; anything else is refused (PASE_ERR_ARG) before a launch.
+ * How pass 1 (pase_bn_prelu_bwd_reduce) or pass 2 (pase_bn_prelu_bwd_apply_src; srcA NULL:
+ * pase_bn_prelu_bwd_apply with a stored du) runs with these arguments on the current device
+ * (host only, launches nothing; arguments as in those calls, dst_lo / dst_fmt only in pass 2):
+ * out4 = {path (0: register kernels, 1: staged persistent kernels), time steps per work item
+ * (steps per thread or tile rows), work items of all samples (thread runs of one channel
+ * quad, or tiles), blocks of the launch (256 threads each)}. */
+int pase_bn_bwd_plan(int pass, const void* y, int y_bf16, long y_sample_stride, int N, int T,
+                     int C, const void* srcA, int a_bf16, long a_sample_stride,
+                     long a_row_stride, int padL, int padR,
+                     const float* srcB, long b_sample_stride, long b_row_stride, int b_shift,
+                     const float* pool, long pool_sample_stride, long pool_row_stride,
+                     int pool_d, int pool_T,
+                     void* dst, void* dst_lo, int dst_fmt, long dst_sample_stride, long* out4);
 /* plain per-channel PReLU on (rows,C) (MLPBlock / GDeconv1DBlock act) */
 int pase_prelu_fwd(const float* u, float* h, const float* alpha, long rows, int C,
                    long ldu, long ldh, void* stream);

@@ -135,3 +135,12 @@ def tc_gemm_tn_plan(I, J, groups, rows_per_group, mode):
     if rc != 0:
         raise RuntimeError("pase_tc_gemm_tn_plan failed: " + last_error())
     return out[0], out[1]
+
+
+def bn_bwd_plan(pass_, *args):
+    """How a BatchNorm/PReLU backward pass runs on the current device: `args` as the
+    pase_bn_bwd_plan arguments after `pass` up to dst_sample_stride (tensors or device
+    pointers).  -> dict(path=0 register / 1 staged, rows, items, grid)."""
+    out = (ctypes.c_long * 4)()
+    call("pase_bn_bwd_plan", pass_, *args, ctypes.addressof(out))
+    return {"path": out[0], "rows": out[1], "items": out[2], "grid": out[3]}

@@ -781,6 +781,106 @@ inline unsigned blocks_for(long total, int threads, int cap_mult = 8) {
   return (unsigned)b;
 }
 
+// The operands of one BatchNorm/PReLU backward call (fields the entry point does not take
+// stay zero / NULL).
+BnStreamArgs bn_bwd_args(const void* y, int y_bf16, long y_ss, int N, int T, int C,
+                         const void* srcA, int a_bf16, long a_ss, long a_rs, int padL, int padR,
+                         const float* srcB, long b_ss, long b_rs, int b_shift, const float* pool,
+                         long p_ss, long p_rs, int pool_d, int pool_T, void* dst, void* dst_lo,
+                         int dst_fmt, long d_ss) {
+  BnStreamArgs a{};
+  a.y = y; a.y_bf16 = y_bf16; a.y_ss = y_ss; a.N = N; a.T = T; a.C = C;
+  a.s = BwdSrc{srcA, a_ss, a_rs, padL, padR, srcB, b_ss, b_rs, b_shift,
+               pool, p_ss, p_rs, pool ? pool_d : 0, pool_T};
+  a.a_bf16 = a_bf16;
+  a.dst = dst; a.dst_lo = dst_lo; a.dst_fmt = dst_fmt; a.d_ss = d_ss;
+  return a;
+}
+
+// Which kernel runs a backward pass and how it is cut (also reported by pase_bn_bwd_plan).
+//   pass 1 (pase_bn_prelu_bwd_reduce): staged when it writes only its sums (dst == NULL) and
+//     pase_bn_stream_ok accepts the operands;
+//   pass 2 (pase_bn_prelu_bwd_apply_src): staged when, in addition, dst / dst_lo take the
+//     staged kernel's 16-byte stores; srcA == NULL: pase_bn_prelu_bwd_apply (stored du),
+//     always the register kernel.
+// Register kernels: one thread per run of `rows` time steps of a channel quad; when the
+// grid stride keeps each thread on its channel quad, the grid is capped and threads loop.
+struct BnBwdPlan {
+  int path, rows;       // 0 register / 1 staged; time steps per work item
+  long items, gx;       // work items (thread runs or tiles) of all samples; blocks per sample
+  long blocks;          // blocks of the launch
+};
+
+BnBwdPlan bn_bwd_plan(const BnStreamArgs& a, int pass) {
+  BnBwdPlan p{};
+  bool staged = a.s.A != nullptr && pase_bn_stream_ok(a);
+  if (pass == 1)
+    staged = staged && a.dst == nullptr;
+  else
+    staged = staged && (a.d_ss % 8) == 0 && aligned16(a.dst) &&
+             (a.dst_lo == nullptr || aligned16(a.dst_lo));
+  if (staged) {
+    const BnStreamPlan sp = pase_bn_stream_plan(a);
+    p.path = 1; p.rows = sp.TT; p.items = sp.total; p.gx = sp.grid; p.blocks = sp.grid;
+    return p;
+  }
+  const int RUN = bn_run();
+  const long threads = (long)(a.C / 4) * ((a.T + RUN - 1) / RUN);
+  long gx = (threads + THREADS - 1) / THREADS;
+  if ((THREADS % (a.C / 4)) == 0) {          // stride keeps the channel quad: cap the grid
+    long cap = ((RUN == 8 ? 8L : 16L) * pase_num_sms() + a.N - 1) / a.N;
+    if (cap < 1) cap = 1;
+    if (gx > cap) gx = cap;
+  }
+  p.path = 0; p.rows = RUN; p.items = threads * a.N; p.gx = gx; p.blocks = gx * a.N;
+  return p;
+}
+
+// The register kernels read and write every operand in quads of channels (a float4, or four
+// 16-bit values in 8 bytes): pointers must be aligned to the quad's size and every row and
+// sample stride must hold whole quads, else a kernel faults on a misaligned address.
+#define PASE_CHECK_QUAD(fn, p, esz, name)                                                   \
+  PASE_CHECK_ARG(((reinterpret_cast<uintptr_t>(p)) & (4u * (esz) - 1u)) == 0,                \
+                 "%s: %s must be %d-byte aligned", fn, name, 4 * (int)(esz))
+#define PASE_CHECK_STRIDE(fn, v, name)                                                      \
+  PASE_CHECK_ARG(((v) % 4) == 0, "%s: %s=%ld must be a multiple of 4", fn, name, (long)(v))
+
+// Checks of the operands of the three backward entry points, before any launch.  dst: du
+// (pass 1, type of y) or dy (pass 2, format dst_fmt); du: the stored du of
+// pase_bn_prelu_bwd_apply.
+int bn_bwd_check(const char* fn, const BnStreamArgs& a, int pass, const void* du) {
+  const int ysz = a.y_bf16 ? 2 : 4;
+  PASE_CHECK_QUAD(fn, a.y, ysz, "y");
+  PASE_CHECK_STRIDE(fn, a.y_ss, "y_sample_stride");
+  if (a.s.A) {
+    PASE_CHECK_QUAD(fn, a.s.A, a.a_bf16 ? 2 : 4, "srcA");
+    PASE_CHECK_STRIDE(fn, a.s.a_ss, "a_sample_stride");
+    PASE_CHECK_STRIDE(fn, a.s.a_rs, "a_row_stride");
+    PASE_CHECK_ARG(a.s.a_rs >= a.C, "%s: a_row_stride=%ld < C=%d", fn, a.s.a_rs, a.C);
+  }
+  if (a.s.B) {
+    PASE_CHECK_QUAD(fn, a.s.B, 4, "srcB");
+    PASE_CHECK_STRIDE(fn, a.s.b_ss, "b_sample_stride");
+    PASE_CHECK_STRIDE(fn, a.s.b_rs, "b_row_stride");
+    PASE_CHECK_ARG(a.s.b_rs >= a.C, "%s: b_row_stride=%ld < C=%d", fn, a.s.b_rs, a.C);
+  }
+  if (a.s.P && a.s.pool_d != 0) {
+    PASE_CHECK_QUAD(fn, a.s.P, 4, "pool");
+    PASE_CHECK_STRIDE(fn, a.s.p_ss, "pool_sample_stride");
+    PASE_CHECK_STRIDE(fn, a.s.p_rs, "pool_row_stride");
+    PASE_CHECK_ARG(a.s.pool_d > 0 && a.s.pool_T >= 0 && (long)a.s.pool_T * a.s.pool_d <= a.T,
+                   "%s: pool_T=%d x pool_d=%d exceeds T=%d", fn, a.s.pool_T, a.s.pool_d, a.T);
+  }
+  const int dsz = pass == 1 ? ysz : (a.dst_fmt == PASE_FMT_F32 ? 4 : 2);
+  if (a.dst) {
+    PASE_CHECK_QUAD(fn, a.dst, dsz, "dst");
+    PASE_CHECK_STRIDE(fn, a.d_ss, "dst_sample_stride");
+  }
+  if (a.dst_lo) PASE_CHECK_QUAD(fn, a.dst_lo, dsz, "dst_lo");
+  if (du) PASE_CHECK_QUAD(fn, du, ysz, "du");
+  return PASE_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -841,11 +941,25 @@ int pase_bn_prelu_pad_fwd(const void* y, int y_bf16, long y_sample_stride, int N
                  "pase_bn_prelu_pad_fwd: C=%d must be a positive multiple of 4", C);
   PASE_CHECK_ARG((padL == 0 && padR == 0) || (padL < T && padR < T),
                  "pase_bn_prelu_pad_fwd: reflect pad (%d,%d) >= T=%d", padL, padR, T);
-  PASE_CHECK_ARG((dst_row_stride % 4) == 0 && (dst_sample_stride % 4) == 0 &&
-                     (y_sample_stride % 4) == 0 && aligned16(y) && aligned16(dst),
-                 "pase_bn_prelu_pad_fwd: strides/pointers must be 4-element aligned");
   PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2 && (dst_fmt != PASE_FMT_F16X2 || dst_lo),
                  "pase_bn_prelu_pad_fwd: bad dst_fmt %d / missing lo", dst_fmt);
+  {
+    const char* fn = "pase_bn_prelu_pad_fwd";
+    const int dsz = dst_fmt == PASE_FMT_F32 ? 4 : 2;
+    PASE_CHECK_QUAD(fn, y, y_bf16 ? 2 : 4, "y");
+    PASE_CHECK_STRIDE(fn, y_sample_stride, "y_sample_stride");
+    PASE_CHECK_QUAD(fn, dst, dsz, "dst");
+    if (dst_lo) PASE_CHECK_QUAD(fn, dst_lo, dsz, "dst_lo");
+    PASE_CHECK_STRIDE(fn, dst_sample_stride, "dst_sample_stride");
+    PASE_CHECK_STRIDE(fn, dst_row_stride, "dst_row_stride");
+    if (pool && pool_d != 0) {
+      PASE_CHECK_QUAD(fn, pool, 4, "pool");
+      PASE_CHECK_STRIDE(fn, pool_sample_stride, "pool_sample_stride");
+      PASE_CHECK_STRIDE(fn, pool_row_stride, "pool_row_stride");
+      PASE_CHECK_ARG(pool_d > 0 && pool_T >= 0 && (long)pool_T * pool_d <= T,
+                     "%s: pool_T=%d x pool_d=%d exceeds T=%d", fn, pool_T, pool_d, T);
+    }
+  }
   if (pool == nullptr) pool_d = 0;
   const int Tp = T + padL + padR;
   const int RUN = bn_run();
@@ -887,30 +1001,33 @@ int pase_bn_prelu_bwd_reduce(const void* y, int y_bf16, long y_sample_stride, in
                  "sums only, see pase_bn_prelu_bwd_apply_src)");
   PASE_CHECK_ARG(N > 0 && T > 0 && C > 0 && (C % 4) == 0 && C <= 4096,
                  "pase_bn_prelu_bwd_reduce: C=%d must be a multiple of 4, <= 4096", C);
-  BwdSrc s{srcA, a_sample_stride, a_row_stride, padL, padR, srcB, b_sample_stride, b_row_stride,
-           b_shift, pool, pool_sample_stride, pool_row_stride, pool ? pool_d : 0, pool_T};
-  if (dst == nullptr) {                    // sums only: persistent staged kernel when it fits
-    BnStreamArgs sa{};
-    sa.y = y; sa.y_bf16 = y_bf16; sa.y_ss = y_sample_stride; sa.N = N; sa.T = T; sa.C = C;
+  BnStreamArgs sa = bn_bwd_args(y, y_bf16, y_sample_stride, N, T, C, srcA, a_bf16,
+                                a_sample_stride, a_row_stride, padL, padR, srcB, b_sample_stride,
+                                b_row_stride, b_shift, pool, pool_sample_stride, pool_row_stride,
+                                pool_d, pool_T, dst, nullptr, 0, dst_sample_stride);
+  const int rc = bn_bwd_check("pase_bn_prelu_bwd_reduce", sa, 1, nullptr);
+  if (rc != PASE_OK) return rc;
+  const BwdSrc& s = sa.s;
+  const BnBwdPlan plan = bn_bwd_plan(sa, 1);
+  if (plan.path == 1) {                    // sums only: persistent staged kernel
     sa.mean = mean; sa.invstd = invstd; sa.scale = scale; sa.shift = shift; sa.alpha = alpha;
-    sa.s = s; sa.a_bf16 = a_bf16; sa.S1 = S1; sa.S2 = S2; sa.dalpha = dalpha; sa.amax = amax;
-    if (pase_bn_stream_ok(sa)) return pase_bn_stream_reduce(sa, (cudaStream_t)stream);
+    sa.S1 = S1; sa.S2 = S2; sa.dalpha = dalpha; sa.amax = amax;
+    return pase_bn_stream_reduce(sa, (cudaStream_t)stream);
   }
-  const int RUN = bn_run();
-  const long threads = (long)(C / 4) * ((T + RUN - 1) / RUN);
-  long gx = (threads + THREADS - 1) / THREADS;
-  if ((THREADS % (C / 4)) == 0) {          // stride keeps the channel quad: cap the grid
-    long cap = ((RUN == 8 ? 8L : 16L) * pase_num_sms() + N - 1) / N;
-    if (cap < 1) cap = 1;
-    if (gx > cap) gx = cap;
-  }
-  dim3 grid((unsigned)gx, N);
+  const int RUN = plan.rows;
+  dim3 grid((unsigned)plan.gx, N);
   const size_t sm = 3 * C * sizeof(double) + 2 * sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
+  // C >= 2048: the block sums need more than the default 48 KB of dynamic shared memory
 #define PASE_RED_R(YT, GT, RV)                                                               \
-  bn_prelu_bwd_reduce_kernel<YT, GT, RV><<<grid, THREADS, sm, st>>>(                         \
-      reinterpret_cast<const YT*>(y), y_sample_stride, T, C, mean, invstd, scale, shift,     \
-      alpha, s, reinterpret_cast<YT*>(dst), dst_sample_stride, S1, S2, dalpha, amax)
+  do {                                                                                       \
+    if (sm > 48 * 1024)                                                                      \
+      cudaFuncSetAttribute(bn_prelu_bwd_reduce_kernel<YT, GT, RV>,                           \
+                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);            \
+    bn_prelu_bwd_reduce_kernel<YT, GT, RV><<<grid, THREADS, sm, st>>>(                       \
+        reinterpret_cast<const YT*>(y), y_sample_stride, T, C, mean, invstd, scale, shift,   \
+        alpha, s, reinterpret_cast<YT*>(dst), dst_sample_stride, S1, S2, dalpha, amax);      \
+  } while (0)
 #define PASE_RED(YT, GT) do { if (RUN == 8) PASE_RED_R(YT, GT, 8); else PASE_RED_R(YT, GT, 4); } while (0)
   if (y_bf16) {
     if (a_bf16) PASE_RED(__nv_bfloat16, __nv_bfloat16);
@@ -941,15 +1058,14 @@ int pase_bn_prelu_bwd_apply(const void* y, int y_bf16, long y_sample_stride, int
                  "and fp32 y/du");
   PASE_CHECK_ARG((dst_fmt == PASE_FMT_BF16) == (y_bf16 != 0),
                  "pase_bn_prelu_bwd_apply: bf16 y/du goes with bf16 dst (and only with it)");
-  const int RUN = bn_run();
-  const long threads = (long)(C / 4) * ((T + RUN - 1) / RUN);
-  long gx = (threads + THREADS - 1) / THREADS;
-  if ((THREADS % (C / 4)) == 0) {
-    long cap = ((RUN == 8 ? 8L : 16L) * pase_num_sms() + N - 1) / N;
-    if (cap < 1) cap = 1;
-    if (gx > cap) gx = cap;
-  }
-  dim3 grid((unsigned)gx, N);
+  const BnStreamArgs sa = bn_bwd_args(y, y_bf16, y_sample_stride, N, T, C, nullptr, 0, 0, 0, 0,
+                                      0, nullptr, 0, 0, 0, nullptr, 0, 0, 0, 0, dst, dst_lo,
+                                      dst_fmt, dst_sample_stride);
+  const int rc = bn_bwd_check("pase_bn_prelu_bwd_apply", sa, 2, du);
+  if (rc != PASE_OK) return rc;
+  const BnBwdPlan plan = bn_bwd_plan(sa, 2);          // always the register kernel
+  const int RUN = plan.rows;
+  dim3 grid((unsigned)plan.gx, N);
   const size_t sm = C * sizeof(double) + sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_APP_R(YT, DF, RV)                                                                \
@@ -990,28 +1106,22 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
   PASE_CHECK_ARG((dst_fmt == PASE_FMT_BF16) == (y_bf16 != 0),
                  "pase_bn_prelu_bwd_apply_src: bf16 y goes with bf16 dst (and only with it)");
   PASE_CHECK_ARG(!a_bf16 || y_bf16, "pase_bn_prelu_bwd_apply_src: bf16 srcA needs bf16 y");
-  BwdSrc s{srcA, a_sample_stride, a_row_stride, padL, padR, srcB, b_sample_stride, b_row_stride,
-           b_shift, pool, pool_sample_stride, pool_row_stride, pool ? pool_d : 0, pool_T};
-  {
-    BnStreamArgs sa{};
-    sa.y = y; sa.y_bf16 = y_bf16; sa.y_ss = y_sample_stride; sa.N = N; sa.T = T; sa.C = C;
+  BnStreamArgs sa = bn_bwd_args(y, y_bf16, y_sample_stride, N, T, C, srcA, a_bf16,
+                                a_sample_stride, a_row_stride, padL, padR, srcB, b_sample_stride,
+                                b_row_stride, b_shift, pool, pool_sample_stride, pool_row_stride,
+                                pool_d, pool_T, dst, dst_lo, dst_fmt, dst_sample_stride);
+  const int rc = bn_bwd_check("pase_bn_prelu_bwd_apply_src", sa, 2, nullptr);
+  if (rc != PASE_OK) return rc;
+  const BwdSrc& s = sa.s;
+  const BnBwdPlan plan = bn_bwd_plan(sa, 2);
+  if (plan.path == 1) {
     sa.mean = mean; sa.invstd = invstd; sa.gamma = gamma; sa.scale = scale; sa.shift = shift;
-    sa.alpha = alpha; sa.s = s; sa.a_bf16 = a_bf16; sa.S1in = S1; sa.S2in = S2;
-    sa.inv_count = 1.0 / count; sa.dst = dst; sa.dst_lo = dst_lo; sa.dst_fmt = dst_fmt;
-    sa.d_ss = dst_sample_stride; sa.dbias = dbias_acc; sa.amax = const_cast<float*>(amax); sa.scale_out = scale_out;
-    if (pase_bn_stream_ok(sa) && (dst_sample_stride % 8) == 0 && aligned16(dst) &&
-        (dst_lo == nullptr || aligned16(dst_lo)))
-      return pase_bn_stream_apply(sa, (cudaStream_t)stream);
+    sa.alpha = alpha; sa.S1in = S1; sa.S2in = S2; sa.inv_count = 1.0 / count;
+    sa.dbias = dbias_acc; sa.amax = const_cast<float*>(amax); sa.scale_out = scale_out;
+    return pase_bn_stream_apply(sa, (cudaStream_t)stream);
   }
-  const int RUN = bn_run();
-  const long threads = (long)(C / 4) * ((T + RUN - 1) / RUN);
-  long gx = (threads + THREADS - 1) / THREADS;
-  if ((THREADS % (C / 4)) == 0) {
-    long cap = ((RUN == 8 ? 8L : 16L) * pase_num_sms() + N - 1) / N;
-    if (cap < 1) cap = 1;
-    if (gx > cap) gx = cap;
-  }
-  dim3 grid((unsigned)gx, N);
+  const int RUN = plan.rows;
+  dim3 grid((unsigned)plan.gx, N);
   const size_t sm = C * sizeof(double) + sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_APS_R(YT, GT, DF, RV)                                                             \
@@ -1030,6 +1140,33 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
 #undef PASE_APS
 #undef PASE_APS_R
   PASE_LAUNCH_CHECK("pase_bn_prelu_bwd_apply_src");
+  return PASE_OK;
+}
+
+int pase_bn_bwd_plan(int pass, const void* y, int y_bf16, long y_sample_stride, int N, int T,
+                     int C, const void* srcA, int a_bf16, long a_sample_stride,
+                     long a_row_stride, int padL, int padR, const float* srcB,
+                     long b_sample_stride, long b_row_stride, int b_shift, const float* pool,
+                     long pool_sample_stride, long pool_row_stride, int pool_d, int pool_T,
+                     void* dst, void* dst_lo, int dst_fmt, long dst_sample_stride, long* out4) {
+  PASE_CHECK_ARG(out4 && y && (pass == 1 || pass == 2) && (pass == 2 || srcA),
+                 "pase_bn_bwd_plan: bad args");
+  PASE_CHECK_ARG(N > 0 && T > 0 && C > 0 && (C % 4) == 0 && C <= 4096,
+                 "pase_bn_bwd_plan: C=%d must be a multiple of 4, <= 4096", C);
+  PASE_CHECK_ARG(pass == 1 || (dst && dst_fmt >= 0 && dst_fmt <= 2),
+                 "pase_bn_bwd_plan: pass 2 needs dst and a dst_fmt in 0..2");
+  const BnStreamArgs sa = bn_bwd_args(y, y_bf16, y_sample_stride, N, T, C, srcA, a_bf16,
+                                      a_sample_stride, a_row_stride, padL, padR, srcB,
+                                      b_sample_stride, b_row_stride, b_shift, pool,
+                                      pool_sample_stride, pool_row_stride, pool_d, pool_T, dst,
+                                      pass == 1 ? nullptr : dst_lo, dst_fmt, dst_sample_stride);
+  const int rc = bn_bwd_check("pase_bn_bwd_plan", sa, pass, nullptr);
+  if (rc != PASE_OK) return rc;
+  const BnBwdPlan p = bn_bwd_plan(sa, pass);
+  out4[0] = p.path;
+  out4[1] = p.rows;
+  out4[2] = p.items;
+  out4[3] = p.blocks;
   return PASE_OK;
 }
 

@@ -321,11 +321,11 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
 }
 
 template <typename YT, typename GT, int DF, bool APPLY, typename TC>
-int launch_cfg(const BnStreamArgs& a, cudaStream_t st) {
+int launch_cfg(const BnStreamArgs& a, const BnStreamPlan& p, cudaStream_t st) {
   Geo g;
-  g.TT = TC::TE / a.C;
-  g.tps = (a.T + g.TT - 1) / g.TT;
-  g.total = (long)a.N * g.tps;
+  g.TT = p.TT;
+  g.tps = p.tps;
+  g.total = p.total;
   const size_t smem = (size_t)TC::NS * TC::TE * (sizeof(YT) + sizeof(GT)) +
                       TC::NS * sizeof(uint64_t) + (size_t)3 * a.C * sizeof(double) +
                       2 * sizeof(float);
@@ -340,9 +340,7 @@ int launch_cfg(const BnStreamArgs& a, cudaStream_t st) {
     }
     attr_done = true;
   }
-  long grid = 2L * pase_num_sms();
-  if (grid > g.total) grid = g.total;
-  PASE_LAUNCH(kern, (unsigned)grid, THREADS, smem, st, a, g);
+  PASE_LAUNCH(kern, (unsigned)p.grid, THREADS, smem, st, a, g);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     pase_set_error("bn_stream: launch failed: %s", cudaGetErrorString(e));
@@ -362,8 +360,9 @@ int tile_elems() {
 
 template <typename YT, typename GT, int DF, bool APPLY>
 int launch(const BnStreamArgs& a, cudaStream_t st) {
-  if (tile_elems() == 2048 && a.C <= 512) return launch_cfg<YT, GT, DF, APPLY, TileCfg<2048, 6>>(a, st);
-  return launch_cfg<YT, GT, DF, APPLY, TileCfg<4096, 3>>(a, st);
+  const BnStreamPlan p = pase_bn_stream_plan(a);
+  if (p.TE == 2048) return launch_cfg<YT, GT, DF, APPLY, TileCfg<2048, 6>>(a, p, st);
+  return launch_cfg<YT, GT, DF, APPLY, TileCfg<4096, 3>>(a, p, st);
 }
 
 bool stream_enabled() {
@@ -393,6 +392,17 @@ bool pase_bn_stream_ok(const BnStreamArgs& a) {
   if (a.s.B && ((reinterpret_cast<uintptr_t>(a.s.B) & 15u) || a.s.b_ss % 4 || a.s.b_rs % 4))
     return false;
   return true;
+}
+
+BnStreamPlan pase_bn_stream_plan(const BnStreamArgs& a) {
+  BnStreamPlan p;
+  p.TE = (tile_elems() == 2048 && a.C <= 512) ? 2048 : 4096;
+  p.TT = p.TE / a.C;
+  p.tps = (a.T + p.TT - 1) / p.TT;
+  p.total = (long)a.N * p.tps;
+  p.grid = 2L * pase_num_sms();
+  if (p.grid > p.total) p.grid = p.total;
+  return p;
 }
 
 int pase_bn_stream_reduce(const BnStreamArgs& a, cudaStream_t st) {
