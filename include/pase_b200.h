@@ -377,6 +377,48 @@ int pase_lps_post(const float* C, long ldc, int N, int frames, int nbins, int de
                   int width, const float* fir, const float* mean, const float* stdv, float* out,
                   void* stream);
 
+/* ---- on-device waveform distortions (pase/transforms.py:38-146 config_distortions /
+ * PCompose; the host planner is pase_b200/distortions.py).  Job tables are int64 DEVICE rows,
+ * one per sample (row b acts on row b of every operand); a row whose first field is 0 is not
+ * drawn and its sample is left untouched, and a row that does not fit its operands is treated
+ * the same way.  Rows of x / out / seg / label are `ld*` elements apart.  Reductions are fp64
+ * in a fixed order, so results are reproducible bit for bit. */
+/* Workspace bytes pase_fft_conv needs for this geometry (host-only). */
+int pase_fft_conv_workspace(int njobs, int T, int Lmax, long* bytes);
+/* FFT convolution + energy scale (Reverb transforms.py:1071-1103, BandDrop 1263-1297,
+ * Downsample 1162-1197).  jobs: njobs rows {on, n, filt_off, L, p, mode}, n <= T, L <= Lmax,
+ * 0 <= p < L, filt_off + L <= bank_len.  With h = bank[filt_off, +L) and
+ * full = signal.convolve(x[0, n), h, 'full'), y[t] = full[p + t] for t < n:
+ *   mode 0 (FIR):    E = y.y;    out = sqrt(Ex/E) y if E > 0, else x
+ *   mode 1 (reverb): E = full.full (tail included); out = sqrt(Ex/E) y if E > 0, else y
+ *   mode 2 (raw):    out = y
+ * where Ex = x[0,n).x[0,n).  out may equal x (in place); out[n, T) is not written.  Uniformly
+ * partitioned overlap-save: 4096-sample blocks, 8192-point fp32 FFTs in shared memory.
+ * twiddle: 4096 (re, im) pairs exp(-2 pi i k / 8192).  ws: >= pase_fft_conv_workspace bytes,
+ * 16-byte aligned. */
+int pase_fft_conv(const float* x, long ldx, const float* bank, long bank_len, const long* jobs,
+                  int njobs, int T, int Lmax, const float* twiddle, void* ws, long ws_bytes,
+                  float* out, long ldo, void* stream);
+/* Noise / overlap segment (transforms.py:1644-1658, 1720-1733): jobs rows {on, pool_off,
+ * avail}; out[u] = pool[pool_off + u] for u < avail, 0 for avail <= u < T. */
+int pase_segment_gather(const float* pool, long pool_len, const long* jobs, int njobs, int T,
+                        float* out, long ldo, void* stream);
+/* In-place additive mix (SimpleAdditive transforms.py:1633-1675 with guard = 1,
+ * SimpleAdditiveShift 1714-1766 with guard = 0): jobs rows {on, shift, guard}; the noise is
+ * n[t] = 0 for t < shift, seg[t - shift] after; K = sqrt(Ex / (snr_lin En)) (1 if En == 0);
+ * x <- sqrt(Ex / (v.v + 1e-14)) v with v = x + K n.  guard: En == 0 leaves x as it is. */
+int pase_noise_mix(float* x, long ldx, const float* seg, long lds, const long* jobs,
+                   const double* snr_lin, int njobs, int T, void* stream);
+/* In-place Clipping (transforms.py:1522-1536): jobs rows {on};
+ * x <- min(max(x, cf min x), cf max x). */
+int pase_clip(float* x, long ldx, const long* jobs, const double* cf, int njobs, int T,
+              void* stream);
+/* Overlap label (transforms.py:1738-1748): jobs rows {on, shift, guard} (the overlap mix
+ * table); label[j] = mean of (t >= shift) over t in [j d, (j+1) d), 0 where on == 0.
+ * d divides T. */
+int pase_overlap_label(const long* jobs, int njobs, int T, int d, float* label, long ldl,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif
