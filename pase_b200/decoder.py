@@ -11,7 +11,7 @@ weight gradient is the same TN GEMM the encoder uses.
 """
 import torch
 
-from . import ops
+from . import gemm, ops
 from . import functional as Fn
 
 
@@ -62,6 +62,7 @@ class _DecoderStackFn(torch.autograd.Function):
         rows = rows.detach().contiguous()
         plan.generation += 1
         G = plan.geoms
+        p = Fn.gemm_precision()
         g0 = G[0]
         plan.xz[0][:B * g0.Pd * g0.Cin].view(B, g0.Pd, g0.Cin)[:, g0.taps - 1:g0.taps - 1 + T] \
             .copy_(rows.view(B, T, g0.Cin))
@@ -70,9 +71,9 @@ class _DecoderStackFn(torch.autograd.Function):
             W, b, alpha = params[3 * i].detach(), params[3 * i + 1].detach(), \
                 params[3 * i + 2].detach()
             call("pase_deconv_w_to_fwd", W.reshape(-1), plan.Wu[i], g.Cin, g.Cout, g.k, g.s, g.taps)
-            Fn.gemm_nt(plan.xz[i], g.Cin, plan.xz[i].numel(), plan.Wu[i], g.taps * g.Cin,
-                       plan.Wu[i].numel(), plan.yfull[i], g.s * g.Cout, B * g.Pd, g.s * g.Cout,
-                       g.taps * g.Cin, b.repeat(g.s).contiguous(), g.Pd, g.U, g.U)
+            gemm.nt(p, plan.xz[i], g.Cin, plan.xz[i].numel(), plan.Wu[i], g.taps * g.Cin,
+                    plan.yfull[i], g.s * g.Cout, B * g.Pd, g.s * g.Cout, g.taps * g.Cin,
+                    bias=b.repeat(g.s).contiguous(), rows_in=g.Pd, t_valid=g.U, rows_out=g.U)
             if i + 1 < len(G):
                 nx = G[i + 1]
                 dst, d_ss = plan.xz[i + 1][(nx.taps - 1) * nx.Cin:], nx.Pd * nx.Cin
@@ -96,6 +97,7 @@ class _DecoderStackFn(torch.autograd.Function):
                                "forward before this backward ran")
         params = ctx.saved_tensors
         B, G = plan.B, plan.geoms
+        p = Fn.gemm_precision()
         grads = [None] * len(params)
         src = dh.contiguous().reshape(-1)
         dev = dh.device
@@ -116,24 +118,25 @@ class _DecoderStackFn(torch.autograd.Function):
             call("pase_cast_d2f", acc, small, 4 * C, 1.0)
             grads[3 * i + 2] = small[2 * C:3 * C].clone().view_as(alpha)
             grads[3 * i + 1] = small[:C].clone()
-            # dY feeds the weight-gradient and the input-gradient GEMM: one operand conversion
-            dyop = plan.dyfull[i]
-            mode = Fn._MODES[Fn.PRECISION]
-            if mode not in (None, 0) and (g.s * C) % Fn._eb(mode) == 0 and \
-                    g.Cin % Fn._eb(mode) == 0 and (g.taps * g.Cin) % Fn._eb(mode) == 0:
-                dyop = Fn.to_operand(plan.dyfull[i], plan.dyfull[i].numel(), mode, "grad")
-            Fn.gemm_tn(dyop, g.s * C, plan.dyfull[i].numel(), plan.xz[i], g.Cin,
-                       plan.xz[i].numel(), plan.dWu[i], g.taps * g.Cin, g.s * C, g.taps * g.Cin,
-                       g.U, groups=B, pitchA=g.U, offA=0, pitchB=g.Pd)
+            # dY feeds the weight-gradient and the input-gradient GEMM: when both take the
+            # tensor cores, one operand conversion
+            dy, n_dy = plan.dyfull[i], plan.dyfull[i].numel()
+            dyop = None
+            if gemm.tn_ok(p, g.s * C, g.Cin, g.s * C, g.taps * g.Cin) and \
+                    gemm.nt_ok(p, g.s * C, g.k * C, g.k * C):
+                dyop = gemm.to_operand(p, dy, n_dy, "grad")
+            gemm.tn(p, dy, g.s * C, n_dy, plan.xz[i], g.Cin, plan.xz[i].numel(), plan.dWu[i],
+                    g.taps * g.Cin, g.s * C, g.taps * g.Cin, g.U, groups=B, pitchA=g.U, offA=0,
+                    pitchB=g.Pd, a_op=dyop)
             dW = torch.empty_like(W)
             call("pase_deconv_w_from_fwd", plan.dWu[i], dW.reshape(-1), g.Cin, g.Cout, g.k, g.s,
                  g.taps)
             grads[3 * i] = dW
             if i > 0 or ctx.needs_input_grad[0]:
                 call("pase_deconv_w_to_bwd", W.reshape(-1), plan.Wb[i], g.Cin, g.Cout, g.k)
-                Fn.gemm_nt(dyop, g.s * C, plan.dyfull[i].numel(), plan.Wb[i], g.k * C,
-                           plan.Wb[i].numel(), plan.dx[i], g.Cin, B * g.U, g.Cin, g.k * C, None,
-                           g.U, g.T_in, g.T_in, a_kind="grad")
+                gemm.nt(p, dy, g.s * C, n_dy, plan.Wb[i], g.k * C, plan.dx[i], g.Cin, B * g.U,
+                        g.Cin, g.k * C, rows_in=g.U, t_valid=g.T_in, rows_out=g.T_in,
+                        a_kind="grad", a_op=dyop)
                 src = plan.dx[i]
         dx = None
         if ctx.needs_input_grad[0]:

@@ -16,25 +16,12 @@ projection (mean-pool commutes with a bias-free 1x1 conv, frontend.py:182,
 skips and the QRNN output are concatenated so W + all skips are one GEMM.
 """
 import math
-import os
 import torch
 
-from . import ops
+from . import gemm, ops
 
 BN_EPS = 1e-5
 BN_MOMENTUM = 0.1
-SINC_FOLD = 4            # polyphase fold of the sinc layer on the fp32 FFMA path
-# on the tensor-core path one folded row = one 128-byte TMA row: 32 fp32 / 64 16-bit elements
-TC_SINC_FOLD = {0: 32, 1: 32, 2: 64, 3: 64}
-# numerics of the GEMMs (pase_tc_gemm_* `mode`): None = fp32 FFMA; 0 = TF32; 1 = 3xTF32
-# (fp32-equivalent); 2 = bf16 operands AND bf16 activation storage; 3 = 3xF16 (fp16 operand
-# pairs, fp32-equivalent products at half the tensor time / operand bytes of 3xTF32)
-PRECISIONS = {"fp32": None, "3xtf32": 1, "tf32": 0, "bf16": 2, "3xf16": 3}
-# storage format codes of the C-ABI (include/pase_b200.h)
-FMT_F32, FMT_BF16, FMT_F16X2 = 0, 1, 2
-OP_FMT = {None: FMT_F32, 0: FMT_F32, 1: FMT_F32, 2: FMT_BF16, 3: FMT_F16X2}
-OP_DTYPE = {None: torch.float32, 0: torch.float32, 1: torch.float32, 2: torch.bfloat16,
-            3: torch.float16}
 
 
 def _cdiv(a, b):
@@ -111,18 +98,6 @@ def frame_counts(cfg, T):
     return [g.T_out for g in build_geometry(cfg, T)]
 
 
-class Operand(object):
-    """One GEMM operand in the format of the plan's GEMM mode.
-    hi / lo: the tensors handed to pase_tc_gemm_* (lo None outside the split modes);
-    alpha: device float[2] = {1/s, s} when the operand is a power-of-two scaled gradient
-    (3xF16), else None;  src: the fp32 tensor it is converted from (None when the producing
-    kernel writes the operand format directly)."""
-    __slots__ = ("hi", "lo", "alpha", "src", "kind", "amax")
-
-    def __init__(self, hi, lo=None, alpha=None, src=None, kind="act", amax=None):
-        self.hi, self.lo, self.alpha, self.src, self.kind, self.amax = hi, lo, alpha, src, kind, amax
-
-
 class EncoderPlan(object):
     """All HBM buffers of one (N, T) problem, allocated once and reused every
     step (180 GB HBM: nothing is recomputed or re-allocated).  Padded operand
@@ -137,25 +112,19 @@ class EncoderPlan(object):
 
     def __init__(self, cfg, N, T, device, prec="fp32"):
         self.cfg, self.N, self.T, self.device = cfg, N, T, device
-        if prec not in PRECISIONS:
-            raise ValueError("precision must be one of %s" % (sorted(PRECISIONS),))
-        self.prec, self.mode = prec, PRECISIONS[prec]
-        mode = self.mode
-        self.fmt = OP_FMT[mode]
-        self.op_dtype = OP_DTYPE[mode]
-        self.split_mode = mode in (1, 3)
-        self.y_bf16 = 1 if mode == 2 else 0
-        self.eb = 64 if mode in (2, 3) else 32          # elements per 128-byte TMA row
-        self._ops = {}
+        if prec not in gemm.PRECISIONS:
+            raise ValueError("precision must be one of %s" % (sorted(gemm.PRECISIONS),))
+        self.precision = p = gemm.PRECISIONS[prec]
+        self._ops = {}             # name -> gemm.Operand
         self._wtables = {}
-        self.geoms = build_geometry(cfg, T, TC_SINC_FOLD[mode] if mode is not None else SINC_FOLD)
+        self.geoms = build_geometry(cfg, T, p.sinc_fold)
         G = self.geoms
-        if mode in (2, 3):
+        if p.esz == 2:
             for g in G:
-                if (g.lda % 64) or (g.Cout % 64 and not g.sinc):
+                if (g.lda % p.eb) or (g.Cout % p.eb and not g.sinc):
                     raise NotImplementedError(
-                        "precision %r needs channel counts that are multiples of 64 (block %d: "
-                        "Cin=%d Cout=%d stride=%d)" % (prec, g.idx, g.Cin, g.Cout, g.s))
+                        "precision %r needs channel counts that are multiples of %d (block %d: "
+                        "Cin=%d Cout=%d stride=%d)" % (prec, p.eb, g.idx, g.Cin, g.Cout, g.s))
         self.nblk = len(G)
         self.Tq = G[-1].T_out
         self.emb = cfg["emb_dim"]
@@ -166,12 +135,12 @@ class EncoderPlan(object):
         self.H = (cfg["rnn_dim"] // 2) * 2 if self.rnn else 0
         f32 = dict(dtype=torch.float32, device=device)
         f64 = dict(dtype=torch.float64, device=device)
-        opd = dict(dtype=self.op_dtype, device=device)
-        yd = dict(dtype=torch.bfloat16 if mode == 2 else torch.float32, device=device)
+        opd = dict(dtype=p.dtype, device=device)
+        yd = dict(dtype=torch.bfloat16 if p.act_bf16 else torch.float32, device=device)
         z = lambda n: torch.zeros(int(n), **f32)
         e = lambda n: torch.empty(int(n), **f32)
         zo = lambda n: torch.zeros(int(n), **opd)          # operand-format buffers (hi / lo)
-        zlo = lambda n: torch.zeros(int(n), **opd) if self.split_mode else None
+        zlo = lambda n: torch.zeros(int(n), **opd) if p.split else None
 
         # concatenated [rnn-out | pooled skips] operand of the output projection
         self.col_off = []
@@ -189,7 +158,7 @@ class EncoderPlan(object):
             n_apad = N * g.apad_floats + g.K + 64
             self.apad.append(zo(n_apad))
             self.apad_lo.append(zlo(n_apad))
-            self._ops[("apad", g.idx)] = Operand(self.apad[-1], self.apad_lo[-1])
+            self._ops[("apad", g.idx)] = gemm.Operand(self.apad[-1], self.apad_lo[-1])
             self.y.append(torch.empty(int(N * g.rows_out * g.Nn), **yd))
             self.bn.append(torch.zeros(4, g.Cout, **f32))       # mean, invstd, scale, shift
             self.Wt.append(e(g.Nn * g.K))
@@ -199,7 +168,7 @@ class EncoderPlan(object):
             Cq, H = self.Clast, self.H
             n_xq = N * (self.Tq + 1) * Cq + 2 * Cq + 64
             self.xq, self.xq_lo = zo(n_xq), zlo(n_xq)
-            self._ops["xq"] = Operand(self.xq, self.xq_lo)
+            self._ops["xq"] = gemm.Operand(self.xq, self.xq_lo)
             self.Yg, self.Cst = e(rows * 3 * H), e(rows * H)
             self.Wq = e(3 * H * 2 * Cq)
         self.cat = z(rows * self.Kc)
@@ -235,19 +204,20 @@ class EncoderPlan(object):
         warm-up steps and never inside a CUDA-graph capture."""
         if self.backward_ready:
             return
-        G, N, mode, device = self.geoms, self.N, self.mode, self.device
+        G, N, p, device = self.geoms, self.N, self.precision, self.device
         f32 = dict(dtype=torch.float32, device=device)
         f64 = dict(dtype=torch.float64, device=device)
-        opd = dict(dtype=self.op_dtype, device=device)
-        yd = dict(dtype=torch.bfloat16 if mode == 2 else torch.float32, device=device)
+        opd = dict(dtype=p.dtype, device=device)
+        yd = dict(dtype=torch.bfloat16 if p.act_bf16 else torch.float32, device=device)
         z = lambda n: torch.zeros(int(n), **f32)
         e = lambda n: torch.empty(int(n), **f32)
         zo = lambda n: torch.zeros(int(n), **opd)
-        zlo = lambda n: torch.zeros(int(n), **opd) if self.split_mode else None
+        zlo = lambda n: torch.zeros(int(n), **opd) if p.split else None
+        f16x2 = p.fmt == gemm.FMT_F16X2           # gradients carry power-of-two scales
         self.dWt, self.Wd, self.dyz, self.dyz_lo, self.dxpad, self.gscale = [], [], [], [], [], []
         for g in G:
             self.dWt.append(e(g.Nn * g.K))
-            gs = torch.ones(2, **f32) if mode == 3 else None
+            gs = torch.ones(2, **f32) if f16x2 else None
             self.gscale.append(gs)
             if g.sinc:
                 n_dyz = N * g.rows_out * g.Nn + 128
@@ -259,8 +229,7 @@ class EncoderPlan(object):
                 self.dxpad.append(torch.empty(int(N * g.apad_floats), **yd) if g.idx > 0 else None)
             self.dyz.append(zo(n_dyz))
             self.dyz_lo.append(zlo(n_dyz))
-            self._ops[("dyz", g.idx)] = Operand(self.dyz[-1], self.dyz_lo[-1],
-                                                None if gs is None else gs, kind="grad")
+            self._ops[("dyz", g.idx)] = gemm.Operand(self.dyz[-1], self.dyz_lo[-1], gs)
         rows = self.rows
         if self.rnn:
             Cq, H = self.Clast, self.H
@@ -286,68 +255,33 @@ class EncoderPlan(object):
         self.stats_b = torch.zeros(n, **f64)
         self.grad_vec = torch.zeros(n, **f32)
         # running maxima for the 3xF16 gradient scales: 2 floats per use, zeroed per backward
-        self.amax = torch.zeros(2 * (self.nblk + 4), **f32) if mode == 3 else None
+        self.amax = torch.zeros(2 * (self.nblk + 4), **f32) if f16x2 else None
         self.backward_ready = True
 
     # -- GEMM operands -----------------------------------------------------------------
     def operand(self, name, buf, fresh=True, kind="act"):
-        """Operand `name` in the plan's GEMM format.  Operands whose producer writes the GEMM
-        format directly (apad, xq, dyz) are registered at construction; everything else is an
-        fp32 tensor converted here (`fresh=False` reuses this step's earlier conversion):
-          tf32   : the tensor itself;
-          3xtf32 : activations: the tensor is "hi" (tf32 tensor cores truncate), lo = rn(x-trunc(x));
-                   weights: explicit hi = rn(x), lo = rn(x - hi) (no coherent bias);
-          bf16   : bf16 copy;    3xf16 : fp16 (hi, lo') pair, gradients pre-scaled by a power
-                   of two (alpha = {1/s, s} on the device)."""
+        """Operand `name` in the plan's GEMM format (gemm.Operand).  Operands whose producer
+        writes the GEMM format directly (apad, xq, dyz, the conv weights) are registered with
+        no fp32 source; everything else is the fp32 tensor `buf` converted into buffers kept
+        per name (`fresh=False` reuses this step's earlier conversion)."""
         op = self._ops.get(name)
         if op is not None and op.src is None:
             return op
-        mode = self.mode
-        if mode == 0:
-            return Operand(buf)
         if op is None or op.src.numel() != buf.numel() or op.src.data_ptr() != buf.data_ptr():
-            f32 = dict(dtype=torch.float32, device=self.device)
-            if mode == 1:
-                hi = torch.zeros_like(buf) if kind == "weight" else buf
-                op = Operand(hi, torch.zeros_like(buf), src=buf, kind=kind)
-            elif mode == 2:
-                op = Operand(torch.zeros(buf.numel(), dtype=torch.bfloat16, device=self.device),
-                             src=buf, kind=kind)
-            else:
-                h = torch.zeros(buf.numel(), dtype=torch.float16, device=self.device)
-                grad = kind == "grad"
-                op = Operand(h, torch.zeros_like(h),
-                             torch.ones(2, **f32) if grad else None, src=buf, kind=kind,
-                             amax=torch.zeros(2, **f32) if grad else None)
+            op = gemm.operand_buffers(self.precision, buf.numel(), self.device, kind, buf,
+                                      torch.zeros)
             self._ops[name] = op
             fresh = True
-        if fresh:
-            n = buf.numel()
-            if mode == 1:
-                ops.call("pase_split_tf32", buf, op.hi if kind == "weight" else None, op.lo, n)
-            elif mode == 2:
-                ops.call("pase_cast_bf16", buf, op.hi, n)
-            else:
-                if op.amax is not None:
-                    op.amax.zero_()
-                    ops.call("pase_absmax", buf, n, op.amax)
-                ops.call("pase_split_f16", buf, op.hi, op.lo, n, op.amax, op.alpha)
-        return op
+        return gemm.convert(self.precision, op, buf.numel(), kind) if fresh else op
 
     def w_operand(self, name, buf):
         """(hi, lo) buffers of a weight operand written by pase_conv_w_batch itself."""
-        mode = self.mode
-        if mode is None or mode == 0:
+        if self.precision.reads_fp32:
             return None, None
         op = self._ops.get(name)
         if op is None:
-            if mode == 1:
-                op = Operand(torch.zeros_like(buf), torch.zeros_like(buf))
-            elif mode == 2:
-                op = Operand(torch.zeros(buf.numel(), dtype=torch.bfloat16, device=self.device))
-            else:
-                h = torch.zeros(buf.numel(), dtype=torch.float16, device=self.device)
-                op = Operand(h, torch.zeros_like(h))
+            op = gemm.operand_buffers(self.precision, buf.numel(), self.device, "weight",
+                                      new=torch.zeros)
             self._ops[name] = op
         return op.hi, op.lo
 
@@ -372,69 +306,41 @@ class EncoderPlan(object):
             table = torch.tensor(rows, dtype=torch.int64).reshape(-1).to(self.device)
             ent = (rows, table)
             self._wtables[key] = ent
-        fmt = {1: 0, 2: 1, 3: 2}.get(self.mode, 0)
+        fmt = self.precision.fmt
         if tiled:
             ops.call("pase_conv_w_batch", ent[1], len(rows), blocks, op + 3, dst_base, fmt)
         else:
             ops.call("pase_conv_w_batch", ent[1], len(rows), start, op, dst_base, fmt)
 
-    def _tc_ok(self, *elem_strides):
-        """Tensor-core path: every operand row stride must be a multiple of 16 bytes (and the
-        A operand's folded row a multiple of 128 bytes -- checked by the caller)."""
-        q = 8 if self.mode in (2, 3) else 4
-        return all(s % q == 0 for s in elem_strides)
-
     def nt(self, an, A, lda, afresh, bn, B, ldb, bfresh, C, ldc, M, N, K, alpha, bias,
            rows_in, t_valid, rows_out, fold, cs, cq, acc, akind="act"):
-        """C = alpha * A B^T (+ bias): tensor-core kernel in the plan's GEMM mode, or the fp32
-        FFMA kernel (precision fp32, or shapes the TMA path cannot address)."""
-        direct = an in self._ops and self._ops[an].src is None      # no fp32 copy exists
-        if self.mode is None or lda % self.eb != 0 or not self._tc_ok(K, ldb):
-            if direct and self.mode in (2, 3):
-                raise NotImplementedError("precision %r: GEMM shape (lda=%d K=%d) outside the "
-                                          "tensor-core path" % (self.prec, lda, K))
-            return ops.call("pase_gemm_nt", A, lda, B, ldb, C, ldc, M, N, K, alpha, bias,
-                            rows_in, t_valid, rows_out, fold, cs, cq, acc)
-        a = self.operand(an, A, afresh, akind)
-        b = self.operand(bn, B, bfresh, "weight")
-        c16 = 1 if C.dtype == torch.bfloat16 else 0
-        return ops.call("pase_tc_gemm_nt", a.hi, a.lo, a.hi.numel() // lda, lda, b.hi, b.lo, ldb,
-                        C, ldc, M, N, K, alpha, None if a.alpha is None else a.alpha, bias,
-                        rows_in, t_valid, rows_out, fold, cs, cq, acc, self.mode, c16)
+        """C = alpha * A B^T (+ bias) in the plan's precision (gemm.nt) over the operands
+        `an` / `bn` of buffers A / B."""
+        return gemm.nt(self.precision, A, lda, A.numel(), B, ldb, C, ldc, M, N, K, alpha, bias,
+                       rows_in, t_valid, rows_out, fold, cs, cq, acc, akind,
+                       lambda: self.operand(an, A, afresh, akind),
+                       lambda: self.operand(bn, B, bfresh, "weight"))
 
     def tn(self, an, A, lda, pitchA, offA, afresh, bn, B, ldb, pitchB, bfresh, C, ldc, I, J,
            groups, rpg, alpha, acc, akind="grad"):
-        direct = (an in self._ops and self._ops[an].src is None) or \
-            (bn in self._ops and self._ops[bn].src is None)
-        if self.mode is None or ldb % self.eb != 0 or not self._tc_ok(lda) or I % 4 != 0 or \
-                J % self.eb != 0:
-            if direct and self.mode in (2, 3):
-                raise NotImplementedError("precision %r: weight-gradient GEMM shape (lda=%d "
-                                          "ldb=%d I=%d J=%d) outside the tensor-core path"
-                                          % (self.prec, lda, ldb, I, J))
-            return ops.call("pase_gemm_tn", A, lda, pitchA, offA, B, ldb, pitchB, 0, C, ldc, I, J,
-                            groups, rpg, alpha, acc)
-        a = self.operand(an, A, afresh, akind)
-        b = self.operand(bn, B, bfresh, "act")
-        return ops.call("pase_tc_gemm_tn", a.hi, a.lo, lda, pitchA, offA, b.hi, b.lo, ldb, pitchB,
-                        b.hi.numel() // ldb, C, ldc, I, J, groups, rpg, alpha,
-                        None if a.alpha is None else a.alpha, acc, self.mode)
+        """C = alpha * A^T B in the plan's precision (gemm.tn)."""
+        return gemm.tn(self.precision, A, lda, A.numel(), B, ldb, B.numel(), C, ldc, I, J, rpg,
+                       groups, pitchA, offA, pitchB, alpha, acc, akind,
+                       lambda: self.operand(an, A, afresh, akind),
+                       lambda: self.operand(bn, B, bfresh, "act"))
 
-    def nbytes(self):
-        tot, seen = 0, set()
-
-        def add(t):
-            nonlocal tot
-            if isinstance(t, torch.Tensor) and t.data_ptr() not in seen:
-                seen.add(t.data_ptr())
-                tot += t.numel() * t.element_size()
+    def tensors(self):
+        """Every tensor the plan owns, the GEMM operand buffers included."""
         for v in self.__dict__.values():
             for t in (v if isinstance(v, list) else [v]):
-                add(t)
+                if isinstance(t, torch.Tensor):
+                    yield t
         for op in self._ops.values():
-            add(op.hi)
-            add(op.lo)
-        return tot
+            yield from (t for t in (op.hi, op.lo, op.alpha, op.amax) if t is not None)
+
+    def nbytes(self):
+        seen = {t.data_ptr(): t.numel() * t.element_size() for t in self.tensors()}
+        return sum(seen.values())
 
 
 def sinc_constants(k, sr, device):
@@ -471,7 +377,7 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
     plan.generation += 1
     P = lambda name: _flat(params[name])
     buf = lambda name: _flat(mod.get_buffer(name))
-    fmt, ybf = plan.fmt, plan.y_bf16
+    fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
 
     g0 = G[0]
     call("pase_reflect_pad_wave", x.reshape(-1), plan.apad[0], plan.apad_lo[0], fmt, N, plan.T,
@@ -486,7 +392,7 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
     for l, g in enumerate(G):
         if not g.sinc:
             hi, lo = plan.w_operand(("Wt", l), plan.Wt[l])
-            dst = plan.Wt[l] if plan.mode in (None, 0, 1) else None
+            dst = plan.Wt[l] if plan.precision.fmt == gemm.FMT_F32 else None
             jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
                          1, 1, g.Cout * g.Cin * g.k))
     if jobs:
@@ -535,7 +441,7 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
             dst_lo = None if plan.xq_lo is None else plan.xq_lo[C:]
             d_ss, d_rs, pl, pr = (Tq + 1) * C, C, 0, 0
         else:
-            dst, dst_lo, dfmt, d_ss, d_rs, pl, pr = plan.cat, None, FMT_F32, Tq * Kc, Kc, 0, 0
+            dst, dst_lo, dfmt, d_ss, d_rs, pl, pr = plan.cat, None, gemm.FMT_F32, Tq * Kc, Kc, 0, 0
         if plan.skips and l + 1 < plan.nblk:
             pool, pd = plan.cat[plan.col_off[l]:], plan.pool_d[l]
         else:
@@ -626,13 +532,13 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     sb.zero_()
     if plan.amax is not None:
         plan.amax.zero_()
-    fmt, ybf = plan.fmt, plan.y_bf16
+    fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
     # dgrad operands (operand format) of every conv block with an input gradient: one launch
     jobs = []
     for l, g in enumerate(G):
         if not g.sinc and l > 0:
             hi, lo = plan.w_operand(("Wd", l), plan.Wd[l])
-            dst = plan.Wd[l] if plan.mode in (None, 0, 1) else None
+            dst = plan.Wd[l] if plan.precision.fmt == gemm.FMT_F32 else None
             jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
                          g.s, g.taps, g.s * g.Cin * g.taps * g.Cout))
     if jobs:
@@ -731,25 +637,13 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
         # gradient sources (no du tensor: one activation-sized write + read less per block)
         src = (s["A"], s["a_bf16"], s["a_ss"], s["a_rs"], s["padL"], s["padR"],
                s["B"], s["b_ss"], s["b_rs"], s["b_shift"], pool, Tq * Kc, Kc, pd, Tq)
-        if os.environ.get("PASE_B200_BN_DU") == "1":      # debug: two passes with a stored du
-            du = torch.empty(N * d_ss + 64, dtype=plan.y[l].dtype, device=plan.y[l].device)
-            call("pase_bn_prelu_bwd_reduce", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, mean, invstd,
-                 scale, shift, P(pre + "act.weight"), *src, du, d_ss, S1, S2, dal, amax)
-            call("pase_bn_prelu_bwd_apply", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, mean, invstd,
-                 P(pre + "norm.weight"), S1 if training else zeros[:C],
-                 S2 if training else zeros[C:2 * C], float(N * g.T_out), du, dst, dst_lo, fmt, d_ss,
-                 None if g.sinc else dbi, amax, plan.gscale[l])
-            _bn_du_debug = True
-        else:
-            _bn_du_debug = False
-            call("pase_bn_prelu_bwd_reduce", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, mean, invstd,
-                 scale, shift, P(pre + "act.weight"), *src, None, d_ss, S1, S2, dal, amax)
+        call("pase_bn_prelu_bwd_reduce", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, mean, invstd,
+             scale, shift, P(pre + "act.weight"), *src, None, d_ss, S1, S2, dal, amax)
         if training:
             a1, a2 = S1, S2
         else:
             a1, a2 = zeros[:C], zeros[C:2 * C]
-        if not _bn_du_debug:
-          call("pase_bn_prelu_bwd_apply_src", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, mean, invstd,
+        call("pase_bn_prelu_bwd_apply_src", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, mean, invstd,
              P(pre + "norm.weight"), scale, shift, P(pre + "act.weight"), a1, a2,
              float(N * g.T_out), *src, dst, dst_lo, fmt, d_ss, None if g.sinc else dbi, amax,
              plan.gscale[l])

@@ -143,7 +143,7 @@ class WaveFe(Model):
         if cfg["norm_out"]:
             self.norm_out = nn.BatchNorm1d(emb, affine=False)
         self._plans = OrderedDict()
-        # GEMM numerics (encoder.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (wgmma,
+        # GEMM numerics (gemm.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (wgmma,
         # fp32-equivalent), "tf32" (wgmma), "bf16" (wgmma, bf16 operands and activations)
         self.precision = os.environ.get("PASE_B200_PRECISION", DEFAULT_PRECISION)
         self._sinc_n = self._sinc_win = None

@@ -9,20 +9,27 @@ import os
 
 import torch
 
-from . import ops
+from . import gemm, ops
 
 # GEMM numerics of the heads (same meaning as WaveFe.precision): "3xf16" / "3xtf32" (wgmma,
 # fp32-equivalent products), "tf32", "bf16" (bf16 operands, fp32 everything else), or "fp32"
 # (FFMA kernels).
 PRECISION = os.environ.get("PASE_B200_PRECISION", "3xf16")
-_MODES = {"fp32": None, "3xtf32": 1, "tf32": 0, "bf16": 2, "3xf16": 3}
 
 
 def set_precision(p):
     global PRECISION
-    if p not in _MODES:
-        raise ValueError("precision must be one of %s" % sorted(_MODES))
+    if p not in gemm.PRECISIONS:
+        raise ValueError("precision must be one of %s" % sorted(gemm.PRECISIONS))
     PRECISION = p
+
+
+def gemm_precision():
+    """The heads' precision record (gemm.PRECISIONS)."""
+    return gemm.PRECISIONS[PRECISION]
+
+
+_F16X3 = gemm.PRECISIONS["3xf16"]          # the fused regression head's only format
 
 
 def _ru4(n):
@@ -33,102 +40,11 @@ def _ru(n, m):
     return (n + m - 1) // m * m
 
 
-def _eb(mode):
-    """elements per 128-byte TMA row of the GEMM operands"""
-    return 64 if mode in (2, 3) else 32
-
-
 def _pad_ld(n):
     """leading dimension of a rows-matrix with n columns: tensor-core modes pad to one
     128-byte row so the matrix can itself be a TMA operand."""
-    mode = _MODES[PRECISION]
-    return _ru4(n) if mode is None else _ru(n, _eb(mode))
-
-
-class Operand(object):
-    """A GEMM operand converted to the current mode's format: hi / lo tensors + the device
-    scalar that undoes a gradient's power-of-two scale (3xF16)."""
-    __slots__ = ("hi", "lo", "alpha")
-
-    def __init__(self, hi, lo=None, alpha=None):
-        self.hi, self.lo, self.alpha = hi, lo, alpha
-
-
-def to_operand(flat, n, mode, kind="act"):
-    """flat: fp32 1-D view (>= n elements).  kind: 'act' | 'weight' | 'grad'."""
-    if isinstance(flat, Operand):
-        return flat
-    dev = flat.device
-    if mode == 0:
-        return Operand(flat)
-    if mode == 1:
-        lo = torch.empty(n, dtype=torch.float32, device=dev)
-        if kind == "weight":
-            hi = torch.empty(n, dtype=torch.float32, device=dev)
-            ops.call("pase_split_tf32", flat, hi, lo, n)
-            return Operand(hi, lo)
-        ops.call("pase_split_tf32", flat, None, lo, n)
-        return Operand(flat, lo)
-    if mode == 2:
-        hi = torch.empty(n, dtype=torch.bfloat16, device=dev)
-        ops.call("pase_cast_bf16", flat, hi, n)
-        return Operand(hi)
-    hi = torch.empty(n, dtype=torch.float16, device=dev)
-    lo = torch.empty(n, dtype=torch.float16, device=dev)
-    if kind == "grad":
-        amax = torch.zeros(2, dtype=torch.float32, device=dev)
-        scale = torch.empty(2, dtype=torch.float32, device=dev)
-        ops.call("pase_absmax", flat, n, amax)
-        ops.call("pase_split_f16", flat, hi, lo, n, amax, scale)
-        return Operand(hi, lo, scale)
-    ops.call("pase_split_f16", flat, hi, lo, n, None, None)
-    return Operand(hi, lo)
-
-
-def gemm_nt(A, lda, a_used, B, ldb, b_used, C, ldc, M, N, K, bias, rows_in=None, t_valid=None,
-            rows_out=None, a_kind="act"):
-    """C[map(m),n] = sum_k A[m*lda+k] B[n*ldb+k] + bias[n]; dispatches wgmma / FFMA.
-    Optional row map (rows_in, t_valid, rows_out) as in pase_gemm_nt.  A / B may be fp32 flat
-    views or already-converted Operands."""
-    mode = _MODES[PRECISION]
-    if rows_in is None:
-        rows_in = t_valid = rows_out = M
-    esz = 2 if mode in (2, 3) else 4
-    if mode is None or lda % _eb(mode) != 0 or (K * esz) % 16 != 0 or (ldb * esz) % 16 != 0:
-        assert not isinstance(A, Operand) and not isinstance(B, Operand)
-        return ops.call("pase_gemm_nt", A, lda, B, ldb, C, ldc, M, N, K, 1.0, bias,
-                        rows_in, t_valid, rows_out, 1, None, None, 0)
-    a = to_operand(A, a_used, mode, a_kind)
-    b = to_operand(B, b_used, mode, "weight")
-    return ops.call("pase_tc_gemm_nt", a.hi, a.lo, a_used // lda, lda, b.hi, b.lo, ldb, C, ldc,
-                    M, N, K, 1.0, a.alpha, bias, rows_in, t_valid, rows_out, 1, None, None, 0,
-                    mode, 0)
-
-
-def gemm_tn(A, lda, a_used, B, ldb, b_used, C, ldc, I, J, rows, groups=1, pitchA=None, offA=0,
-            pitchB=None, a_kind="grad"):
-    """C[i,j] = sum_r A[rowA(r)*lda+i] B[rowB(r)*ldb+j] over `groups` x `rows` rows."""
-    mode = _MODES[PRECISION]
-    pitchA = rows if pitchA is None else pitchA
-    pitchB = rows if pitchB is None else pitchB
-    esz = 2 if mode in (2, 3) else 4
-    if mode is None or ldb % _eb(mode) != 0 or (lda * esz) % 16 != 0 or I % 4 != 0 or \
-            J % _eb(mode) != 0:
-        assert not isinstance(A, Operand) and not isinstance(B, Operand)
-        return ops.call("pase_gemm_tn", A, lda, pitchA, offA, B, ldb, pitchB, 0, C, ldc, I, J,
-                        groups, rows, 1.0, 0)
-    a = to_operand(A, a_used, mode, a_kind)
-    b = to_operand(B, b_used, mode, "act")
-    return ops.call("pase_tc_gemm_tn", a.hi, a.lo, lda, pitchA, offA, b.hi, b.lo, ldb, pitchB,
-                    b_used // ldb, C, ldc, I, J, groups, rows, 1.0, a.alpha, 0, mode)
-
-
-def tc_shapes_ok(lda, K, ldb):
-    """True when gemm_nt would take the tensor-core path in the current mode."""
-    mode = _MODES[PRECISION]
-    esz = 2 if mode in (2, 3) else 4
-    return mode is not None and lda % _eb(mode) == 0 and (K * esz) % 16 == 0 and \
-        (ldb * esz) % 16 == 0
+    p = gemm_precision()
+    return _ru(n, p.eb) if p.tc else _ru4(n)
 
 
 def _rows_ld(x):
@@ -177,14 +93,12 @@ class _LinearRows(torch.autograd.Function):
             out[:, N:].zero_()
         # the input is a GEMM operand twice (A here, B of the weight-gradient GEMM in
         # backward): convert it to the operand format once and keep it
-        xop = _flat_from(x)
-        mode = _MODES[PRECISION]
-        if mode not in (None, 0) and tc_shapes_ok(ldx, K, K):
-            xop = to_operand(xop, rows * ldx, mode, "act")
-        gemm_nt(xop, ldx, rows * ldx, w2.reshape(-1), K, N * K, out.reshape(-1), ldo,
-                rows, N, K, None if bias is None else bias.detach().reshape(-1))
+        p, xf = gemm_precision(), _flat_from(x)
+        xop = gemm.to_operand(p, xf, rows * ldx) if gemm.nt_ok(p, ldx, K, K) else None
+        gemm.nt(p, xf, ldx, rows * ldx, w2.reshape(-1), K, out.reshape(-1), ldo, rows, N, K,
+                bias=None if bias is None else bias.detach().reshape(-1), a_op=xop)
         ctx.save_for_backward(x, w2)
-        ctx.xop = xop if isinstance(xop, Operand) else None
+        ctx.xop = xop
         ctx.ldx, ctx.N, ctx.has_bias, ctx.wshape, ctx.ldo = ldx, N, bias is not None, \
             weight.shape, ldo
         return out
@@ -196,11 +110,11 @@ class _LinearRows(torch.autograd.Function):
         N, ldx, ldo = ctx.N, ctx.ldx, ctx.ldo
         assert dy.shape == (rows, ldo)
         dev = x.device
-        mode = _MODES[PRECISION]
+        p = gemm_precision()
         # the tensor-core weight-gradient kernel reads dY in whole 128-byte column blocks: a dY
         # whose leading dimension is a multiple of that block (every tensor-core mode pads so)
         # needs no slack; otherwise copy it into a buffer with 64 zeroed floats behind it
-        blk = _eb(mode) if mode is not None else 4
+        blk = p.eb if p.tc else 4
         if dy.is_contiguous() and ldo % blk == 0 and dy.data_ptr() % 16 == 0:
             dyb = dy.reshape(-1)
             n_dy = rows * ldo
@@ -209,25 +123,22 @@ class _LinearRows(torch.autograd.Function):
             dyb[:rows * ldo].view(rows, ldo).copy_(dy)
             dyb[rows * ldo:].zero_()
             n_dy = rows * ldo + 64
-        dyf = dyb
-        # dY feeds both backward GEMMs: convert it to the operand format once
-        if mode is not None and mode != 0 and tc_shapes_ok(ldo, ldo, ldo) and \
-                ldx % _eb(mode) == 0 and K % _eb(mode) == 0 and ldo % 4 == 0:
-            dyf = to_operand(dyb, n_dy, mode, "grad")
+        # dY feeds both backward GEMMs: when both take the tensor cores, convert it to the
+        # operand format once (and the weight gradient reuses the forward's operand of X)
+        dyop = None
+        if gemm.nt_ok(p, ldo, ldo, ldo) and gemm.tn_ok(p, ldo, ldx, ldo, K):
+            dyop = gemm.to_operand(p, dyb, n_dy, "grad")
         dx = dW = db = None
         if ctx.needs_input_grad[0]:
             wT = torch.empty(K, ldo, dtype=torch.float32, device=dev)
             ops.call("pase_transpose_pad", w2.reshape(-1), K, wT.reshape(-1), ldo, N, K)
             dx = torch.empty(rows, K, dtype=torch.float32, device=dev)
-            gemm_nt(dyf, ldo, rows * ldo, wT.reshape(-1), ldo, K * ldo, dx.reshape(-1), K,
-                    rows, K, ldo, None, a_kind="grad")
+            gemm.nt(p, dyb, ldo, rows * ldo, wT.reshape(-1), ldo, dx.reshape(-1), K, rows, K,
+                    ldo, a_kind="grad", a_op=dyop)
         if ctx.needs_input_grad[1]:
             dWp = torch.empty(ldo, K, dtype=torch.float32, device=dev)
-            xb = _flat_from(x)
-            if ctx.xop is not None and isinstance(dyf, Operand):
-                xb = ctx.xop                     # same format as the B operand of the TN GEMM
-            gemm_tn(dyf, ldo, rows * ldo, xb, ldx, rows * ldx, dWp.reshape(-1), K,
-                    ldo, K, rows)
+            gemm.tn(p, dyb, ldo, rows * ldo, _flat_from(x), ldx, rows * ldx, dWp.reshape(-1), K,
+                    ldo, K, rows, a_op=dyop, b_op=None if dyop is None else ctx.xop)
             dW = dWp[:N].reshape(ctx.wshape)
         dy = dyb[:rows * ldo].view(rows, ldo)
         if ctx.has_bias and ctx.needs_input_grad[2]:
@@ -352,8 +263,8 @@ class _FusedLinearCtxMSE(torch.autograd.Function):
         assert Fl == F and N == F * r and rows == B * T
         w2 = weight.detach().reshape(N, -1).contiguous()
         ldr = _ru(N, 128)
-        hop = to_operand(_flat_from(h), rows * ldh, 3, "act")
-        wop = to_operand(w2.reshape(-1), N * K, 3, "weight")
+        hop = gemm.to_operand(_F16X3, _flat_from(h), rows * ldh)
+        wop = gemm.to_operand(_F16X3, w2.reshape(-1), N * K, "weight")
         # power-of-two scale from the bound |residual| <= max||h_m|| max||W_n|| + max|b| + max|label|
         am = torch.zeros(4, dtype=torch.float32, device=dev)
         ops.call("pase_rownorm_max", _flat_from(h), ldh, rows, K, am[0:1])
@@ -389,17 +300,18 @@ class _FusedLinearCtxMSE(torch.autograd.Function):
         coef = 2.0 / float(rows * N)
         # d loss / d pred = g * coef * residual; the stored pair is s * residual
         adev = (g.detach().reshape(1).float() * coef) * scale[0:1]
-        rop = Operand(ent["hi"], ent["lo"], adev)
+        rop = gemm.Operand(ent["hi"], ent["lo"], adev)      # exists only as the fp16 pair
         dh = dW = db = None
         if ctx.needs_input_grad[0]:
             wT = torch.empty(K, ldr, dtype=torch.float32, device=dev)
             ops.call("pase_transpose_pad", w2.reshape(-1), K, wT.reshape(-1), ldr, N, K)
             dh = torch.empty(rows, K, dtype=torch.float32, device=dev)
-            gemm_nt(rop, ldr, rows * ldr, wT.reshape(-1), ldr, K * ldr, dh.reshape(-1), K,
-                    rows, K, ldr, None, a_kind="grad")
+            gemm.nt(_F16X3, None, ldr, rows * ldr, wT.reshape(-1), ldr, dh.reshape(-1), K,
+                    rows, K, ldr, a_kind="grad", a_op=rop)
         if ctx.needs_input_grad[1]:
             dWp = torch.empty(ldr, K, dtype=torch.float32, device=dev)
-            gemm_tn(rop, ldr, rows * ldr, ctx.hop, ldh, rows * ldh, dWp.reshape(-1), K, ldr, K, rows)
+            gemm.tn(_F16X3, None, ldr, rows * ldr, None, ldh, rows * ldh, dWp.reshape(-1), K,
+                    ldr, K, rows, a_op=rop, b_op=ctx.hop)
             dW = dWp[:N].reshape(wshape)
         if has_bias and ctx.needs_input_grad[2]:
             dbf = torch.empty(ldr, dtype=torch.float32, device=dev)
@@ -415,7 +327,7 @@ def fused_linear_ctx_mse(h, weight, bias, label, F, r):
 
 def fused_head_ok(K, ldh):
     """The fused output layer needs the 3xF16 tensor-core path."""
-    return _MODES[PRECISION] == 3 and ldh % 64 == 0 and K % 64 == 0
+    return gemm_precision() is _F16X3 and ldh % 64 == 0 and K % 64 == 0
 
 
 # ------------------------------------------------------------------ losses ---

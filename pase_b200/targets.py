@@ -17,7 +17,7 @@ import math
 import numpy as np
 import torch
 
-from . import ops
+from . import gemm, ops
 
 
 def savgol_taps(width, order):
@@ -107,7 +107,7 @@ class LPS(object):
         spec = torch.empty(rows * self.ldc, dtype=torch.float32, device=dev)
         ops.call("pase_tc_gemm_nt", a_hi, a_lo, rows, self.lda, c["hi"], c["lo"], self.lda, spec,
                  self.ldc, rows, 2 * self.nbins, self.lda, 1.0, None, None, rows, rows, rows, 1,
-                 None, None, 0, 3, 0)
+                 None, None, 0, gemm.PRECISIONS["3xf16"].mode, 0)
         F = (1 + self.der_order) * self.nbins
         out = torch.empty(B, F, frames, dtype=torch.float32, device=dev)
         ops.call("pase_lps_post", spec, self.ldc, B, frames, self.nbins, self.der_order,

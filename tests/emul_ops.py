@@ -578,8 +578,33 @@ def _operand(hi, lo, mode, n=None):
     return hi.float() + (lo if n is None else lo[:n]).float() / F16_LO_MUL
 
 
+def _tc_format(name, mode, Ahi, Alo, Bhi, Blo):
+    """The mode checks both tensor-core entry points share (csrc/gemm_tc.cu), and the element
+    type each mode reads; returns (element size, elements per 128-byte row)."""
+    assert mode in (0, 1, 2, 3), "%s: mode %r" % (name, mode)
+    assert mode not in (1, 3) or (Alo is not None and Blo is not None), \
+        "%s: split modes need lo operands" % name
+    dtype = (torch.float32, torch.float32, torch.bfloat16, torch.float16)[mode]
+    for t in (Ahi, Alo, Bhi, Blo):
+        assert t is None or t.dtype == dtype, "%s: mode %d operand dtype %s" % (name, mode, t.dtype)
+    esz = dtype.itemsize
+    return esz, 128 // esz
+
+
 def pase_tc_gemm_nt(Ahi, Alo, a_rows, R, Bhi, Blo, ldb, C, ldc, M, N, K, alpha, alpha_dev, bias,
                     rows_in, t_valid, rows_out, fold, colsum, colsumsq, accumulate, mode, c_bf16):
+    # the PASE_CHECK_ARG preconditions of the C entry point: a shape it refuses fails here
+    assert Ahi is not None and Bhi is not None and M > 0 and N > 0 and K > 0
+    esz, eb = _tc_format("pase_tc_gemm_nt", mode, Ahi, Alo, Bhi, Blo)
+    assert R >= eb and R % eb == 0, "pase_tc_gemm_nt: R=%d must be a multiple of %d" % (R, eb)
+    assert (K * esz) % 16 == 0 and (ldb * esz) % 16 == 0 and ldb >= K, \
+        "pase_tc_gemm_nt: K/ldb alignment (K=%d ldb=%d)" % (K, ldb)
+    assert Ahi.data_ptr() % 16 == 0 and Bhi.data_ptr() % 16 == 0, \
+        "pase_tc_gemm_nt: operand alignment"
+    assert rows_in > 0 and rows_out > 0 and fold > 0 and N % fold == 0, \
+        "pase_tc_gemm_nt: bad row map"
+    assert (colsum is None) == (colsumsq is None) and (colsum is None or N <= 4096) and \
+        (colsum is None or not accumulate), "pase_tc_gemm_nt: statistics"
     Alo, Blo = _like(Alo, Ahi), _like(Blo, Bhi)
     need = M * R + K
     A = torch.zeros(need)
@@ -601,6 +626,12 @@ def pase_tc_gemm_nt(Ahi, Alo, a_rows, R, Bhi, Blo, ldb, C, ldc, M, N, K, alpha, 
 
 def pase_tc_gemm_tn(Ahi, Alo, lda, pitchA, offA, Bhi, Blo, R, pitchB, b_rows_total, C, ldc, I, J,
                     groups, rows_per_group, alpha, alpha_dev, accumulate, mode):
+    assert Ahi is not None and Bhi is not None and I > 0 and J > 0 and groups > 0 and \
+        rows_per_group > 0, "pase_tc_gemm_tn: bad args"
+    esz, eb = _tc_format("pase_tc_gemm_tn", mode, Ahi, Alo, Bhi, Blo)
+    assert R >= eb and R % eb == 0 and (lda * esz) % 16 == 0 and I % 4 == 0 and J % eb == 0, \
+        "pase_tc_gemm_tn: need R%%%d==0, lda*%d%%16==0, I%%4==0, J%%%d==0 (R=%d lda=%d I=%d J=%d)" \
+        % (eb, esz, eb, R, lda, I, J)
     Alo, Blo = _like(Alo, Ahi), _like(Blo, Bhi)
     A = _operand(Ahi, Alo, mode)
     needB = ((groups - 1) * pitchB + rows_per_group) * R + J

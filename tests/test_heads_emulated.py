@@ -66,8 +66,20 @@ def check_case(gold, meta, model, batch, device, rtol=1e-4, atol=1e-5):
     assert check_grads(grads, gold, 2e-3, 2e-4, l2_keys=dec) > 20
 
 
-@pytest.mark.parametrize("name", ["pase_mini_workers_1600", "pase_plus_workers_3200"])
-def test_pase_workers_host_logic(name, emulated):
+def _workers_case(name, precision):
+    # the heads' default precision keeps the bare case name as its test id
+    return pytest.param(name, precision, id=name if precision == "3xf16" else
+                        "%s-%s" % (name, precision))
+
+
+# tf32 and bf16 miss the fp32 bars by their operand formats
+@pytest.mark.parametrize("name,precision", [
+    _workers_case(n, p) for n in ("pase_mini_workers_1600", "pase_plus_workers_3200")
+    for p in ("3xf16", "3xtf32", "fp32")])
+def test_pase_workers_host_logic(name, precision, emulated, monkeypatch):
+    from pase_b200 import functional as Fn
+    monkeypatch.setattr(Fn, "PRECISION", Fn.PRECISION)       # restored after the test
+    Fn.set_precision(precision)
     gold, meta, model, batch = build_case(name)
     check_case(gold, meta, model, batch, "cpu")
 

@@ -165,8 +165,8 @@ def test_weight_batch_table_is_cached_and_rebuilt(emulated, monkeypatch):
     y2, g2 = step()
     assert [t for _, t, _ in seen] == [t for _, t, _ in first]       # same device tables
     plan = model._plan(x.shape[0], x.shape[2], x.device)
-    plan_ptrs = {t.untyped_storage().data_ptr() for v in plan.__dict__.values()
-                 for t in (v if isinstance(v, list) else [v]) if isinstance(t, torch.Tensor)}
+    plan_ptrs = {t.untyped_storage().data_ptr() for t in plan.tensors()}
+    assert all(op.hi.untyped_storage().data_ptr() in plan_ptrs for op in plan._ops.values())
     for k, g in g2.items():
         assert g.untyped_storage().data_ptr() not in plan_ptrs, k
         assert g1[k].untyped_storage().data_ptr() != g.untyped_storage().data_ptr() or \
