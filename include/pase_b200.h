@@ -305,6 +305,10 @@ int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst,
                        int N, int T, int H, void* stream);
 int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long lddh,
                        float* dY, int N, int T, int H, void* stream);
+/* Which kernels the two scans run for T time steps (host only, launches nothing): out1 =
+ * segments per block of the time-segmented kernels (16, 24 or 32; T <= 512), or 0 for the
+ * sequential kernels (T > 512). */
+int pase_qrnn_scan_plan(int T, int* out1);
 
 /* ---- worker losses (losses.py:6-37, utils.py:63-68) ----------------------- */
 /* pred (B*T, F*r) channel-last, label (B,F,T): sum (pred - ctx(label))^2 -> acc */

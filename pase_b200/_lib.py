@@ -137,6 +137,16 @@ def tc_gemm_tn_plan(I, J, groups, rows_per_group, mode):
     return out[0], out[1]
 
 
+def qrnn_scan_plan(T):
+    """Segments per block of the time-segmented QRNN scans for T time steps (16, 24, 32), or 0
+    when the sequential kernels run."""
+    out = (ctypes.c_int * 1)()
+    rc = lib().pase_qrnn_scan_plan(T, ctypes.cast(out, ctypes.c_void_p))
+    if rc != 0:
+        raise RuntimeError("pase_qrnn_scan_plan failed: " + last_error())
+    return out[0]
+
+
 def bn_bwd_plan(pass_, *args):
     """How a BatchNorm/PReLU backward pass runs on the current device: `args` as the
     pase_bn_bwd_plan arguments after `pass` up to dst_sample_stride (tensors or device

@@ -1240,6 +1240,7 @@ int pase_out_bwd_reduce(const float* dout, const float* dout_ntc, const float* y
                         double* S1, double* S2, void* stream) {
   PASE_CHECK_ARG((dout || dout_ntc) && y && mean && invstd && g_ntc && S1 && S2,
                  "pase_out_bwd_reduce: null pointer");
+  PASE_CHECK_ARG(N > 0 && T > 0 && C > 0, "pase_out_bwd_reduce: N=%d T=%d C=%d", N, T, C);
   dim3 grid((T + 31) / 32, (C + 31) / 32, N), block(32, 8);
   PASE_LAUNCH((out_bwd_reduce_kernel), grid, block, 0, (cudaStream_t)stream, dout, dout_ntc, y, mean, invstd,
                                                                   T, C, g_ntc, S1, S2);

@@ -4,7 +4,6 @@
 // Replaces torchqrnn's runtime-compiled recurrent_forget_mult kernels
 // (reference call site: pase/models/modules.py:52, frontend.py:256-259).
 #include "common.cuh"
-#include <cstdlib>
 
 namespace {
 
@@ -228,13 +227,11 @@ qrnn_scan_bwd_seg_kernel(const float* __restrict__ Y, const float* __restrict__ 
   }
 }
 
-inline bool seg_scan_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("PASE_B200_QRNN_SEG");
-    v = (e && atoi(e) == 0) ? 0 : 1;
-  }
-  return v == 1;
+// Segments per block of the time-segmented kernels for T time steps (the template width: 16,
+// 24 or 32), or 0 above MAX_SEGS segments, where only the sequential kernels apply.
+inline int seg_width(int T) {
+  const int nseg = (T + SEG - 1) / SEG;
+  return nseg <= 16 ? 16 : nseg <= 24 ? 24 : nseg <= MAX_SEGS ? MAX_SEGS : 0;
 }
 
 }  // namespace
@@ -243,14 +240,15 @@ extern "C" {
 
 int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst, int N, int T, int H,
                        void* stream) {
-  PASE_CHECK_ARG(Y && h && Cst && N > 0 && T > 0 && H > 0 && ldh >= H,
-                 "pase_qrnn_scan_fwd: bad args");
-  const int nseg = (T + SEG - 1) / SEG;
-  if (nseg <= MAX_SEGS && seg_scan_enabled()) {
-    if (nseg <= 16)
+  PASE_CHECK_ARG(Y && h && Cst, "pase_qrnn_scan_fwd: null pointer");
+  PASE_CHECK_ARG(N > 0 && T > 0 && H > 0, "pase_qrnn_scan_fwd: N=%d T=%d H=%d", N, T, H);
+  PASE_CHECK_ARG(ldh >= H, "pase_qrnn_scan_fwd: ldh=%ld < H=%d", ldh, H);
+  const int nseg = (T + SEG - 1) / SEG, width = seg_width(T);
+  if (width) {
+    if (width == 16)
       PASE_LAUNCH((qrnn_scan_fwd_seg_kernel<16>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
                   (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
-    else if (nseg <= 24)
+    else if (width == 24)
       PASE_LAUNCH((qrnn_scan_fwd_seg_kernel<24>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
                   (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
     else
@@ -267,14 +265,15 @@ int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst, int N, in
 
 int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long lddh, float* dY,
                        int N, int T, int H, void* stream) {
-  PASE_CHECK_ARG(Y && Cst && dh && dY && N > 0 && T > 0 && H > 0 && lddh >= H,
-                 "pase_qrnn_scan_bwd: bad args");
-  const int nseg = (T + SEG - 1) / SEG;
-  if (nseg <= MAX_SEGS && seg_scan_enabled()) {
-    if (nseg <= 16)
+  PASE_CHECK_ARG(Y && Cst && dh && dY, "pase_qrnn_scan_bwd: null pointer");
+  PASE_CHECK_ARG(N > 0 && T > 0 && H > 0, "pase_qrnn_scan_bwd: N=%d T=%d H=%d", N, T, H);
+  PASE_CHECK_ARG(lddh >= H, "pase_qrnn_scan_bwd: lddh=%ld < H=%d", lddh, H);
+  const int nseg = (T + SEG - 1) / SEG, width = seg_width(T);
+  if (width) {
+    if (width == 16)
       PASE_LAUNCH((qrnn_scan_bwd_seg_kernel<16>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
                   (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
-    else if (nseg <= 24)
+    else if (width == 24)
       PASE_LAUNCH((qrnn_scan_bwd_seg_kernel<24>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
                   (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
     else
@@ -286,6 +285,12 @@ int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long l
   dim3 grid((H + 127) / 128, N);
   PASE_LAUNCH((qrnn_scan_bwd_kernel), grid, 128, 0, (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
   PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd");
+  return PASE_OK;
+}
+
+int pase_qrnn_scan_plan(int T, int* out1) {
+  PASE_CHECK_ARG(out1 && T > 0, "pase_qrnn_scan_plan: bad args");
+  out1[0] = seg_width(T);
   return PASE_OK;
 }
 

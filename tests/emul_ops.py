@@ -346,7 +346,8 @@ def pase_cast_d2f(src, dst, n, scale):
 
 
 def pase_out_affine_nct(y, scale, shift, out, out_ntc, N, T, C):
-    v = y[:N * T * C].view(N, T, C) * scale[:C] + shift[:C]
+    # one rounding of y*scale + shift, as the kernel's fmaf
+    v = (y[:N * T * C].view(N, T, C).double() * scale[:C].double() + shift[:C].double()).float()
     out[:N * C * T] = v.permute(0, 2, 1).reshape(-1)
     if out_ntc is not None:
         out_ntc[:N * T * C] = v.reshape(-1)
