@@ -93,6 +93,21 @@ int pase_tc_gemm_nt(const void* Ahi, const void* Alo, long a_rows, int R,
                     int rows_in, int t_valid, int rows_out, int fold,
                     double* colsum, double* colsumsq, int accumulate, int mode, int c_bf16,
                     void* stream);
+/* Packed variable-length forms of pase_gemm_nt (FFMA) and pase_tc_gemm_nt (inference: alpha 1,
+ * no statistics, no accumulation).  Utterance i's GEMM rows are contiguous; each one's padded
+ * operand starts on a folded-row boundary, so a row reads the K elements of its own utterance
+ * and the loads are those of the uniform kernels.  Only the epilogue's row map differs: var_tab
+ * (DEVICE, 3*nvar+1 ints) = row0[0..nvar] (first GEMM row of each utterance, ascending; row0[nvar]
+ * = rows in use, <= M), orow0[nvar] (first output row), t_valid[nvar].  Row m of utterance i
+ * (u = m - row0[i]) stores element (u, n) at output row orow0[i] + u iff
+ * u*fold + n/(N/fold) < t_valid[i]; rows >= row0[nvar] store nothing. */
+int pase_gemm_nt_var(const float* A, long lda, const float* B, long ldb, float* C, long ldc,
+                     int M, int N, int K, const float* bias, const int* var_tab, int nvar,
+                     int fold, void* stream);
+int pase_tc_gemm_nt_var(const void* Ahi, const void* Alo, long a_rows, int R,
+                        const void* Bhi, const void* Blo, long ldb, void* C, long ldc,
+                        int M, int N, int K, const float* bias, const int* var_tab, int nvar,
+                        int fold, int mode, int c_bf16, void* stream);
 int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int offA,
                     const void* Bhi, const void* Blo, int R, int pitchB, long b_rows_total,
                     float* C, long ldc, int I, int J, int groups, int rows_per_group,
@@ -191,6 +206,10 @@ int pase_sinc_grad(const float* dWp, const float* low_hz, const float* band_hz,
 /* (N,T) waveform -> reflect-padded rows of pitch `pitch` elements */
 int pase_reflect_pad_wave(const float* x, void* dst, void* dst_lo, int dst_fmt, int N, int T,
                           int padL, int padR, long pitch, void* stream);
+/* Packed variable-length form: tab (DEVICE, nseg rows of 3 ints) {x_off, T, dst_off}: utterance
+ * x[x_off, +T) reflect-padded into dst[dst_off, +T+padL+padR); max_T >= every T. */
+int pase_reflect_pad_wave_var(const float* x, const int* tab, int nseg, int max_T, void* dst,
+                              void* dst_lo, int dst_fmt, int padL, int padR, void* stream);
 /* batch statistics -> per-channel affine; updates running stats (training) */
 int pase_bn_finalize(const double* colsum, const double* colsumsq, int C, int fold,
                      double count, const float* gamma, const float* beta,
@@ -209,6 +228,18 @@ int pase_bn_prelu_pad_fwd(const void* y, int y_bf16, long y_sample_stride, int N
                           int padL, int padR,
                           float* pool, long pool_sample_stride, long pool_row_stride,
                           int pool_d, int pool_T, void* stream);
+/* Packed variable-length form (eval BatchNorm: scale / shift from pase_bn_eval_affine): tab
+ * (DEVICE, nseg rows of 6 ints) {T, y_off, dst_off, pool_off, pool_d, pool_T}: utterance i's
+ * y[y_off + t*C + c] (t < T) -> dst[dst_off + tau*dst_row_stride + c] with its own reflect halo,
+ * and its own dense-skip pool (pool_d, pool_T; pool_T * pool_d <= T) into
+ * pool[pool_off + j*pool_row_stride + c] (pool zeroed by the caller; NULL: no pool).  sep != 0
+ * also writes zeros to the row ahead of each utterance (dst_off - dst_row_stride, C elements):
+ * the x_{t-1} of the QRNN's first step.  max_T >= every T.  One launch for all utterances. */
+int pase_bn_prelu_pad_fwd_var(const void* y, int y_bf16, const int* tab, int nseg, int max_T,
+                              int C, const float* scale, const float* shift, const float* alpha,
+                              void* dst, void* dst_lo, int dst_fmt, long dst_row_stride,
+                              int padL, int padR, float* pool, long pool_row_stride, int sep,
+                              void* stream);
 /* backward, pass 1: g = sum of gradient sources (srcA: fp32 or bf16 as its dgrad GEMM
  * wrote it; srcB / pool: fp32); du = PReLU'(u) g written to dst (same type as y; NULL:
  * not stored, see pase_bn_prelu_bwd_apply_src);
@@ -285,6 +316,13 @@ int pase_cast_d2f(const double* src, float* dst, int n, float scale, void* strea
 /* out (N,C,T) = y*scale+shift; optionally also the channel-last copy out_ntc */
 int pase_out_affine_nct(const float* y, const float* scale, const float* shift,
                         float* out, float* out_ntc, int N, int T, int C, void* stream);
+/* Packed variable-length output with select_output (pase/models/modules.py:62-74) fused:
+ * tab (DEVICE, nseg rows of 3 ints) {y_row, T, out_off}; h = y[y_row + t, :]*scale+shift;
+ * mode 0: out[out_off..] (C,T) = h; 1 (avg_norm): h - mean_t h; 2 (avg_concat): (2C,T) =
+ * [h ; mean_t h]; 3 (avg_norm_concat): [h - mean_t h ; mean_t h].  The time mean is a double
+ * sum in a fixed order. */
+int pase_out_affine_var(const float* y, const float* scale, const float* shift, float* out,
+                        const int* tab, int nseg, int C, int mode, void* stream);
 /* g_ntc = dout(N,C,T)^T + dout_ntc; S1 += g, S2 += g*xhat (double[C]) */
 int pase_out_bwd_reduce(const float* dout, const float* dout_ntc, const float* y,
                         const float* mean, const float* invstd, int N, int T, int C,
@@ -303,6 +341,11 @@ int pase_ntc_to_nct(const float* src, long src_row_stride, float* dst, int N, in
 /* Y (rows=N*T, 3H) pre-activations -> h (row stride ldh), cell state Cst (rows,H) */
 int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst,
                        int N, int T, int H, void* stream);
+/* Packed variable-length forward: tab (DEVICE, nseg rows of 2 ints) {row0, T}: rows row0 ..
+ * row0+T-1 of Y / h / Cst are one utterance.  Each utterance runs the kernel its own T selects
+ * (pase_qrnn_scan_plan), so its result is that of a B=1 scan.  Two launches. */
+int pase_qrnn_scan_fwd_var(const float* Y, float* h, long ldh, float* Cst, const int* tab,
+                           int nseg, int H, void* stream);
 int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long lddh,
                        float* dY, int N, int T, int H, void* stream);
 /* Which kernels the two scans run for T time steps (host only, launches nothing): out1 =

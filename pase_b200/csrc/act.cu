@@ -32,6 +32,33 @@ __global__ void reflect_pad_wave_kernel(const float* __restrict__ x, void* __res
   }
 }
 
+// Packed variable-length form: blockIdx.y = utterance, tab row {x_off, T, dst_off}.
+template <int DF>
+__global__ void reflect_pad_wave_var_kernel(const float* __restrict__ x, const int* __restrict__ tab,
+                                            void* __restrict__ dst_v, void* __restrict__ dst_lo_v,
+                                            int padL, int padR) {
+  pdl_wait();
+  const int* r = tab + 3 * blockIdx.y;
+  const float* xn = x + __ldg(r);
+  const int T = __ldg(r + 1), Tp = T + padL + padR;
+  const long d0 = __ldg(r + 2);
+  for (int tau = blockIdx.x * blockDim.x + threadIdx.x; tau < Tp; tau += gridDim.x * blockDim.x) {
+    const float v = xn[reflect_idx(tau - padL, T)];
+    const long o = d0 + tau;
+    if constexpr (DF == PASE_FMT_F32) {
+      reinterpret_cast<float*>(dst_v)[o] = v;
+      if (dst_lo_v != nullptr) reinterpret_cast<float*>(dst_lo_v)[o] = tf32_residual(v);
+    } else if constexpr (DF == PASE_FMT_BF16) {
+      reinterpret_cast<__nv_bfloat16*>(dst_v)[o] = __float2bfloat16_rn(v);
+    } else {
+      __half h, l;
+      f16_split(v, h, l);
+      reinterpret_cast<__half*>(dst_v)[o] = h;
+      reinterpret_cast<__half*>(dst_lo_v)[o] = l;
+    }
+  }
+}
+
 __global__ void bn_finalize_kernel(const double* __restrict__ colsum,
                                    const double* __restrict__ colsumsq, int C, int fold,
                                    double count, const float* __restrict__ gamma,
@@ -89,24 +116,21 @@ __device__ __forceinline__ float prelu1(float u, float a) { return u > 0.f ? u :
 //   reads (i.e. after rounding to bf16 in the bf16 format); the thread that writes the first
 //   time step of a pooling window sums the whole window in time order, so each window mean
 //   has one writer and comes out the same on every run.
+// One sample: yn its raw conv output, dst / pool offsets d_base / p_base; thread idx owns the
+// channel quad idx % (C/4) over RUN time steps of the padded output.
 template <typename YT, int DF, int RUN>
-__global__ void __launch_bounds__(THREADS)
-bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
-                        const float* __restrict__ scale, const float* __restrict__ shift,
-                        const float* __restrict__ alpha, void* __restrict__ dst_v, long d_ss,
-                        long d_rs, int padL, int Tp, float* __restrict__ pool, long p_ss,
-                        long p_rs, int pool_d, int pool_T, void* __restrict__ dst_lo_v) {
-  pdl_wait();
+__device__ __forceinline__ void bn_prelu_pad_fwd_sample(
+    const YT* __restrict__ yn, long idx, int T, int C, const float* __restrict__ scale,
+    const float* __restrict__ shift, const float* __restrict__ alpha, void* __restrict__ dst_v,
+    long d_base, long d_rs, int padL, int Tp, float* __restrict__ pool, long p_base, long p_rs,
+    int pool_d, int pool_T, void* __restrict__ dst_lo_v) {
   const int C4 = C >> 2;
-  const int n = blockIdx.y;
-  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int q = (int)(idx % C4);
   const long run = idx / C4;
   const long tau0 = run * RUN;
   if (tau0 >= Tp) return;
   const int c = q * 4;
   const float4 sc = ld4(scale + c), sh = ld4(shift + c), al = ld4(alpha + c);
-  const YT* yn = y + (long)n * y_ss;
   const int pool_len = pool_d > 0 ? pool_T * pool_d : 0;
   const float inv_d = pool_d > 0 ? 1.f / (float)pool_d : 0.f;
   const int nvalid = (Tp - tau0) < RUN ? (int)(Tp - tau0) : RUN;
@@ -125,7 +149,7 @@ bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
     a.y = prelu1(fmaf(v.y, sc.y, sh.y), al.y);
     a.z = prelu1(fmaf(v.z, sc.z, sh.z), al.z);
     a.w = prelu1(fmaf(v.w, sc.w, sh.w), al.w);
-    const long o = (long)n * d_ss + tau * d_rs + c;
+    const long o = d_base + tau * d_rs + c;
     if constexpr (DF == PASE_FMT_F32) {
       st4(reinterpret_cast<float*>(dst_v) + o, a);
       if (dst_lo_v != nullptr)      // 3xTF32 residual of the operand just written
@@ -151,13 +175,60 @@ bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
         if constexpr (DF == PASE_FMT_BF16) b = rt4t(static_cast<const __nv_bfloat16*>(nullptr), b);
         ps.x += b.x; ps.y += b.y; ps.z += b.z; ps.w += b.w;
       }
-      float* pp = pool + (long)n * p_ss + (long)(tr / pool_d) * p_rs + c;
+      float* pp = pool + p_base + (long)(tr / pool_d) * p_rs + c;
       atomicAdd(pp + 0, ps.x * inv_d);
       atomicAdd(pp + 1, ps.y * inv_d);
       atomicAdd(pp + 2, ps.z * inv_d);
       atomicAdd(pp + 3, ps.w * inv_d);
     }
   }
+}
+
+template <typename YT, int DF, int RUN>
+__global__ void __launch_bounds__(THREADS)
+bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
+                        const float* __restrict__ scale, const float* __restrict__ shift,
+                        const float* __restrict__ alpha, void* __restrict__ dst_v, long d_ss,
+                        long d_rs, int padL, int Tp, float* __restrict__ pool, long p_ss,
+                        long p_rs, int pool_d, int pool_T, void* __restrict__ dst_lo_v) {
+  pdl_wait();
+  const int n = blockIdx.y;
+  bn_prelu_pad_fwd_sample<YT, DF, RUN>(y + (long)n * y_ss,
+                                       (long)blockIdx.x * blockDim.x + threadIdx.x, T, C, scale,
+                                       shift, alpha, dst_v, (long)n * d_ss, d_rs, padL, Tp, pool,
+                                       (long)n * p_ss, p_rs, pool_d, pool_T, dst_lo_v);
+}
+
+// Packed variable-length form: blockIdx.y = utterance, tab row {T, y_off, dst_off, pool_off,
+// pool_d, pool_T} (elements).  sep != 0: the row ahead of each utterance's output (dst_off -
+// d_rs, C elements) is written zero (the QRNN input's x_{-1} row).
+template <typename YT, int DF, int RUN>
+__global__ void __launch_bounds__(THREADS)
+bn_prelu_pad_fwd_var_kernel(const YT* __restrict__ y, const int* __restrict__ tab, int C,
+                            const float* __restrict__ scale, const float* __restrict__ shift,
+                            const float* __restrict__ alpha, void* __restrict__ dst_v, long d_rs,
+                            int padL, int padR, float* __restrict__ pool, long p_rs, int sep,
+                            void* __restrict__ dst_lo_v) {
+  pdl_wait();
+  const int* r = tab + 6 * blockIdx.y;
+  const int T = __ldg(r), pool_d = pool != nullptr ? __ldg(r + 4) : 0;
+  const long d_base = __ldg(r + 2);
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (sep && idx < (C >> 2)) {
+    const long o = d_base - d_rs + 4 * idx;
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (DF == PASE_FMT_F32) {
+      st4(reinterpret_cast<float*>(dst_v) + o, z);
+      if (dst_lo_v != nullptr) st4(reinterpret_cast<float*>(dst_lo_v) + o, z);
+    } else if constexpr (DF == PASE_FMT_BF16) {
+      st4t(reinterpret_cast<__nv_bfloat16*>(dst_v) + o, z);
+    } else {
+      st4_f16x2(reinterpret_cast<__half*>(dst_v) + o, reinterpret_cast<__half*>(dst_lo_v) + o, z);
+    }
+  }
+  bn_prelu_pad_fwd_sample<YT, DF, RUN>(y + __ldg(r + 1), idx, T, C, scale, shift, alpha, dst_v,
+                                       d_base, d_rs, padL, T + padL + padR, pool, __ldg(r + 3),
+                                       p_rs, pool_d, __ldg(r + 5), dst_lo_v);
 }
 
 // ---- backward pass 1: du + reductions ----
@@ -653,6 +724,59 @@ __global__ void out_affine_nct_kernel(const float* __restrict__ y, const float* 
   }
 }
 
+// Packed variable-length output: blockIdx.y = utterance, tab row {y_row, T, out_off}; block
+// (32, 8) owns 32 channels.  h = y*scale+shift as in out_affine_nct_kernel; the time mean of
+// each channel is a double sum in a fixed order (8 strided partial sums, then added in order).
+// mode 0: out (C,T) = h; 1: h - mean; 2: (2C,T) = [h ; mean]; 3: [h - mean ; mean].
+__global__ void __launch_bounds__(256)
+out_affine_var_kernel(const float* __restrict__ y, const float* __restrict__ scale,
+                      const float* __restrict__ shift, float* __restrict__ out,
+                      const int* __restrict__ tab, int C, int mode) {
+  pdl_wait();
+  __shared__ float tile[32][33];
+  __shared__ double part[8][32];
+  __shared__ float mean_s[32];
+  const int* r = tab + 3 * blockIdx.y;
+  const int T = __ldg(r + 1);
+  const float* yn = y + (long)__ldg(r) * C;
+  float* on = out + __ldg(r + 2);
+  const int c0 = blockIdx.x * 32, tx = threadIdx.x, ty = threadIdx.y;
+  const int c = c0 + tx;
+  const float sc = c < C ? scale[c] : 0.f, sh = c < C ? shift[c] : 0.f;
+  if (mode != 0) {
+    double s = 0.0;
+    if (c < C)
+      for (int t = ty; t < T; t += 8) s += (double)fmaf(yn[(long)t * C + c], sc, sh);
+    part[ty][tx] = s;
+    __syncthreads();
+    if (ty == 0) {
+      double m = 0.0;
+      for (int k = 0; k < 8; ++k) m += part[k][tx];
+      mean_s[tx] = (float)(m / (double)T);
+    }
+    __syncthreads();
+  }
+  const bool sub = mode == 1 || mode == 3, cat = mode >= 2;
+  for (int t0 = 0; t0 < T; t0 += 32) {
+    for (int i = ty; i < 32; i += 8) {
+      const int t = t0 + i;
+      if (t < T && c < C) {
+        const float v = fmaf(yn[(long)t * C + c], sc, sh);
+        tile[i][tx] = sub ? v - mean_s[tx] : v;
+      }
+    }
+    __syncthreads();
+    for (int i = ty; i < 32; i += 8) {
+      const int cc = c0 + i, t = t0 + tx;
+      if (t < T && cc < C) {
+        on[(long)cc * T + t] = tile[tx][i];
+        if (cat) on[(long)(C + cc) * T + t] = mean_s[i];
+      }
+    }
+    __syncthreads();
+  }
+}
+
 // g[n,t,c] = dout_nct[n,c,t] (+ dout_ntc[n,t,c]); S1 += g, S2 += g*xhat
 __global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
                                       const float* __restrict__ dout_ntc,
@@ -906,6 +1030,25 @@ int pase_reflect_pad_wave(const float* x, void* dst, void* dst_lo, int dst_fmt, 
   return PASE_OK;
 }
 
+int pase_reflect_pad_wave_var(const float* x, const int* tab, int nseg, int max_T, void* dst,
+                              void* dst_lo, int dst_fmt, int padL, int padR, void* stream) {
+  PASE_CHECK_ARG(x && tab && dst && nseg > 0 && max_T > 0, "pase_reflect_pad_wave_var: bad args");
+  PASE_CHECK_ARG(padL < max_T && padR < max_T && padL >= 0 && padR >= 0,
+                 "pase_reflect_pad_wave_var: reflect pad (%d,%d)", padL, padR);
+  PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2 && (dst_fmt != PASE_FMT_F16X2 || dst_lo),
+                 "pase_reflect_pad_wave_var: bad dst_fmt %d / missing lo", dst_fmt);
+  dim3 grid(blocks_for((long)max_T + padL + padR, 256, 4), nseg);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dst_fmt == PASE_FMT_F32)
+    PASE_LAUNCH((reflect_pad_wave_var_kernel<PASE_FMT_F32>), grid, 256, 0, st, x, tab, dst, dst_lo, padL, padR);
+  else if (dst_fmt == PASE_FMT_BF16)
+    PASE_LAUNCH((reflect_pad_wave_var_kernel<PASE_FMT_BF16>), grid, 256, 0, st, x, tab, dst, dst_lo, padL, padR);
+  else
+    PASE_LAUNCH((reflect_pad_wave_var_kernel<PASE_FMT_F16X2>), grid, 256, 0, st, x, tab, dst, dst_lo, padL, padR);
+  PASE_LAUNCH_CHECK("pase_reflect_pad_wave_var");
+  return PASE_OK;
+}
+
 int pase_bn_finalize(const double* colsum, const double* colsumsq, int C, int fold, double count,
                      const float* gamma, const float* beta, float* running_mean,
                      float* running_var, float momentum, float eps, float* mean, float* invstd,
@@ -984,6 +1127,53 @@ int pase_bn_prelu_pad_fwd(const void* y, int y_bf16, long y_sample_stride, int N
 #undef PASE_FWD
 #undef PASE_FWD_R
   PASE_LAUNCH_CHECK("pase_bn_prelu_pad_fwd");
+  return PASE_OK;
+}
+
+int pase_bn_prelu_pad_fwd_var(const void* y, int y_bf16, const int* tab, int nseg, int max_T,
+                              int C, const float* scale, const float* shift, const float* alpha,
+                              void* dst, void* dst_lo, int dst_fmt, long dst_row_stride,
+                              int padL, int padR, float* pool, long pool_row_stride, int sep,
+                              void* stream) {
+  const char* fn = "pase_bn_prelu_pad_fwd_var";
+  PASE_CHECK_ARG(y && tab && dst && scale && shift && alpha, "%s: null pointer", fn);
+  PASE_CHECK_ARG(nseg > 0 && max_T > 0 && C > 0 && (C % 4) == 0,
+                 "%s: nseg=%d max_T=%d C=%d (C a positive multiple of 4)", fn, nseg, max_T, C);
+  PASE_CHECK_ARG(padL >= 0 && padR >= 0, "%s: reflect pad (%d,%d)", fn, padL, padR);
+  PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2 && (dst_fmt != PASE_FMT_F16X2 || dst_lo),
+                 "%s: bad dst_fmt %d / missing lo", fn, dst_fmt);
+  {
+    const int dsz = dst_fmt == PASE_FMT_F32 ? 4 : 2;
+    PASE_CHECK_QUAD(fn, y, y_bf16 ? 2 : 4, "y");
+    PASE_CHECK_QUAD(fn, dst, dsz, "dst");
+    if (dst_lo) PASE_CHECK_QUAD(fn, dst_lo, dsz, "dst_lo");
+    PASE_CHECK_STRIDE(fn, dst_row_stride, "dst_row_stride");
+    if (pool) {
+      PASE_CHECK_QUAD(fn, pool, 4, "pool");
+      PASE_CHECK_STRIDE(fn, pool_row_stride, "pool_row_stride");
+    }
+  }
+  const int RUN = bn_run();
+  const long threads = (long)(C / 4) * (((long)max_T + padL + padR + RUN - 1) / RUN);
+  dim3 grid((unsigned)((threads + THREADS - 1) / THREADS), nseg);
+  cudaStream_t st = (cudaStream_t)stream;
+#define PASE_FWD_R(YT, DF, RV)                                                                 \
+  PASE_LAUNCH((bn_prelu_pad_fwd_var_kernel<YT, DF, RV>), grid, THREADS, 0, st,                \
+      reinterpret_cast<const YT*>(y), tab, C, scale, shift, alpha, dst, dst_row_stride, padL,  \
+      padR, pool, pool_row_stride, sep, dst_lo)
+#define PASE_FWD(YT, DF) do { if (RUN == 8) PASE_FWD_R(YT, DF, 8); else PASE_FWD_R(YT, DF, 4); } while (0)
+  if (y_bf16) {
+    if (dst_fmt == PASE_FMT_F32) PASE_FWD(__nv_bfloat16, PASE_FMT_F32);
+    else if (dst_fmt == PASE_FMT_BF16) PASE_FWD(__nv_bfloat16, PASE_FMT_BF16);
+    else PASE_FWD(__nv_bfloat16, PASE_FMT_F16X2);
+  } else {
+    if (dst_fmt == PASE_FMT_F32) PASE_FWD(float, PASE_FMT_F32);
+    else if (dst_fmt == PASE_FMT_BF16) PASE_FWD(float, PASE_FMT_BF16);
+    else PASE_FWD(float, PASE_FMT_F16X2);
+  }
+#undef PASE_FWD
+#undef PASE_FWD_R
+  PASE_LAUNCH_CHECK(fn);
   return PASE_OK;
 }
 
@@ -1232,6 +1422,17 @@ int pase_out_affine_nct(const float* y, const float* scale, const float* shift, 
   PASE_LAUNCH((out_affine_nct_kernel), grid, block, 0, (cudaStream_t)stream, y, scale, shift, out, out_ntc, T,
                                                                   C);
   PASE_LAUNCH_CHECK("pase_out_affine_nct");
+  return PASE_OK;
+}
+
+int pase_out_affine_var(const float* y, const float* scale, const float* shift, float* out,
+                        const int* tab, int nseg, int C, int mode, void* stream) {
+  PASE_CHECK_ARG(y && scale && shift && out && tab && nseg > 0 && C > 0,
+                 "pase_out_affine_var: bad args");
+  PASE_CHECK_ARG(mode >= 0 && mode <= 3, "pase_out_affine_var: mode %d", mode);
+  PASE_LAUNCH((out_affine_var_kernel), dim3((C + 31) / 32, nseg), dim3(32, 8), 0,
+              (cudaStream_t)stream, y, scale, shift, out, tab, C, mode);
+  PASE_LAUNCH_CHECK("pase_out_affine_var");
   return PASE_OK;
 }
 

@@ -114,6 +114,25 @@ __device__ __forceinline__ int reflect_idx(int t, int T) {
   return t;
 }
 
+// Packed variable-length row map of the *_gemm_nt_var entry points.  tab: 3n+1 ints, row0[0..n]
+// (first GEMM row of each utterance, ascending; row0[n] = rows in use), then orow0[n] (first
+// output row) and t_valid[n].  Row m of utterance i is its local row u = m - row0[i], stored at
+// output row orow0[i] + u.  Returns false for rows past row0[n].
+__device__ __forceinline__ bool var_row(const int* __restrict__ tab, int n, int m, int& orow,
+                                        int& t_valid, int& u) {
+  if (m >= __ldg(tab + n)) return false;
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(tab + mid) <= m) lo = mid;
+    else hi = mid - 1;
+  }
+  u = m - __ldg(tab + lo);
+  orow = __ldg(tab + n + 1 + lo) + u;
+  t_valid = __ldg(tab + 2 * n + 1 + lo);
+  return true;
+}
+
 // ---- storage formats of activation-sized tensors (C-ABI `*_fmt` / `*_bf16` arguments) ----
 //   PASE_FMT_F32     fp32 (optionally with a tf32-residual twin for the 3xTF32 GEMM mode)
 //   PASE_FMT_BF16    bf16

@@ -26,10 +26,12 @@ struct SmemNT {
 
 struct RowMap {
   int rows_in, t_valid, rows_out, fold, cols_per_fold;
+  const int* var_tab;              // packed variable-length map (var_row), VAR kernels only
+  int var_n;
 };
 
 // ------------------------------------------------------------------ NT ----
-template <int BN>
+template <int BN, bool VAR = false>
 __global__ void __launch_bounds__(NT, 2)
 gemm_nt_kernel(const float* __restrict__ A, long lda, const float* __restrict__ B, long ldb,
                float* __restrict__ C, long ldc, int M, int N, int K, float alpha,
@@ -131,9 +133,18 @@ gemm_nt_kernel(const float* __restrict__ A, long lda, const float* __restrict__ 
   for (int i = 0; i < 8; ++i) {
     const int m = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
     if (m >= M) continue;
-    const int g = m / rm.rows_in;
-    const int u = m - g * rm.rows_in;
-    const long orow = (long)g * rm.rows_out + u;
+    int u, t_valid;
+    long orow;
+    if constexpr (VAR) {
+      int o;
+      if (!var_row(rm.var_tab, rm.var_n, m, o, t_valid, u)) continue;
+      orow = o;
+    } else {
+      const int g = m / rm.rows_in;
+      u = m - g * rm.rows_in;
+      orow = (long)g * rm.rows_out + u;
+      t_valid = rm.t_valid;
+    }
 #pragma unroll
     for (int jq = 0; jq < TN / 4; ++jq) {
       const int nb = n0 + (jq == 0 ? tx * 4 : (BN / 2) + tx * 4);
@@ -142,7 +153,7 @@ gemm_nt_kernel(const float* __restrict__ A, long lda, const float* __restrict__ 
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int n = nb + j;
-        ok[j] = (n < N) && (u * rm.fold + (n / rm.cols_per_fold) < rm.t_valid);
+        ok[j] = (n < N) && (u * rm.fold + (n / rm.cols_per_fold) < t_valid);
         float x = acc[i][jq * 4 + j] * alpha;
         if (bias != nullptr && n < N) x += bias[n];
         v[j] = x;
@@ -337,19 +348,19 @@ gemm_tn_kernel(const float* __restrict__ A, long lda, const float* __restrict__ 
   }
 }
 
-template <int BN>
+template <int BN, bool VAR = false>
 int launch_nt(const float* A, long lda, const float* B, long ldb, float* C, long ldc, int M,
               int N, int K, float alpha, const float* bias, RowMap rm, double* colsum,
               double* colsumsq, int accumulate, cudaStream_t st) {
   static bool attr_set = false;
   const size_t smem = sizeof(SmemNT<BN>);
   if (!attr_set) {
-    cudaFuncSetAttribute(gemm_nt_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaFuncSetAttribute(gemm_nt_kernel<BN, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)smem);
     attr_set = true;
   }
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
-  gemm_nt_kernel<BN><<<grid, NT, smem, st>>>(A, lda, B, ldb, C, ldc, M, N, K, alpha, bias, rm,
+  gemm_nt_kernel<BN, VAR><<<grid, NT, smem, st>>>(A, lda, B, ldb, C, ldc, M, N, K, alpha, bias, rm,
                                             colsum, colsumsq, accumulate);
   PASE_LAUNCH_CHECK("pase_gemm_nt");
   return PASE_OK;
@@ -408,7 +419,7 @@ extern "C" int pase_gemm_nt(const float* A, long lda, const float* B, long ldb, 
                  rows_out, fold, N);
   PASE_CHECK_ARG((colsum == nullptr) == (colsumsq == nullptr),
                  "pase_gemm_nt: colsum and colsumsq must be given together");
-  RowMap rm{rows_in, t_valid, rows_out, fold, N / fold};
+  RowMap rm{rows_in, t_valid, rows_out, fold, N / fold, nullptr, 0};
   cudaStream_t st = (cudaStream_t)stream;
   if (N <= 64)
     return launch_nt<64>(A, lda, B, ldb, C, ldc, M, N, K, alpha, bias, rm, colsum, colsumsq,
@@ -433,4 +444,23 @@ extern "C" int pase_gemm_tn(const float* A, long lda, int pitchA, int offA, cons
   RedMap rm{rows_per_group, pitchA, offA, pitchB, offB, (long)groups * rows_per_group};
   if (J <= 64) return launch_tn<64>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, accumulate, st);
   return launch_tn<128>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, accumulate, st);
+}
+
+extern "C" int pase_gemm_nt_var(const float* A, long lda, const float* B, long ldb, float* C,
+                                long ldc, int M, int N, int K, const float* bias,
+                                const int* var_tab, int nvar, int fold, void* stream) {
+  PASE_CHECK_ARG(A && B && C && var_tab && nvar > 0, "pase_gemm_nt_var: null operand / table");
+  PASE_CHECK_ARG(M > 0 && N > 0 && K > 0, "pase_gemm_nt_var: bad shape M=%d N=%d K=%d", M, N, K);
+  PASE_CHECK_ARG((lda % 4) == 0 && (ldb % 4) == 0 && (K % 4) == 0,
+                 "pase_gemm_nt_var: lda, ldb, K must be multiples of 4 (lda=%ld ldb=%ld K=%d)",
+                 lda, ldb, K);
+  PASE_CHECK_ARG(aligned16(A) && aligned16(B), "pase_gemm_nt_var: A/B must be 16-byte aligned");
+  PASE_CHECK_ARG(fold > 0 && (N % fold) == 0, "pase_gemm_nt_var: fold=%d N=%d", fold, N);
+  RowMap rm{1, 0, 1, fold, N / fold, var_tab, nvar};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (N <= 64)
+    return launch_nt<64, true>(A, lda, B, ldb, C, ldc, M, N, K, 1.f, bias, rm, nullptr, nullptr,
+                               0, st);
+  return launch_nt<128, true>(A, lda, B, ldb, C, ldc, M, N, K, 1.f, bias, rm, nullptr, nullptr, 0,
+                              st);
 }

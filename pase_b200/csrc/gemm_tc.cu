@@ -260,6 +260,8 @@ __device__ __forceinline__ void fold_chunk(float (&sums)[NR], const float (&acc)
 
 struct RowMap {
   int rows_in, t_valid, rows_out, fold, cols_per_fold;
+  const int* var_tab;              // packed variable-length map (var_row), VAR kernels only
+  int var_n;
 };
 
 constexpr int NTHREADS = 384;
@@ -322,7 +324,7 @@ struct NTArgs {
 
 // Output stage of the NT kernel: alpha / bias, row map and validity, store (fp32 or bf16),
 // BatchNorm column statistics of the fp32 values (into shared-memory column sums).
-template <int NR, bool OUT16>
+template <int NR, bool OUT16, bool VAR>
 __device__ __forceinline__ void nt_output(float (&v)[NR], const NTArgs& a, float alpha,
                                           const Frag& f, double* s_stats) {
   const int N = a.N;
@@ -333,7 +335,14 @@ __device__ __forceinline__ void nt_output(float (&v)[NR], const NTArgs& a, float
     const int m = f.m[h];
     orow[h] = 0;
     nlim[h] = 0;
-    if (m < a.M) {
+    if constexpr (VAR) {
+      int o, tv, u;
+      if (m < a.M && var_row(a.rm.var_tab, a.rm.var_n, m, o, tv, u)) {
+        orow[h] = o;
+        const long lim = (long)(tv - u * a.rm.fold) * a.rm.cols_per_fold;
+        nlim[h] = lim <= 0 ? 0 : (lim >= N ? N : (int)lim);
+      }
+    } else if (m < a.M) {
       const int g = m / a.rm.rows_in;
       const int u = m - g * a.rm.rows_in;
       orow[h] = (long)g * a.rm.rows_out + u;
@@ -484,7 +493,7 @@ struct NTCfg {
   static constexpr int NR = BN / 2;                        // accumulator registers per thread
 };
 
-template <int BN, int MODE, bool OUT16, bool CTX>
+template <int BN, int MODE, bool OUT16, bool CTX, bool VAR = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo,
@@ -615,8 +624,8 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
       if constexpr (MT::SPLIT) nt_output_ctx<NR>(sums, a, alpha, f, cx_loss);
       else nt_output_ctx<NR>(acc, a, alpha, f, cx_loss);
     } else {
-      if constexpr (MT::SPLIT) nt_output<NR, OUT16>(sums, a, alpha, f, s_stats);
-      else nt_output<NR, OUT16>(acc, a, alpha, f, s_stats);
+      if constexpr (MT::SPLIT) nt_output<NR, OUT16, VAR>(sums, a, alpha, f, s_stats);
+      else nt_output<NR, OUT16, VAR>(acc, a, alpha, f, s_stats);
     }
   }
   if constexpr (CTX) {
@@ -946,7 +955,7 @@ int make_map(CUtensorMap* map, const void* base, int mode, int rank, const uint6
     }                                                                      \
   } while (0)
 
-template <int BN, int MODE, bool OUT16, bool CTX>
+template <int BN, int MODE, bool OUT16, bool CTX, bool VAR = false>
 int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
               const CUtensorMap& bl, NTArgs a, cudaStream_t st) {
   using Cfg = NTCfg<BN, MODE>;
@@ -959,7 +968,7 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
     return PASE_ERR_UNSUPPORTED;
   }
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt_kernel<BN, MODE, OUT16, CTX>,
+    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt_kernel<BN, MODE, OUT16, CTX, VAR>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
       pase_set_error("pase_tc_gemm_nt: smem attribute: %s", cudaGetErrorString(e));
@@ -969,7 +978,7 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
   }
   const long tiles = (long)((a.N + BN - 1) / BN) * ((a.M + BM - 1) / BM);
   const int grid = (int)(tiles < pase_num_sms() ? tiles : pase_num_sms());
-  PASE_LAUNCH((tc_gemm_nt_kernel<BN, MODE, OUT16, CTX>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
+  PASE_LAUNCH((tc_gemm_nt_kernel<BN, MODE, OUT16, CTX, VAR>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
   PASE_TC_LAUNCH_CHECK(CTX ? "pase_tc_gemm_nt_ctxmse" : "pase_tc_gemm_nt");
   return PASE_OK;
 }
@@ -1101,11 +1110,17 @@ int pase_split_tf32(const float* x, float* hi, float* lo, long n, void* stream) 
 
 // A: [a_rows x R] elements (hi / lo parts; lo NULL outside the split modes); B: [N x K]
 // (ldb >= K).  Element type by mode: fp32 (0, 1), bf16 (2), fp16 (3).
-int pase_tc_gemm_nt(const void* Ahi, const void* Alo, long a_rows, int R, const void* Bhi,
+}  // extern "C"
+
+namespace {
+
+// pase_tc_gemm_nt and pase_tc_gemm_nt_var: var_tab == nullptr selects the uniform row map
+int tc_gemm_nt_impl(const void* Ahi, const void* Alo, long a_rows, int R, const void* Bhi,
                     const void* Blo, long ldb, void* C, long ldc, int M, int N, int K,
                     float alpha, const float* alpha_dev, const float* bias, int rows_in,
                     int t_valid, int rows_out, int fold, double* colsum, double* colsumsq,
-                    int accumulate, int mode, int c_bf16, void* stream) {
+                    int accumulate, int mode, int c_bf16, const int* var_tab, int var_n,
+                    void* stream) {
   PASE_CHECK_ARG(Ahi && Bhi && C && M > 0 && N > 0 && K > 0, "pase_tc_gemm_nt: bad args");
   PASE_CHECK_ARG(mode >= 0 && mode <= 3, "pase_tc_gemm_nt: mode %d (0 tf32, 1 3xtf32, 2 bf16, "
                  "3 3xf16)", mode);
@@ -1151,26 +1166,53 @@ int pase_tc_gemm_nt(const void* Ahi, const void* Alo, long a_rows, int R, const 
   NTArgs a;
   a.R = R; a.C = C; a.ldc = ldc; a.M = M; a.N = N; a.K = K; a.alpha = alpha;
   a.alpha_dev = alpha_dev; a.bias = bias;
-  a.rm = RowMap{rows_in, t_valid, rows_out, fold, N / fold};
+  a.rm = RowMap{rows_in, t_valid, rows_out, fold, N / fold, var_tab, var_n};
   a.colsum = colsum; a.colsumsq = colsumsq; a.accumulate = accumulate; a.flush_kb = flush_kb;
   a.stages = 0; a.stat_cols = 0;
   a.cx_label = nullptr; a.cx_F = a.cx_T = a.cx_r = a.cx_nvalid = 0; a.cx_scale = nullptr;
   a.cx_lo = nullptr; a.cx_loss = nullptr; a.cx_db = nullptr;
   cudaStream_t st = (cudaStream_t)stream;
-#define PASE_NT(BNV)                                                                       \
+#define PASE_NT(BNV, VARV)                                                                 \
   switch (mode * 2 + (c_bf16 ? 1 : 0)) {                                                   \
-    case 0: return launch_nt<BNV, 0, false, false>(ah, al, bh, bl, a, st);                 \
-    case 1: return launch_nt<BNV, 0, true, false>(ah, al, bh, bl, a, st);                  \
-    case 2: return launch_nt<BNV, 1, false, false>(ah, al, bh, bl, a, st);                 \
-    case 3: return launch_nt<BNV, 1, true, false>(ah, al, bh, bl, a, st);                  \
-    case 4: return launch_nt<BNV, 2, false, false>(ah, al, bh, bl, a, st);                 \
-    case 5: return launch_nt<BNV, 2, true, false>(ah, al, bh, bl, a, st);                  \
-    case 6: return launch_nt<BNV, 3, false, false>(ah, al, bh, bl, a, st);                 \
-    default: return launch_nt<BNV, 3, true, false>(ah, al, bh, bl, a, st);                 \
+    case 0: return launch_nt<BNV, 0, false, false, VARV>(ah, al, bh, bl, a, st);           \
+    case 1: return launch_nt<BNV, 0, true, false, VARV>(ah, al, bh, bl, a, st);            \
+    case 2: return launch_nt<BNV, 1, false, false, VARV>(ah, al, bh, bl, a, st);           \
+    case 3: return launch_nt<BNV, 1, true, false, VARV>(ah, al, bh, bl, a, st);            \
+    case 4: return launch_nt<BNV, 2, false, false, VARV>(ah, al, bh, bl, a, st);           \
+    case 5: return launch_nt<BNV, 2, true, false, VARV>(ah, al, bh, bl, a, st);            \
+    case 6: return launch_nt<BNV, 3, false, false, VARV>(ah, al, bh, bl, a, st);           \
+    default: return launch_nt<BNV, 3, true, false, VARV>(ah, al, bh, bl, a, st);           \
   }
-  if (BN == 64) { PASE_NT(64) }
-  PASE_NT(128)
+  if (var_tab != nullptr) {
+    if (BN == 64) { PASE_NT(64, true) }
+    PASE_NT(128, true)
+  }
+  if (BN == 64) { PASE_NT(64, false) }
+  PASE_NT(128, false)
 #undef PASE_NT
+}
+
+}  // namespace
+
+extern "C" {
+
+int pase_tc_gemm_nt(const void* Ahi, const void* Alo, long a_rows, int R, const void* Bhi,
+                    const void* Blo, long ldb, void* C, long ldc, int M, int N, int K,
+                    float alpha, const float* alpha_dev, const float* bias, int rows_in,
+                    int t_valid, int rows_out, int fold, double* colsum, double* colsumsq,
+                    int accumulate, int mode, int c_bf16, void* stream) {
+  return tc_gemm_nt_impl(Ahi, Alo, a_rows, R, Bhi, Blo, ldb, C, ldc, M, N, K, alpha, alpha_dev,
+                         bias, rows_in, t_valid, rows_out, fold, colsum, colsumsq, accumulate,
+                         mode, c_bf16, nullptr, 0, stream);
+}
+
+int pase_tc_gemm_nt_var(const void* Ahi, const void* Alo, long a_rows, int R, const void* Bhi,
+                        const void* Blo, long ldb, void* C, long ldc, int M, int N, int K,
+                        const float* bias, const int* var_tab, int nvar, int fold, int mode,
+                        int c_bf16, void* stream) {
+  PASE_CHECK_ARG(var_tab && nvar > 0, "pase_tc_gemm_nt_var: empty utterance table");
+  return tc_gemm_nt_impl(Ahi, Alo, a_rows, R, Bhi, Blo, ldb, C, ldc, M, N, K, 1.f, nullptr, bias,
+                         1, 0, 1, fold, nullptr, nullptr, 0, mode, c_bf16, var_tab, nvar, stream);
 }
 
 // Fused output layer of a regression head (MLPMinion W + ContextualizedLoss MSE,
@@ -1207,7 +1249,7 @@ int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
   NTArgs a;
   a.R = R; a.C = Rhi; a.ldc = ldr; a.M = M; a.N = (int)ldr; a.K = K; a.alpha = 1.f;
   a.alpha_dev = nullptr; a.bias = bias;
-  a.rm = RowMap{M, M, M, 1, (int)ldr};
+  a.rm = RowMap{M, M, M, 1, (int)ldr, nullptr, 0};
   a.colsum = nullptr; a.colsumsq = nullptr; a.accumulate = 0;
   a.flush_kb = K > 512 ? 2 : 0;
   a.stages = 0; a.stat_cols = 0;

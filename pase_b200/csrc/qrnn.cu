@@ -11,16 +11,9 @@ constexpr int UNROLL = 8;
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 
-__global__ void __launch_bounds__(128)
-qrnn_scan_fwd_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
-                     float* __restrict__ Cst, int T, int H) {
-  pdl_wait();
-  const int n = blockIdx.y;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= H) return;
-  const float* y = Y + (long)n * T * 3 * H + c;
-  float* hp = h + (long)n * T * ldh + c;
-  float* cp = Cst + (long)n * T * H + c;
+// One sample's sequential scan of hidden unit c: y / hp / cp point at its first time step.
+__device__ __forceinline__ void qrnn_fwd_seq(const float* __restrict__ y, float* __restrict__ hp,
+                                             long ldh, float* __restrict__ cp, int T, int H) {
   float cprev = 0.f;
   int t = 0;
   for (; t + UNROLL <= T; t += UNROLL) {
@@ -45,6 +38,17 @@ qrnn_scan_fwd_kernel(const float* __restrict__ Y, float* __restrict__ h, long ld
     cp[(long)t * H] = cprev;
     hp[(long)t * ldh] = oo * cprev;
   }
+}
+
+__global__ void __launch_bounds__(128)
+qrnn_scan_fwd_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
+                     float* __restrict__ Cst, int T, int H) {
+  pdl_wait();
+  const int n = blockIdx.y;
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= H) return;
+  qrnn_fwd_seq(Y + (long)n * T * 3 * H + c, h + (long)n * T * ldh + c, ldh,
+               Cst + (long)n * T * H + c, T, H);
 }
 
 __global__ void __launch_bounds__(128)
@@ -112,18 +116,16 @@ qrnn_scan_bwd_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
 constexpr int SEG = 16;
 constexpr int MAX_SEGS = 32;
 
-template <int NSEG_MAX>
-__global__ void __launch_bounds__(32 * NSEG_MAX, 1)
-qrnn_scan_fwd_seg_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
-                         float* __restrict__ Cst, int T, int H) {
-  pdl_wait();
-  __shared__ float sA[MAX_SEGS][33], sB[MAX_SEGS][33];
-  const int lane = threadIdx.x, seg = threadIdx.y, n = blockIdx.y;
+// One sample's segmented scan: rows row0 .. row0+T-1 of Y / h / Cst; segment threadIdx.y.
+__device__ __forceinline__ void qrnn_fwd_seg(const float* __restrict__ Y, float* __restrict__ h,
+                                             long ldh, float* __restrict__ Cst, long row0, int T,
+                                             int H, float (*sA)[33], float (*sB)[33]) {
+  const int lane = threadIdx.x, seg = threadIdx.y;
   const int c = blockIdx.x * 32 + lane;
   const bool live = c < H;
   const int t0 = seg * SEG;
   const int len = (T - t0) < SEG ? (T - t0) : SEG;
-  const float* y = Y + ((long)n * T + t0) * 3 * H + c;
+  const float* y = Y + (row0 + t0) * 3 * H + c;
   float z[SEG], f[SEG], o[SEG];
 #pragma unroll
   for (int i = 0; i < SEG; ++i) {
@@ -151,8 +153,8 @@ qrnn_scan_fwd_seg_kernel(const float* __restrict__ Y, float* __restrict__ h, lon
   float cin = 0.f;
   for (int s2 = 0; s2 < seg; ++s2) cin = sA[s2][lane] * cin + sB[s2][lane];
   if (!live) return;
-  float* hp = h + ((long)n * T + t0) * ldh + c;
-  float* cp = Cst + ((long)n * T + t0) * H + c;
+  float* hp = h + (row0 + t0) * ldh + c;
+  float* cp = Cst + (row0 + t0) * H + c;
 #pragma unroll
   for (int i = 0; i < SEG; ++i) {
     if (i < len) {
@@ -161,6 +163,15 @@ qrnn_scan_fwd_seg_kernel(const float* __restrict__ Y, float* __restrict__ h, lon
       hp[(long)i * ldh] = o[i] * ct;
     }
   }
+}
+
+template <int NSEG_MAX>
+__global__ void __launch_bounds__(32 * NSEG_MAX, 1)
+qrnn_scan_fwd_seg_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
+                         float* __restrict__ Cst, int T, int H) {
+  pdl_wait();
+  __shared__ float sA[MAX_SEGS][33], sB[MAX_SEGS][33];
+  qrnn_fwd_seg(Y, h, ldh, Cst, (long)blockIdx.y * T, T, H, sA, sB);
 }
 
 template <int NSEG_MAX>
@@ -234,9 +245,49 @@ inline int seg_width(int T) {
   return nseg <= 16 ? 16 : nseg <= 24 ? 24 : nseg <= MAX_SEGS ? MAX_SEGS : 0;
 }
 
+// Packed variable-length forms: blockIdx.y = utterance, tab row {row0, T}.  Each utterance
+// runs the algorithm its own length selects (seg_width), so it gets the bits of a B=1 scan:
+// the segmented kernel skips utterances longer than MAX_SEGS segments, the sequential one the
+// others.  Segments past an utterance's end scan nothing and pass the state through.
+__global__ void __launch_bounds__(32 * MAX_SEGS, 1)
+qrnn_scan_fwd_seg_var_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
+                             float* __restrict__ Cst, const int* __restrict__ tab, int H) {
+  pdl_wait();
+  __shared__ float sA[MAX_SEGS][33], sB[MAX_SEGS][33];
+  const int T = __ldg(tab + 2 * blockIdx.y + 1);
+  if (T > SEG * MAX_SEGS) return;
+  qrnn_fwd_seg(Y, h, ldh, Cst, __ldg(tab + 2 * blockIdx.y), T, H, sA, sB);
+}
+
+__global__ void __launch_bounds__(128)
+qrnn_scan_fwd_seq_var_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
+                             float* __restrict__ Cst, const int* __restrict__ tab, int H) {
+  pdl_wait();
+  const int T = __ldg(tab + 2 * blockIdx.y + 1);
+  const long row0 = __ldg(tab + 2 * blockIdx.y);
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (T <= SEG * MAX_SEGS || c >= H) return;
+  qrnn_fwd_seq(Y + row0 * 3 * H + c, h + row0 * ldh + c, ldh, Cst + row0 * H + c, T, H);
+}
+
 }  // namespace
 
 extern "C" {
+
+int pase_qrnn_scan_fwd_var(const float* Y, float* h, long ldh, float* Cst, const int* tab,
+                           int nseg, int H, void* stream) {
+  PASE_CHECK_ARG(Y && h && Cst && tab, "pase_qrnn_scan_fwd_var: null pointer");
+  PASE_CHECK_ARG(nseg > 0 && H > 0 && ldh >= H, "pase_qrnn_scan_fwd_var: nseg=%d H=%d ldh=%ld",
+                 nseg, H, ldh);
+  cudaStream_t st = (cudaStream_t)stream;
+  PASE_LAUNCH((qrnn_scan_fwd_seg_var_kernel), dim3((H + 31) / 32, nseg), dim3(32, MAX_SEGS), 0,
+              st, Y, h, ldh, Cst, tab, H);
+  PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd_var");
+  PASE_LAUNCH((qrnn_scan_fwd_seq_var_kernel), dim3((H + 127) / 128, nseg), 128, 0, st, Y, h, ldh,
+              Cst, tab, H);
+  PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd_var");
+  return PASE_OK;
+}
 
 int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst, int N, int T, int H,
                        void* stream) {

@@ -16,6 +16,8 @@ projection (mean-pool commutes with a bias-free 1x1 conv, frontend.py:182,
 skips and the QRNN output are concatenated so W + all skips are one GEMM.
 """
 import math
+
+import numpy as np
 import torch
 
 from . import gemm, ops
@@ -111,13 +113,25 @@ class EncoderPlan(object):
       3xf16: GEMM operands as fp16 (hi, lo') pairs, everything else fp32."""
 
     def __init__(self, cfg, N, T, device, prec="fp32"):
-        self.cfg, self.N, self.T, self.device = cfg, N, T, device
+        self.N, self.T = N, T
+        self._setup(cfg, device, prec, lambda fold: build_geometry(cfg, T, fold))
+        G = self.geoms
+        self.Tq = G[-1].T_out
+        self.pool_d = [max(g.T_out // self.Tq, 1) for g in G[:-1]]
+        self.rows = N * self.Tq
+        self._alloc([N * g.apad_floats for g in G], [N * g.rows_out * g.Nn for g in G],
+                    self.rows, N * (self.Tq + 1))
+
+    def _setup(self, cfg, device, prec, geometry):
+        """Length-independent state: precision, layer shapes (geometry(sinc_fold) -> geoms),
+        column layout of the output projection's operand."""
+        self.cfg, self.device = cfg, device
         if prec not in gemm.PRECISIONS:
             raise ValueError("precision must be one of %s" % (sorted(gemm.PRECISIONS),))
         self.precision = p = gemm.PRECISIONS[prec]
         self._ops = {}             # name -> gemm.Operand
         self._wtables = {}
-        self.geoms = build_geometry(cfg, T, p.sinc_fold)
+        self.geoms = geometry(p.sinc_fold)
         G = self.geoms
         if p.esz == 2:
             for g in G:
@@ -126,13 +140,25 @@ class EncoderPlan(object):
                         "precision %r needs channel counts that are multiples of %d (block %d: "
                         "Cin=%d Cout=%d stride=%d)" % (prec, p.eb, g.idx, g.Cin, g.Cout, g.s))
         self.nblk = len(G)
-        self.Tq = G[-1].T_out
         self.emb = cfg["emb_dim"]
         self.rnn = bool(cfg["rnn_pool"])
         self.skips = bool(cfg["denseskips"])
         self.norm_out = bool(cfg["norm_out"])
         self.Clast = G[-1].Cout
         self.H = (cfg["rnn_dim"] // 2) * 2 if self.rnn else 0
+        # concatenated [rnn-out | pooled skips] operand of the output projection
+        self.col_off = []
+        off = self.H if self.rnn else self.Clast
+        for g in G[:-1]:
+            self.col_off.append(off)
+            if self.skips:
+                off += g.Cout
+        self.Kc = off
+
+    def _alloc(self, n_apad, n_y, rows, xq_rows):
+        """Forward buffers: padded operands of n_apad[l] elements (+ slack), raw conv outputs of
+        n_y[l], `rows` output frames, `xq_rows` rows of the QRNN input."""
+        G, p, device = self.geoms, self.precision, self.device
         f32 = dict(dtype=torch.float32, device=device)
         f64 = dict(dtype=torch.float64, device=device)
         opd = dict(dtype=p.dtype, device=device)
@@ -142,31 +168,19 @@ class EncoderPlan(object):
         zo = lambda n: torch.zeros(int(n), **opd)          # operand-format buffers (hi / lo)
         zlo = lambda n: torch.zeros(int(n), **opd) if p.split else None
 
-        # concatenated [rnn-out | pooled skips] operand of the output projection
-        self.col_off = []
-        off = self.H if self.rnn else self.Clast
-        for g in G[:-1]:
-            self.col_off.append(off)
-            if self.skips:
-                off += g.Cout
-        self.Kc = off
-        self.pool_d = [max(g.T_out // self.Tq, 1) for g in G[:-1]]
-
         self.apad, self.apad_lo, self.y, self.bn = [], [], [], []
         self.Wt = []
-        for g in G:
-            n_apad = N * g.apad_floats + g.K + 64
+        for g, na, ny in zip(G, n_apad, n_y):
+            n_apad = na + g.K + 64
             self.apad.append(zo(n_apad))
             self.apad_lo.append(zlo(n_apad))
             self._ops[("apad", g.idx)] = gemm.Operand(self.apad[-1], self.apad_lo[-1])
-            self.y.append(torch.empty(int(N * g.rows_out * g.Nn), **yd))
+            self.y.append(torch.empty(int(ny), **yd))
             self.bn.append(torch.zeros(4, g.Cout, **f32))       # mean, invstd, scale, shift
             self.Wt.append(e(g.Nn * g.K))
-        rows = N * self.Tq
-        self.rows = rows
         if self.rnn:
             Cq, H = self.Clast, self.H
-            n_xq = N * (self.Tq + 1) * Cq + 2 * Cq + 64
+            n_xq = xq_rows * Cq + 2 * Cq + 64
             self.xq, self.xq_lo = zo(n_xq), zlo(n_xq)
             self._ops["xq"] = gemm.Operand(self.xq, self.xq_lo)
             self.Yg, self.Cst = e(rows * 3 * H), e(rows * H)
@@ -259,11 +273,12 @@ class EncoderPlan(object):
         self.backward_ready = True
 
     # -- GEMM operands -----------------------------------------------------------------
-    def operand(self, name, buf, fresh=True, kind="act"):
+    def operand(self, name, buf, fresh=True, kind="act", n=None):
         """Operand `name` in the plan's GEMM format (gemm.Operand).  Operands whose producer
         writes the GEMM format directly (apad, xq, dyz, the conv weights) are registered with
         no fp32 source; everything else is the fp32 tensor `buf` converted into buffers kept
-        per name (`fresh=False` reuses this step's earlier conversion)."""
+        per name (`fresh=False` reuses this step's earlier conversion; `n`: convert only the
+        first n elements)."""
         op = self._ops.get(name)
         if op is not None and op.src is None:
             return op
@@ -272,7 +287,8 @@ class EncoderPlan(object):
                                       torch.zeros)
             self._ops[name] = op
             fresh = True
-        return gemm.convert(self.precision, op, buf.numel(), kind) if fresh else op
+        n = buf.numel() if n is None else n
+        return gemm.convert(self.precision, op, n, kind) if fresh else op
 
     def w_operand(self, name, buf):
         """(hi, lo) buffers of a weight operand written by pase_conv_w_batch itself."""
@@ -321,6 +337,13 @@ class EncoderPlan(object):
                        lambda: self.operand(an, A, afresh, akind),
                        lambda: self.operand(bn, B, bfresh, "weight"))
 
+    def nt_var(self, an, A, lda, bn, B, ldb, bfresh, C, ldc, M, N, K, bias, tab, n, fold):
+        """gemm.nt_var over the packed operand `an` (written in the GEMM format by its
+        producer) and the weight operand `bn`."""
+        return gemm.nt_var(self.precision, A, lda, A.numel(), B, ldb, C, ldc, M, N, K, bias, tab,
+                           n, fold, lambda: self.operand(an, A, False),
+                           lambda: self.operand(bn, B, bfresh, "weight"))
+
     def tn(self, an, A, lda, pitchA, offA, afresh, bn, B, ldb, pitchB, bfresh, C, ldc, I, J,
            groups, rpg, alpha, acc, akind="grad"):
         """C = alpha * A^T B in the plan's precision (gemm.tn)."""
@@ -368,6 +391,58 @@ def _flat(t):
     return t.detach().reshape(-1)
 
 
+# -- weight preparation shared by encoder_forward and encoder_forward_packed -----------------
+def _conv_weight_operands(plan, P):
+    """GEMM operands (in the plan's operand format) of every conv block's weight: one launch."""
+    jobs = []
+    for l, g in enumerate(plan.geoms):
+        if not g.sinc:
+            hi, lo = plan.w_operand(("Wt", l), plan.Wt[l])
+            dst = plan.Wt[l] if plan.precision.fmt == gemm.FMT_F32 else None
+            jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
+                         1, 1, g.Cout * g.Cin * g.k))
+    if jobs:
+        plan.w_batch(0, jobs)
+
+
+def _sinc_weights(plan, mod, P, l, g):
+    pre = "blocks.%d." % l
+    ops.call("pase_sinc_make", P(pre + "conv.low_hz_"), P(pre + "conv.band_hz_"),
+             mod._sinc_n, mod._sinc_win, None, plan.Wt[l], g.Cout, g.k, g.fold, g.K,
+             50.0, 50.0, float(plan.cfg["sr"]))
+
+
+def _bn_eval_affine(plan, P, buf, l, g):
+    pre = "blocks.%d." % l
+    mean, invstd, scale, shift = plan.bn[l][0], plan.bn[l][1], plan.bn[l][2], plan.bn[l][3]
+    ops.call("pase_bn_eval_affine", buf(pre + "norm.running_mean"),
+             buf(pre + "norm.running_var"), P(pre + "norm.weight"), P(pre + "norm.bias"),
+             g.Cout, BN_EPS, mean, invstd, scale, shift)
+
+
+def _qrnn_weights(plan, params):
+    """Gate weights in the GEMM's [x_{t-1} | x_t] column order."""
+    Cq, H = plan.Clast, plan.H
+    Wl = params["rnn.layers.0.linear.weight"].detach()
+    torch.cat([Wl[:, Cq:], Wl[:, :Cq]], 1, out=plan.Wq.view(3 * H, 2 * Cq))
+
+
+def _out_weights(plan, params):
+    """[W | dense skips] of the output projection."""
+    emb = plan.emb
+    parts = [params["W.weight"].detach().reshape(emb, -1)]
+    if plan.skips:
+        parts += [params["denseskips.%d.weight" % i].detach().reshape(emb, -1)
+                  for i in range(plan.nblk - 1)]
+    torch.cat(parts, 1, out=plan.Wcat.view(emb, plan.Kc))
+
+
+def _out_bn_eval_affine(plan, buf):
+    bo = plan.bn_out
+    ops.call("pase_bn_eval_affine", buf("norm_out.running_mean"), buf("norm_out.running_var"),
+             None, None, plan.emb, BN_EPS, bo[0], bo[1], bo[2], bo[3])
+
+
 def encoder_forward(plan, mod, x, params, training, save_for_backward):
     """x: (N,1,T) fp32 CUDA tensor.  params: dict name -> tensor.  Returns
     (out (N,emb,Tq), out_ntc (N*Tq, emb))."""
@@ -387,24 +462,13 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
     if plan.skips:
         plan.cat.zero_()
 
-    # GEMM operands (in the plan's operand format) of every conv block's weight: one launch
-    jobs = []
-    for l, g in enumerate(G):
-        if not g.sinc:
-            hi, lo = plan.w_operand(("Wt", l), plan.Wt[l])
-            dst = plan.Wt[l] if plan.precision.fmt == gemm.FMT_F32 else None
-            jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
-                         1, 1, g.Cout * g.Cin * g.k))
-    if jobs:
-        plan.w_batch(0, jobs)
+    _conv_weight_operands(plan, P)
     counters = []
 
     for l, g in enumerate(G):
         pre = "blocks.%d." % l
         if g.sinc:
-            call("pase_sinc_make", P(pre + "conv.low_hz_"), P(pre + "conv.band_hz_"),
-                 mod._sinc_n, mod._sinc_win, None, plan.Wt[l], g.Cout, g.k, g.fold, g.K,
-                 50.0, 50.0, float(cfg["sr"]))
+            _sinc_weights(plan, mod, P, l, g)
             bias = None
         else:
             bias = P(pre + "conv.bias")
@@ -426,9 +490,7 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
                  BN_MOMENTUM, BN_EPS, mean, invstd, scale, shift)
             counters.append(mod.get_buffer(pre + "norm.num_batches_tracked"))
         else:
-            call("pase_bn_eval_affine", buf(pre + "norm.running_mean"),
-                 buf(pre + "norm.running_var"), P(pre + "norm.weight"), P(pre + "norm.bias"),
-                 g.Cout, BN_EPS, mean, invstd, scale, shift)
+            _bn_eval_affine(plan, P, buf, l, g)
         C = g.Cout
         # the producer writes the next GEMM's operand in its own format (3xTF32: + the tf32
         # residual twin; 3xF16: the fp16 pair)
@@ -452,19 +514,13 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
 
     if plan.rnn:
         Cq, H = plan.Clast, plan.H
-        Wl = params["rnn.layers.0.linear.weight"].detach()
-        Wq = plan.Wq.view(3 * H, 2 * Cq)
-        torch.cat([Wl[:, Cq:], Wl[:, :Cq]], 1, out=Wq)               # [x_{t-1} | x_t] order
+        _qrnn_weights(plan, params)
         plan.nt("xq", plan.xq, Cq, False, "Wq", plan.Wq, 2 * Cq, True, plan.Yg, 3 * H,
                 N * (Tq + 1), 3 * H, 2 * Cq, 1.0, P("rnn.layers.0.linear.bias"),
                 Tq + 1, Tq, Tq, 1, None, None, 0)
         call("pase_qrnn_scan_fwd", plan.Yg, plan.cat, Kc, plan.Cst, N, Tq, H)
 
-    parts = [params["W.weight"].detach().reshape(emb, -1)]
-    if plan.skips:
-        parts += [params["denseskips.%d.weight" % i].detach().reshape(emb, -1)
-                  for i in range(plan.nblk - 1)]
-    torch.cat(parts, 1, out=plan.Wcat.view(emb, Kc))
+    _out_weights(plan, params)
     use_stats = plan.norm_out and training
     if use_stats:
         o = plan.fs_out
@@ -481,9 +537,7 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
                  BN_MOMENTUM, BN_EPS, bo[0], bo[1], bo[2], bo[3])
             counters.append(mod.get_buffer("norm_out.num_batches_tracked"))
         else:
-            call("pase_bn_eval_affine", buf("norm_out.running_mean"),
-                 buf("norm_out.running_var"), None, None, emb, BN_EPS,
-                 bo[0], bo[1], bo[2], bo[3])
+            _out_bn_eval_affine(plan, buf)
     if counters:                                 # BatchNorm step counters: one launch
         torch._foreach_add_(counters, 1)
     out = torch.empty(N, emb, Tq, dtype=torch.float32, device=x.device)
@@ -492,6 +546,227 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
          N, Tq, emb)
     plan.last_training = training
     return out, out_ntc
+
+
+# -- packed variable-length inference (DESIGN.md section 11) ----------------------------------
+INDEX_LIMIT = 2 ** 31          # the packed kernels' tables and row counts are 32-bit ints
+OUT_MODES = {None: 0, "avg_norm": 1, "avg_concat": 2, "avg_norm_concat": 3}
+
+
+def _accepts(cfg, T):
+    try:
+        build_geometry(cfg, T)
+        return True
+    except ValueError:
+        return False
+
+
+def min_length(cfg):
+    """Shortest waveform whose every block input is longer than its reflect pads."""
+    hi = 1
+    while not _accepts(cfg, hi):
+        hi *= 2
+    lo = hi // 2 + 1 if hi > 1 else 1
+    while lo < hi:
+        mid = (lo + hi) // 2
+        if _accepts(cfg, mid):
+            hi = mid
+        else:
+            lo = mid + 1
+    return lo
+
+
+def utterance_geometry(cfg, lengths, sinc_fold):
+    """Per-utterance block geometry; an utterance too short for a block's reflect pads raises
+    ValueError naming its index (and, from ConvGeom, the block)."""
+    out = []
+    for i, T in enumerate(lengths):
+        try:
+            out.append(build_geometry(cfg, T, sinc_fold))
+        except ValueError as e:
+            raise ValueError("utterance %d (%d samples): %s" % (i, T, e)) from None
+    return out
+
+
+def split_packs(lengths, max_samples):
+    """Greedy, in order: consecutive utterances while their sum fits max_samples; an utterance
+    longer than max_samples is a pack of its own.  -> list of (start, stop)."""
+    packs, start, total = [], 0, 0
+    for i, T in enumerate(lengths):
+        if i > start and total + T > max_samples:
+            packs.append((start, i))
+            start, total = i, 0
+        total += T
+    if lengths:
+        packs.append((start, len(lengths)))
+    return packs
+
+
+def packed_bounds(geoms, capacity, max_utts):
+    """Upper bounds, over every pack of at most `capacity` samples in at most `max_utts`
+    utterances, of the elements of each block's padded operand and raw output and of the
+    output frames.  Per utterance P = ceil(Tpad / r) <= Tpad / r + 1 and T_out = floor((Tpad -
+    k) / s) + 1, so sums over n utterances are bounded through the summed lengths."""
+    n = np.arange(1, max_utts + 1, dtype=np.int64)
+    L = np.full_like(n, capacity)
+    n_apad, n_y = [], []
+    for g in geoms:
+        r = g.fold if g.sinc else g.s
+        Tpad = L + n * (g.padL + g.padR)
+        n_apad.append(int(((Tpad // r + n) * g.lda).max()))
+        L = (Tpad - n * g.k) // g.s + n
+        n_y.append(int(((L // g.fold + n) * g.Nn).max()))
+    return n_apad, n_y, int(L.max())
+
+
+class PackedPlan(EncoderPlan):
+    """Forward buffers of packed variable-length inference (encoder_forward_packed) for packs
+    of up to `capacity` samples: sized by capacity, not by the lengths in a pack, so one plan
+    serves every pack that fits.  Holds the packed waveform and the device copy of the
+    per-utterance offset table."""
+
+    def __init__(self, cfg, capacity, device, prec="fp32"):
+        self.capacity = int(capacity)
+        self.min_len = min_length(cfg)
+        self._setup(cfg, device, prec, lambda fold: build_geometry(cfg, self.min_len, fold))
+        G = self.geoms
+        self.max_utts = max(self.capacity // self.min_len, 1)
+        n_apad, n_y, rows = packed_bounds(G, self.capacity, self.max_utts)
+        sizes = [("waveform", self.capacity)]
+        sizes += [("block %d operand" % g.idx, na + g.K + 64) for g, na in zip(G, n_apad)]
+        sizes += [("block %d output" % g.idx, ny) for g, ny in zip(G, n_y)]
+        sizes += [("output projection operand", rows * self.Kc),
+                  ("returned features", 2 * rows * self.emb)]
+        if self.rnn:
+            sizes += [("QRNN input", (rows + self.max_utts) * self.Clast + 2 * self.Clast + 64),
+                      ("QRNN gates", rows * 3 * self.H)]
+        for what, n in sizes:
+            if n >= INDEX_LIMIT:
+                raise ValueError(
+                    "a pack of %d samples needs %d elements for the %s, beyond the 32-bit indices "
+                    "of the packed kernels: split it into shorter utterances"
+                    % (self.capacity, n, what))
+        self.rows_cap = rows
+        self._alloc(n_apad, n_y, rows, rows + self.max_utts)
+        self.wave = torch.zeros(self.capacity, dtype=torch.float32, device=device)
+        self.table = torch.zeros(_table_size(self.nblk, self.max_utts), dtype=torch.int32,
+                                 device=device)
+
+
+def _table_size(nblk, n):
+    # wave, per block (GEMM map + BN/PReLU rows), QRNN GEMM map, scan, output
+    return 3 * n + nblk * (3 * n + 1 + 6 * n) + (3 * n + 1) + 2 * n + 3 * n
+
+
+def packed_layout(plan, lengths, geoms, mode):
+    """Offsets of every utterance at every layer, as the int32 table of the packed kernels.
+    -> (host table, {section: offset}, dict of sizes).  Utterance i's rows are contiguous at
+    every layer; each padded operand starts on a folded-row boundary of its GEMM."""
+    G, n = plan.geoms, len(lengths)
+    P = np.array([[g.P for g in gi] for gi in geoms], dtype=np.int64).reshape(n, plan.nblk)
+    RO = np.array([[g.rows_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
+    TO = np.array([[g.T_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
+    cum = lambda a: np.concatenate([np.zeros((1,) + a.shape[1:], np.int64), np.cumsum(a, 0)])
+    row0, orow0 = cum(P), cum(RO)
+    Tq = TO[:, -1]
+    q0, xr0 = cum(Tq), cum(Tq + 1)
+    E = plan.emb * (2 if mode in ("avg_concat", "avg_norm_concat") else 1)
+    o0 = cum(E * Tq)
+    x0 = cum(np.asarray(lengths, dtype=np.int64))
+    Kc, sec, parts = plan.Kc, {}, []
+
+    def put(name, *cols, rows=None):
+        sec[name] = sum(p.size for p in parts)
+        parts.append(np.stack(cols, 1).reshape(-1) if rows is None else np.concatenate(cols))
+
+    put("wave", x0[:n], np.asarray(lengths, np.int64), row0[:n, 0] * G[0].lda)
+    for l, g in enumerate(G):
+        put(("gemm", l), row0[:, l], orow0[:n, l], TO[:, l], rows=True)
+        if l + 1 < plan.nblk:
+            dst = row0[:n, l + 1] * G[l + 1].lda
+        elif plan.rnn:
+            dst = (xr0[:n] + 1) * g.Cout
+        else:
+            dst = q0[:n] * Kc
+        put(("bn", l), TO[:, l], orow0[:n, l] * g.Nn, dst, q0[:n] * Kc,
+            np.maximum(TO[:, l] // Tq, 1), Tq)
+    put("qgemm", xr0, q0[:n], Tq, rows=True)
+    put("scan", q0[:n], Tq)
+    put("out", q0[:n], Tq, o0[:n])
+    table = np.concatenate(parts)
+    assert table.size <= _table_size(plan.nblk, n) and table.max() < INDEX_LIMIT
+    sizes = dict(rows=int(q0[n]), xq_rows=int(xr0[n]), gemm_rows=[int(r) for r in row0[n]],
+                 max_T=int(max(lengths)), max_Tout=[int(t) for t in TO.max(0)],
+                 out=int(o0[n]), offsets=[int(o) for o in o0[:n]], Tq=[int(t) for t in Tq],
+                 E=E)
+    return torch.from_numpy(table.astype(np.int32)), sec, sizes
+
+
+def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None):
+    """Eval-mode forward of utterances packed in x (fp32, sum(lengths) samples, plan.wave):
+    each one computed as a B=1 forward would.  Launches do not depend on the number of
+    utterances.  Returns the list of (1, E, T'_i) features, views of one new buffer."""
+    call = ops.call
+    G, n = plan.geoms, len(lengths)
+    host, sec, sz = packed_layout(plan, lengths, geoms, mode)
+    plan.table[:host.numel()].copy_(host)                    # the one host-to-device copy
+    tab = lambda name: plan.table[sec[name]:]
+    P = lambda name: _flat(params[name])
+    buf = lambda name: _flat(mod.get_buffer(name))
+    fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
+    rows, Kc, emb = sz["rows"], plan.Kc, plan.emb
+
+    g0 = G[0]
+    call("pase_reflect_pad_wave_var", x, tab("wave"), n, sz["max_T"], plan.apad[0],
+         plan.apad_lo[0], fmt, g0.padL, g0.padR)
+    if plan.skips:
+        plan.cat[:rows * Kc].zero_()                         # the pools accumulate into it
+    _conv_weight_operands(plan, P)
+    for l, g in enumerate(G):
+        pre = "blocks.%d." % l
+        if g.sinc:
+            _sinc_weights(plan, mod, P, l, g)
+            bias = None
+        else:
+            bias = P(pre + "conv.bias")
+        plan.nt_var(("apad", l), plan.apad[l], g.lda, ("Wt", l), plan.Wt[l], g.K, g.sinc,
+                    plan.y[l], g.Nn, sz["gemm_rows"][l], g.Nn, g.K, bias, tab(("gemm", l)), n,
+                    g.fold)
+        _bn_eval_affine(plan, P, buf, l, g)
+        C, sep = g.Cout, 0
+        if l + 1 < plan.nblk:
+            nx = G[l + 1]
+            dst, dst_lo, dfmt, d_rs, pl, pr = plan.apad[l + 1], plan.apad_lo[l + 1], fmt, C, \
+                nx.padL, nx.padR
+        elif plan.rnn:
+            dst, dst_lo, dfmt, d_rs, pl, pr, sep = plan.xq, plan.xq_lo, fmt, C, 0, 0, 1
+        else:
+            dst, dst_lo, dfmt, d_rs, pl, pr = plan.cat, None, gemm.FMT_F32, Kc, 0, 0
+        pool = plan.cat[plan.col_off[l]:] if plan.skips and l + 1 < plan.nblk else None
+        call("pase_bn_prelu_pad_fwd_var", plan.y[l], ybf, tab(("bn", l)), n, sz["max_Tout"][l],
+             C, plan.bn[l][2], plan.bn[l][3], P(pre + "act.weight"), dst, dst_lo, dfmt, d_rs,
+             pl, pr, pool, Kc, sep)
+
+    if plan.rnn:
+        Cq, H = plan.Clast, plan.H
+        _qrnn_weights(plan, params)
+        plan.nt_var("xq", plan.xq, Cq, "Wq", plan.Wq, 2 * Cq, True, plan.Yg, 3 * H,
+                    sz["xq_rows"], 3 * H, 2 * Cq, P("rnn.layers.0.linear.bias"), tab("qgemm"), n,
+                    1)
+        call("pase_qrnn_scan_fwd_var", plan.Yg, plan.cat, Kc, plan.Cst, tab("scan"), n, H)
+
+    # the output projection is uniform over the sum of the frame counts
+    _out_weights(plan, params)
+    gemm.nt(plan.precision, plan.cat, Kc, rows * Kc, plan.Wcat, Kc, plan.yout, emb, rows, emb,
+            Kc, 1.0, P("W.bias"), a_op=lambda: plan.operand("cat", plan.cat, True, n=rows * Kc),
+            b_op=lambda: plan.operand("Wcat", plan.Wcat, True, "weight"))
+    bo = plan.bn_out
+    if plan.norm_out:
+        _out_bn_eval_affine(plan, buf)
+    out = torch.empty(sz["out"], dtype=torch.float32, device=x.device)
+    call("pase_out_affine_var", plan.yout, bo[2], bo[3], out, tab("out"), n, emb, OUT_MODES[mode])
+    E = sz["E"]
+    return [out[o:o + E * t].view(1, E, t) for o, t in zip(sz["offsets"], sz["Tq"])]
 
 
 def encoder_backward(plan, mod, params, gout, gntc, training, sink=None):

@@ -18,6 +18,7 @@ import torch.nn as nn
 
 from .modules import Model, format_frontend_chunk, format_frontend_output
 from . import encoder as _enc
+from . import gemm as _gemm
 
 # "3xtf32": wgmma tensor cores with error-compensated TF32 (fp32-equivalent, meets the
 # fp32 parity bar); "fp32": FFMA kernels; "tf32": single-pass TF32 (L2-equivalent only).
@@ -27,6 +28,11 @@ from . import encoder as _enc
 # operand bytes of 3xTF32) when every channel count is a multiple of 64 (PASE.cfg, PASE+.cfg),
 # else 3xTF32.  Both meet the fp32 parity bar (tests/test_encoder_gpu.py).
 DEFAULT_PRECISION = "auto"
+
+# Samples packed into one forward of WaveFe.extract (65.5 s of 16 kHz audio).  The packed plan
+# this sizes holds 1.35 GB for PASE+ in 3xf16 and 0.75 GB in bf16 (EncoderPlan.nbytes() after a
+# call, operand buffers included).
+EXTRACT_MAX_SAMPLES = 1 << 20
 
 _DEFAULTS = dict(
     num_inputs=1, sincnet=True,
@@ -143,6 +149,7 @@ class WaveFe(Model):
         if cfg["norm_out"]:
             self.norm_out = nn.BatchNorm1d(emb, affine=False)
         self._plans = OrderedDict()
+        self._packed_plans = OrderedDict()
         # GEMM numerics (gemm.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (wgmma,
         # fp32-equivalent), "tf32" (wgmma), "bf16" (wgmma, bf16 operands and activations)
         self.precision = os.environ.get("PASE_B200_PRECISION", DEFAULT_PRECISION)
@@ -195,6 +202,19 @@ class WaveFe(Model):
             self._plans.move_to_end(key)
         return plan
 
+    def _packed_plan(self, capacity, device):
+        prec = self.resolved_precision()
+        key = (capacity, str(device), prec)
+        plan = self._packed_plans.get(key)
+        if plan is None:
+            plan = _enc.PackedPlan(self.cfg, capacity, device, prec)
+            self._packed_plans[key] = plan
+            while len(self._packed_plans) > self.MAX_PLANS:
+                self._packed_plans.popitem(last=False)
+        else:
+            self._packed_plans.move_to_end(key)
+        return plan
+
     def _sinc_consts(self, device):
         if self._sinc_n is None or self._sinc_n.device != device:
             k = self.blocks[0].conv.kernel_size
@@ -221,6 +241,59 @@ class WaveFe(Model):
             return _enc._EncoderFn.apply(x, self, plan, self.training, names, *tensors)
         with torch.no_grad():
             return _enc.encoder_forward(plan, self, x, dict(named), self.training, False)
+
+    def extract(self, wavs, mode=None, max_samples=None):
+        """Features of many utterances of any lengths, packed into as few forwards as fit
+        `max_samples` samples each (default EXTRACT_MAX_SAMPLES; greedy, in order; a longer
+        utterance gets a forward of its own).  wavs: list of fp32 (T,), (1,T) or (1,1,T)
+        tensors, on the CPU or the GPU.  Returns, in input order, (1, emb', T'_i) CUDA tensors
+        equal to ``self(wavs[i].view(1,1,-1), mode=mode)`` (mode as select_output); they are
+        views of one buffer per forward.  Eval mode only: train-mode BatchNorm would couple
+        the utterances."""
+        if self.training:
+            raise RuntimeError("WaveFe.extract runs the encoder in eval mode; call .eval() first "
+                               "(train-mode BatchNorm statistics would mix the utterances)")
+        device = self.W.weight.device
+        if device.type != "cuda":
+            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; the module lives "
+                               "on %s. There is no CPU path." % device)
+        return self._extract(wavs, mode, max_samples, device)
+
+    def _extract(self, wavs, mode, max_samples, device):
+        if mode not in _enc.OUT_MODES:
+            raise ValueError("mode must be one of %s, got %r" % (list(_enc.OUT_MODES), mode))
+        cap = EXTRACT_MAX_SAMPLES if max_samples is None else int(max_samples)
+        if cap < 1:
+            raise ValueError("max_samples must be positive, got %r" % (max_samples,))
+        flat = []
+        for i, w in enumerate(wavs):
+            if not isinstance(w, torch.Tensor) or w.dtype != torch.float32:
+                raise TypeError("utterance %d: expected an fp32 tensor, got %s"
+                                % (i, getattr(w, "dtype", type(w))))
+            if w.dim() == 0 or w.dim() > 3 or any(d != 1 for d in w.shape[:-1]):
+                raise ValueError("utterance %d: expected (T,), (1,T) or (1,1,T), got %s"
+                                 % (i, tuple(w.shape)))
+            flat.append(w.reshape(-1))
+        if not flat:
+            return []
+        lengths = [w.numel() for w in flat]
+        fold = _gemm.PRECISIONS[self.resolved_precision()].sinc_fold
+        geoms = _enc.utterance_geometry(self.cfg, lengths, fold)
+        self._sinc_consts(device)
+        params = dict(self.named_parameters())
+        feats = []
+        with torch.no_grad():
+            for a, b in _enc.split_packs(lengths, cap):
+                total = sum(lengths[a:b])
+                plan = self._packed_plan(max(cap, total), device)
+                x = plan.wave[:total]
+                if all(not w.is_cuda for w in flat[a:b]):
+                    x.copy_(torch.cat(flat[a:b]))
+                else:
+                    torch.cat([w.to(device) for w in flat[a:b]], out=x)
+                feats += _enc.encoder_forward_packed(plan, self, x, lengths[a:b], geoms[a:b],
+                                                     params, mode)
+        return feats
 
     def forward(self, batch, device=None, mode=None):
         if device is None:

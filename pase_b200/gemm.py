@@ -130,6 +130,18 @@ def nt(p, A, lda, a_n, B, ldb, C, ldc, M, N, K, alpha=1.0, bias=None, rows_in=No
                     p.mode, 1 if C.dtype == torch.bfloat16 else 0)
 
 
+def nt_var(p, A, lda, a_n, B, ldb, C, ldc, M, N, K, bias, tab, n, fold, a_op=None, b_op=None):
+    """nt over a packed variable-length batch (inference): the row map is the device table `tab`
+    of n utterances (pase_gemm_nt_var); operands as for nt."""
+    if not nt_ok(p, lda, K, ldb):
+        _ffma_operands(p, "GEMM shape (lda=%d K=%d)" % (lda, K), A, B)
+        return ops.call("pase_gemm_nt_var", A, lda, B, ldb, C, ldc, M, N, K, bias, tab, n, fold)
+    a = _tc_operand(a_op, p, A, a_n, "act")
+    b = _tc_operand(b_op, p, B, None if B is None else B.numel(), "weight")
+    return ops.call("pase_tc_gemm_nt_var", a.hi, a.lo, a_n // lda, lda, b.hi, b.lo, ldb, C, ldc,
+                    M, N, K, bias, tab, n, fold, p.mode, 1 if C.dtype == torch.bfloat16 else 0)
+
+
 def tn(p, A, lda, a_n, B, ldb, b_n, C, ldc, I, J, rows, groups=1, pitchA=None, offA=0,
        pitchB=None, alpha=1.0, acc=0, a_kind="grad", a_op=None, b_op=None):
     """C[i, j] (+)= alpha sum_r A[rowA(r)*lda + i] B[rowB(r)*ldb + j] over `groups` x `rows` rows
