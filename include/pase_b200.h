@@ -108,6 +108,12 @@ int pase_tc_gemm_nt_var(const void* Ahi, const void* Alo, long a_rows, int R,
                         const void* Bhi, const void* Blo, long ldb, void* C, long ldc,
                         int M, int N, int K, const float* bias, const int* var_tab, int nvar,
                         int fold, int mode, int c_bf16, void* stream);
+/* How pase_tc_gemm_nt / pase_tc_gemm_nt_var cover an M x N output on `sms` SMs (host only):
+ * out4 = {bn, bulk_m, tail_bn, tail_pieces}.  One launch of 128 x bn tiles takes rows
+ * [0, bulk_m); when the tiles leave a partial last round, a second launch takes rows
+ * [bulk_m, M) at every column in tail_pieces tiles of 128 x tail_bn (tail_bn 0: no second
+ * launch, bulk_m = M).  K is never split, so the results do not depend on the plan. */
+int pase_tc_gemm_nt_plan(int M, int N, int sms, int* out4);
 int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int offA,
                     const void* Bhi, const void* Blo, int R, int pitchB, long b_rows_total,
                     float* C, long ldc, int I, int J, int groups, int rows_per_group,

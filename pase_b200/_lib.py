@@ -126,6 +126,16 @@ def device_info():
     return {"sms": out[0], "cc": (out[1], out[2]), "smem_optin": out[3]}
 
 
+def tc_gemm_nt_plan(M, N, sms):
+    """How pase_tc_gemm_nt covers an M x N output on `sms` SMs: dict(bn, bulk_m, tail_bn,
+    tail_pieces); tail_bn 0 = one launch."""
+    out = (ctypes.c_int * 4)()
+    rc = lib().pase_tc_gemm_nt_plan(M, N, sms, ctypes.cast(out, ctypes.c_void_p))
+    if rc != 0:
+        raise RuntimeError("pase_tc_gemm_nt_plan failed: " + last_error())
+    return {"bn": out[0], "bulk_m": out[1], "tail_bn": out[2], "tail_pieces": out[3]}
+
+
 def tc_gemm_tn_plan(I, J, groups, rows_per_group, mode):
     """(splits, chunks_per_split) of pase_tc_gemm_tn for this shape on the current device."""
     out = (ctypes.c_int * 2)()

@@ -180,6 +180,25 @@ struct KindTag {};
 #define PASE_AB32 "%32, %33, p, 1, 1"
 #define PASE_SC32 "%34"
 #define PASE_TR32 ", %35, %36"
+#define PASE_D4 "{%0, %1, %2, %3}"
+#define PASE_O4 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+#define PASE_AB4 "%4, %5, p, 1, 1"
+#define PASE_SC4 "%6"
+#define PASE_TR4 ", %7, %8"
+#define PASE_D8 "{%0, %1, %2, %3, %4, %5, %6, %7}"
+#define PASE_O8 \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+#define PASE_AB8 "%8, %9, p, 1, 1"
+#define PASE_SC8 "%10"
+#define PASE_TR8 ", %11, %12"
+#define PASE_D16 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
+#define PASE_O16 \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), \
+  "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), \
+  "+f"(d[14]), "+f"(d[15])
+#define PASE_AB16 "%16, %17, p, 1, 1"
+#define PASE_SC16 "%18"
+#define PASE_TR16 ", %19, %20"
 #define PASE_D64 \
   "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, " \
   "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, " \
@@ -210,6 +229,16 @@ struct KindTag {};
                  : PASE_O##NR                                                                \
                  : "l"(da), "l"(db), "r"(scale_d) __VA_ARGS__);                              \
   }
+// n8 / n16 / n32: the narrow tiles of the NT GEMM's last round (nt_plan)
+PASE_WGMMA(4, 0, "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32", "", )
+PASE_WGMMA(4, 1, "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16", PASE_TR4, , "n"(TA), "n"(TB))
+PASE_WGMMA(4, 2, "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16", PASE_TR4, , "n"(TA), "n"(TB))
+PASE_WGMMA(8, 0, "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32", "", )
+PASE_WGMMA(8, 1, "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16", PASE_TR8, , "n"(TA), "n"(TB))
+PASE_WGMMA(8, 2, "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16", PASE_TR8, , "n"(TA), "n"(TB))
+PASE_WGMMA(16, 0, "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32", "", )
+PASE_WGMMA(16, 1, "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16", PASE_TR16, , "n"(TA), "n"(TB))
+PASE_WGMMA(16, 2, "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16", PASE_TR16, , "n"(TA), "n"(TB))
 PASE_WGMMA(32, 0, "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32", "", )
 PASE_WGMMA(32, 1, "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16", PASE_TR32, , "n"(TA), "n"(TB))
 PASE_WGMMA(32, 2, "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16", PASE_TR32, , "n"(TA), "n"(TB))
@@ -304,6 +333,7 @@ struct NTArgs {
   void* C;
   long ldc;
   int M, N, K;
+  int m_base;                      // first row of the first tile (a multiple of BM); rows < M valid
   float alpha;
   const float* alpha_dev;          // optional device scalar multiplied into alpha
   const float* bias;
@@ -514,7 +544,8 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int M = a.M, N = a.N, K = a.K, R = a.R;
-  const int n_tiles = (N + BN - 1) / BN, m_tiles = (M + BM - 1) / BM;
+  const int m_base = a.m_base;
+  const int n_tiles = (N + BN - 1) / BN, m_tiles = (M - m_base + BM - 1) / BM;
   const int total_tiles = n_tiles * m_tiles;
   const int nkb = (K + BK - 1) / BK;
   int flush_kb = a.flush_kb;
@@ -546,7 +577,7 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
       int s = 0;
       uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
+        const int m0 = m_base + (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
         int arow = m0, acol = 0;                 // folded-row view: k = (arow - m0) * R + acol
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait(&empty_bar[s], ph ^ 1, 1);
@@ -590,7 +621,7 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
   int s = 0;
   uint32_t ph = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int m0 = (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
+    const int m0 = m_base + (tile / n_tiles) * BM, n0 = (tile % n_tiles) * BN;
     for (int ch = 0; ch < nchunks; ++ch) {
       const int kb_lo = ch * flush_kb;
       const int kb_hi = (kb_lo + flush_kb < nkb) ? kb_lo + flush_kb : nkb;
@@ -976,11 +1007,77 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
     }
     attr = true;
   }
-  const long tiles = (long)((a.N + BN - 1) / BN) * ((a.M + BM - 1) / BM);
+  const long tiles = (long)((a.N + BN - 1) / BN) * ((a.M - a.m_base + BM - 1) / BM);
   const int grid = (int)(tiles < pase_num_sms() ? tiles : pase_num_sms());
   PASE_LAUNCH((tc_gemm_nt_kernel<BN, MODE, OUT16, CTX, VAR>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
   PASE_TC_LAUNCH_CHECK(CTX ? "pase_tc_gemm_nt_ctxmse" : "pase_tc_gemm_nt");
   return PASE_OK;
+}
+
+// How pase_tc_gemm_nt covers its 128 x bn tiles with one persistent CTA per SM.  When the tiles
+// fill R >= 1 whole rounds and part of one more, that last round would run a few full-K tiles on
+// a few SMs while the others idle.  Then a first (bulk) launch takes the first
+// floor(R sms / n_tiles) tile rows, at most R rounds, and a second (tail) launch takes the rows
+// left, at every column, in 128 x tail_bn pieces: the narrowest width in 8..64 whose pieces fit
+// one round (a piece loads the same A bytes at any width, so the narrowest finishes soonest).
+// K is never split: every output element keeps its k order and fold boundaries, and the tile
+// width only decides which CTA computes it, so a row's result does not depend on where it sits.
+struct NTPlan {
+  int bn;             // tile width of the bulk launch
+  int bulk_m;         // rows [0, bulk_m) are the bulk launch's (M: one launch, no tail)
+  int tail_bn;        // tile width of the tail launch over rows [bulk_m, M); 0: no tail
+  long tail_pieces;
+};
+NTPlan nt_plan(int M, int N, int sms) {
+  NTPlan p;
+  p.bn = N <= 64 ? 64 : 128;
+  p.bulk_m = M;
+  p.tail_bn = 0;
+  p.tail_pieces = 0;
+  const long n_tiles = (N + p.bn - 1) / p.bn, m_tiles = (M + BM - 1) / BM;
+  const long rounds = n_tiles * m_tiles / sms;
+  if (rounds < 1 || (n_tiles * m_tiles) % sms == 0) return p;
+  const long mb = rounds * sms / n_tiles;
+  if (mb < 1) return p;
+  for (int bt = 8; bt < p.bn; bt *= 2) {
+    const long pieces = (m_tiles - mb) * ((N + bt - 1) / bt);
+    if (pieces <= sms) {
+      p.bulk_m = (int)(mb * BM);
+      p.tail_bn = bt;
+      p.tail_pieces = pieces;
+      break;
+    }
+  }
+  return p;
+}
+
+template <int BN, bool VAR>
+int launch_nt_mode(int mode, int c_bf16, const CUtensorMap& ah, const CUtensorMap& al,
+                   const CUtensorMap& bh, const CUtensorMap& bl, const NTArgs& a,
+                   cudaStream_t st) {
+  switch (mode * 2 + (c_bf16 ? 1 : 0)) {
+    case 0: return launch_nt<BN, 0, false, false, VAR>(ah, al, bh, bl, a, st);
+    case 1: return launch_nt<BN, 0, true, false, VAR>(ah, al, bh, bl, a, st);
+    case 2: return launch_nt<BN, 1, false, false, VAR>(ah, al, bh, bl, a, st);
+    case 3: return launch_nt<BN, 1, true, false, VAR>(ah, al, bh, bl, a, st);
+    case 4: return launch_nt<BN, 2, false, false, VAR>(ah, al, bh, bl, a, st);
+    case 5: return launch_nt<BN, 2, true, false, VAR>(ah, al, bh, bl, a, st);
+    case 6: return launch_nt<BN, 3, false, false, VAR>(ah, al, bh, bl, a, st);
+    default: return launch_nt<BN, 3, true, false, VAR>(ah, al, bh, bl, a, st);
+  }
+}
+
+template <bool VAR>
+int launch_nt_width(int bn, int mode, int c_bf16, const CUtensorMap& ah, const CUtensorMap& al,
+                    const CUtensorMap& bh, const CUtensorMap& bl, const NTArgs& a,
+                    cudaStream_t st) {
+  switch (bn) {
+    case 8: return launch_nt_mode<8, VAR>(mode, c_bf16, ah, al, bh, bl, a, st);
+    case 16: return launch_nt_mode<16, VAR>(mode, c_bf16, ah, al, bh, bl, a, st);
+    case 32: return launch_nt_mode<32, VAR>(mode, c_bf16, ah, al, bh, bl, a, st);
+    case 64: return launch_nt_mode<64, VAR>(mode, c_bf16, ah, al, bh, bl, a, st);
+    default: return launch_nt_mode<128, VAR>(mode, c_bf16, ah, al, bh, bl, a, st);
+  }
 }
 
 // How pase_tc_gemm_tn splits its reduction: the split count and the chunks (stages of KR
@@ -1140,7 +1237,7 @@ int tc_gemm_nt_impl(const void* Ahi, const void* Alo, long a_rows, int R, const 
   PASE_CHECK_ARG(colsum == nullptr || N <= 4096, "pase_tc_gemm_nt: stats need N <= 4096");
   PASE_CHECK_ARG(colsum == nullptr || !accumulate, "pase_tc_gemm_nt: stats + accumulate");
   PASE_CHECK_ARG(!c_bf16 || !accumulate, "pase_tc_gemm_nt: bf16 output cannot accumulate");
-  const int BN = N <= 64 ? 64 : 128;
+  const NTPlan plan = nt_plan(M, N, pase_num_sms());
   const int bk = eb;
   // split modes: fold the accumulators into fp32 register sums every K = 128; over K <= 512
   // the tensor core's own accumulation stays below 1e-6 relative, so short reductions (sinc
@@ -1152,7 +1249,7 @@ int tc_gemm_nt_impl(const void* Ahi, const void* Alo, long a_rows, int R, const 
   uint32_t abox[2] = {(uint32_t)bk, (uint32_t)BM};
   uint64_t bdims[2] = {(uint64_t)K, (uint64_t)N};
   uint64_t bstr[1] = {(uint64_t)ldb * esz};
-  uint32_t bbox[2] = {(uint32_t)bk, (uint32_t)BN};
+  uint32_t bbox[2] = {(uint32_t)bk, (uint32_t)plan.bn};
   int rc;
   if ((rc = make_map(&ah, Ahi, mode, 2, adims, astr, abox, "A.hi")) != 0) return rc;
   if ((rc = make_map(&bh, Bhi, mode, 2, bdims, bstr, bbox, "B.hi")) != 0) return rc;
@@ -1164,7 +1261,7 @@ int tc_gemm_nt_impl(const void* Ahi, const void* Alo, long a_rows, int R, const 
     bl = bh;
   }
   NTArgs a;
-  a.R = R; a.C = C; a.ldc = ldc; a.M = M; a.N = N; a.K = K; a.alpha = alpha;
+  a.R = R; a.C = C; a.ldc = ldc; a.M = plan.bulk_m; a.N = N; a.K = K; a.m_base = 0; a.alpha = alpha;
   a.alpha_dev = alpha_dev; a.bias = bias;
   a.rm = RowMap{rows_in, t_valid, rows_out, fold, N / fold, var_tab, var_n};
   a.colsum = colsum; a.colsumsq = colsumsq; a.accumulate = accumulate; a.flush_kb = flush_kb;
@@ -1172,24 +1269,23 @@ int tc_gemm_nt_impl(const void* Ahi, const void* Alo, long a_rows, int R, const 
   a.cx_label = nullptr; a.cx_F = a.cx_T = a.cx_r = a.cx_nvalid = 0; a.cx_scale = nullptr;
   a.cx_lo = nullptr; a.cx_loss = nullptr; a.cx_db = nullptr;
   cudaStream_t st = (cudaStream_t)stream;
-#define PASE_NT(BNV, VARV)                                                                 \
-  switch (mode * 2 + (c_bf16 ? 1 : 0)) {                                                   \
-    case 0: return launch_nt<BNV, 0, false, false, VARV>(ah, al, bh, bl, a, st);           \
-    case 1: return launch_nt<BNV, 0, true, false, VARV>(ah, al, bh, bl, a, st);            \
-    case 2: return launch_nt<BNV, 1, false, false, VARV>(ah, al, bh, bl, a, st);           \
-    case 3: return launch_nt<BNV, 1, true, false, VARV>(ah, al, bh, bl, a, st);            \
-    case 4: return launch_nt<BNV, 2, false, false, VARV>(ah, al, bh, bl, a, st);           \
-    case 5: return launch_nt<BNV, 2, true, false, VARV>(ah, al, bh, bl, a, st);            \
-    case 6: return launch_nt<BNV, 3, false, false, VARV>(ah, al, bh, bl, a, st);           \
-    default: return launch_nt<BNV, 3, true, false, VARV>(ah, al, bh, bl, a, st);           \
+  auto run = [&](int bn, const CUtensorMap& b_hi, const CUtensorMap& b_lo) {
+    return var_tab != nullptr ? launch_nt_width<true>(bn, mode, c_bf16, ah, al, b_hi, b_lo, a, st)
+                              : launch_nt_width<false>(bn, mode, c_bf16, ah, al, b_hi, b_lo, a, st);
+  };
+  if ((rc = run(plan.bn, bh, bl)) != 0 || plan.tail_bn == 0) return rc;
+  // tail: rows [bulk_m, M) at every column, B in boxes of tail_bn rows
+  CUtensorMap th, tl;
+  bbox[1] = (uint32_t)plan.tail_bn;
+  if ((rc = make_map(&th, Bhi, mode, 2, bdims, bstr, bbox, "tail B.hi")) != 0) return rc;
+  if (split) {
+    if ((rc = make_map(&tl, Blo, mode, 2, bdims, bstr, bbox, "tail B.lo")) != 0) return rc;
+  } else {
+    tl = th;
   }
-  if (var_tab != nullptr) {
-    if (BN == 64) { PASE_NT(64, true) }
-    PASE_NT(128, true)
-  }
-  if (BN == 64) { PASE_NT(64, false) }
-  PASE_NT(128, false)
-#undef PASE_NT
+  a.m_base = plan.bulk_m;
+  a.M = M;
+  return run(plan.tail_bn, th, tl);
 }
 
 }  // namespace
@@ -1247,7 +1343,7 @@ int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
   if ((rc = make_map(&bh, Bhi, mode, 2, bdims, bstr, bbox, "ctx B.hi")) != 0) return rc;
   if ((rc = make_map(&bl, Blo, mode, 2, bdims, bstr, bbox, "ctx B.lo")) != 0) return rc;
   NTArgs a;
-  a.R = R; a.C = Rhi; a.ldc = ldr; a.M = M; a.N = (int)ldr; a.K = K; a.alpha = 1.f;
+  a.R = R; a.C = Rhi; a.ldc = ldr; a.M = M; a.N = (int)ldr; a.K = K; a.m_base = 0; a.alpha = 1.f;
   a.alpha_dev = nullptr; a.bias = bias;
   a.rm = RowMap{M, M, M, 1, (int)ldr, nullptr, 0};
   a.colsum = nullptr; a.colsumsq = nullptr; a.accumulate = 0;
@@ -1327,6 +1423,16 @@ int pase_tc_gemm_tn(const void* Ahi, const void* Alo, long lda, int pitchA, int 
   if (BN == 64) { PASE_TN(64) }
   PASE_TN(128)
 #undef PASE_TN
+}
+
+int pase_tc_gemm_nt_plan(int M, int N, int sms, int* out4) {
+  PASE_CHECK_ARG(out4 && M > 0 && N > 0 && sms > 0, "pase_tc_gemm_nt_plan: bad args");
+  const NTPlan p = nt_plan(M, N, sms);
+  out4[0] = p.bn;
+  out4[1] = p.bulk_m;
+  out4[2] = p.tail_bn;
+  out4[3] = (int)p.tail_pieces;
+  return PASE_OK;
 }
 
 int pase_tc_gemm_tn_plan(int I, int J, int groups, int rows_per_group, int mode, int* out2) {
