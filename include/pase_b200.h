@@ -472,6 +472,25 @@ int pase_clip(float* x, long ldx, const long* jobs, const double* cf, int njobs,
 int pase_overlap_label(const long* jobs, int njobs, int T, int d, float* label, long ldl,
                        void* stream);
 
+/* ---- on-device batch assembly (pase/dataset.py:452-513 LibriSpeechSegTupleWavDataset,
+ * pase/transforms.py:295-436 SingleChunkWav / MIChunkWav, 253-292 CachedCompose; the host
+ * planner is pase_b200/batch.py).  Row tables are int64 DEVICE rows drawn and bounds-checked
+ * by the planner; a row that does not fit its pool is skipped (its output is not written).
+ * Pools may be device memory or page-locked host memory read through its mapped address. */
+/* Chunk windows: rows (B, nsrc, 6) {fmt, off, L, beg, scale, rbits}; CTA (s, b) reads
+ * x[j] = u[beg + j], j < T, of utterance u = pool[off, off + L) (fmt 0: pcm int16 k / 32768,
+ * fmt 1: flt fp32), reflected past its end (u[L + i] = u[L - 2 - i]).  scale != 0:
+ * x <- __fmul_rn(__fdiv_rn(x, max|x|), r), r = the fp32 with bits rbits (a silent window gives
+ * 0/0 = NaN, as the reference's norm_and_scale).  Writes out[s * plane + b * T + j] and, for
+ * s == 0 when cchunk != 0, the copy at out[nsrc * plane + b * T + j]. */
+int pase_chunk_gather(const void* pcm, long pcm_len, const float* flt, long flt_len,
+                      const long* rows, int B, int nsrc, int T, int cchunk, float* out,
+                      long plane, void* stream);
+/* Cached-feature slices: rows (B, 3) {off, frames, s}; out (B, F, n) with
+ * out[b, f, t] = pool[off + f * frames + s + t], s + n <= frames. */
+int pase_frames_gather(const float* pool, long pool_len, const long* rows, int B, int F, int n,
+                       float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
