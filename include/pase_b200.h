@@ -379,6 +379,17 @@ int pase_time_mean_fwd(const float* x, long ldx, float* out, long ldo, int B, in
                        void* stream);
 int pase_time_mean_bwd(const float* dout, long ldo, float* dx, long ldx, int B, int T, int C,
                        int accumulate, void* stream);
+/* SPC frame gather (SPCMinion, minions.py:575-649).  frames: DEVICE int64 {t, future_t, past_t},
+ * checked by the host (M + 1 <= t < T - M, t + seq_pad <= future_t < T - N,
+ * N <= past_t < t - seq_pad, M = seq_pad + N); the kernels trust them.  x (B*T, C) rows with row
+ * stride ldx -> out (2B, (N+1)*C) contiguous: row b = [x(b,t) | fut], row B + b = [x(b,t) | past],
+ * fut[c*N + n] = x(b, future_t + n, c), past[c*N + n] = x(b, past_t - N + n, c). */
+int pase_spc_gather(const float* x, long ldx, const long* frames, int B, int T, int C, int N,
+                    int seq_pad, float* out, void* stream);
+/* g (2B, (N+1)*C) -> dense dx (B*T, C): the windows of g copied, g[b, :C] + g[B+b, :C] at frame t,
+ * zeros elsewhere (every element written, no atomics). */
+int pase_spc_gather_bwd(const float* g, const long* frames, int B, int T, int C, int N,
+                        int seq_pad, float* dx, void* stream);
 /* misc fused vector helpers */
 int pase_axpy(const float* x, float* y, long n, float a, void* stream);
 int pase_scale_dev(float* x, long n, const float* dev_scalar, float host_coef, void* stream);

@@ -216,6 +216,58 @@ def time_mean_rows(x, B, T):
     return _TimeMean.apply(x, B, T)
 
 
+def check_spc_frames(T, N, seq_pad, t, future_t, past_t):
+    """The ranges SPCMinion draws from (minions.py:609-627): refuse indices outside them before
+    they reach the device, where the gather kernels trust them."""
+    M = seq_pad + N
+    if not (M + 1 <= t < T - M and t + seq_pad <= future_t < T - N and
+            N <= past_t < t - seq_pad):
+        raise ValueError("SPC frames (t=%r, future_t=%r, past_t=%r) outside the ranges of T'=%d "
+                         "frames, N=%d, seq_pad=%d: need %d <= t < %d, t + %d <= future_t < %d, "
+                         "%d <= past_t < t - %d" % (t, future_t, past_t, T, N, seq_pad, M + 1,
+                                                    T - M, seq_pad, T - N, N, seq_pad))
+
+
+class _SPCGather(torch.autograd.Function):
+    """(B*T, C) rows -> (2B, (N+1)*C) rows [cur | fut ; cur | past] of the SPC worker, the three
+    frame indices read from the device int64 tensor `frames` {t, future_t, past_t}."""
+
+    @staticmethod
+    def forward(ctx, x, frames, B, T, N, seq_pad):
+        x = x.detach()
+        C = x.shape[1]
+        if x.stride(1) != 1:
+            x = x.contiguous()
+        ldx = x.stride(0) if x.shape[0] > 1 else C
+        out = torch.empty(2 * B, (N + 1) * C, dtype=torch.float32, device=x.device)
+        ops.call("pase_spc_gather", x, ldx, frames, B, T, C, N, seq_pad, out)
+        ctx.save_for_backward(frames)
+        ctx.dims = (B, T, C, N, seq_pad)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (frames,) = ctx.saved_tensors
+        B, T, C, N, seq_pad = ctx.dims
+        g = g.contiguous()
+        dx = torch.empty(B * T, C, dtype=torch.float32, device=g.device)
+        ops.call("pase_spc_gather_bwd", g, frames, B, T, C, N, seq_pad, dx)
+        return dx, None, None, None, None, None
+
+
+def spc_gather(rows, B, T, N, seq_pad, frames):
+    """SPC input rows of the (B*T, C) encoder rows.  frames: a device int64 tensor of
+    {t, future_t, past_t} (trusted: a captured step's table, filled by a planner that checked
+    it), or a host triple, checked here and uploaded."""
+    if not isinstance(frames, torch.Tensor):
+        check_spc_frames(T, N, seq_pad, *frames)
+        src = torch.tensor([int(f) for f in frames], dtype=torch.int64)
+        if rows.is_cuda:
+            src = src.pin_memory()
+        frames = src.to(rows.device, non_blocking=True)
+    return _SPCGather.apply(rows, frames, B, T, N, seq_pad)
+
+
 class _NctToRows(torch.autograd.Function):
     """(B,C,T) -> (B*T, C) channel-last rows (boundary conversion for tensors that did not
     come from the encoder's channel-last output)."""

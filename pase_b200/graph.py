@@ -3,8 +3,24 @@ forward + backward through the C-ABI kernels, optimizer update, D2H of the loss)
 step is ONE launch: the hot loop is launch-bound on the host once the kernels take only a
 few ms.  Buffers of the encoder plan are static by construction (EncoderPlan), TMA
 descriptors are kernel parameters, so the captured graph is replayable as is.
+
+GraphedEncoderStep captures the encoder with a given loss; GraphedTrainStep captures the PASE /
+PASE+ training step with its workers, fed by a DeviceBatcher plan uploaded before each replay.
 """
+import random
+
+import numpy as np
 import torch
+
+
+def _refresh_hyperparams(opt, stream):
+    """FlatAdam keeps its hyper-parameter table at one address; write the current lr / betas /
+    eps / weight decay into it on the replay stream, so that a scheduler's change between two
+    replays reaches the captured update."""
+    segments = getattr(opt, "_segments", None)
+    if segments is not None:
+        with torch.cuda.stream(stream):
+            segments()
 
 
 class GraphedEncoderStep(object):
@@ -118,6 +134,7 @@ class GraphedEncoderStep(object):
                 self.stage[1 - k].copy_(self.x_host, non_blocking=True)
                 self.h2d_done[1 - k].record(self.copy_stream)
             self._k = 1 - k
+        _refresh_hyperparams(self.opt, self.stream)
         self.graph.replay()
         if self.graph_b is not None:
             with torch.cuda.stream(self.stream):
@@ -127,6 +144,175 @@ class GraphedEncoderStep(object):
             return None
         self.stream.synchronize()
         return float(self.loss_host)
+
+
+def spc_minions(model):
+    """The SPCMinion heads of a ``pase`` model in the order its forward calls them (regression
+    workers, then classification workers), i.e. the order of their draws."""
+    from .minions import SPCMinion
+    workers = list(model.regression_workers) + list(model.classification_workers)
+    return [m for w in workers for m in w.modules() if isinstance(m, SPCMinion)]
+
+
+class TrainPlanner(object):
+    """Host side of one PASE/PASE+ training step: the batch plan of ``DeviceBatcher.plan`` and
+    the frames of every SPC head, drawn in the order the eager loop draws them (the batch, then
+    the step's SPC frames; the next batch's draws come after).  ``rng``: None (the global
+    random, np.random and torch generators) or a (random.Random, np.random.RandomState,
+    torch.Generator) triple, as for ``plan()``; the SPC frames come from its first member."""
+
+    def __init__(self, model, batcher):
+        self.batcher = batcher
+        self.spc = spc_minions(model)
+        self.Tq = model.frontend.frame_counts(batcher.T)[-1]
+        for m in self.spc:
+            if not m.frames_ok(self.Tq):
+                M = m.seq_pad + m.ctxt_frames
+                raise ValueError("TrainPlanner: chunk_size %d gives T'=%d frames, which leave the "
+                                 "SPC head %s no current frame (range(%d, %d) is empty); use a "
+                                 "longer chunk" % (batcher.T, self.Tq, m.name, M + 1, self.Tq - M))
+
+    def __call__(self, indices, rng=None):
+        """-> (BatchPlan, int64 numpy table: the plan's table then t, future_t, past_t of each
+        SPC head)."""
+        plan = self.batcher.plan(indices, rng)
+        py = random if rng is None else rng[0]
+        frames = [f for m in self.spc for f in m.draw_frames(self.Tq, py)]
+        return plan, np.concatenate([plan.table, np.asarray(frames, dtype=np.int64)])
+
+
+class GraphedTrainStep(object):
+    """One PASE/PASE+ training step from a resident corpus as one CUDA-graph replay: batch
+    assembly (``DeviceBatcher``), the encoder, every worker head and its loss, the summed
+    ('base' scheduler) loss, backward and the single ``FlatAdam`` update.
+
+        step = GraphedTrainStep(model, engine, batcher, B)
+        for indices in BatchSampler(RandomSampler(range(len(wavs))), B, drop_last=True):
+            step(indices)                 # plan on the host, upload, replay; does not wait
+            if bidx % log_freq == 0:
+                losses = step.losses()    # {'total': float, name: float, ...}
+
+    ``model``: a ``pase_b200.pase.pase`` on CUDA in train mode; ``engine``: a ``FlatAdam`` over
+    its parameters with ``bind_encoder(model.frontend)`` applied (not ``peer_dp``);
+    ``batcher``: a ``DeviceBatcher``.  Each call is exactly one step on its own batch: the first
+    `warmup` calls run eagerly through the code that is captured, the next one captures and
+    replays, every later one replays.  The host draws and stages the next step's plan while the
+    device runs the current one; lr changes (``param_groups``, ``views()``) between two calls
+    take effect at the next step.  The step runs on its own stream; each call orders the caller's
+    current stream after it (and the step after the caller's earlier work), so eager work the
+    caller queues between calls, such as a validation pass or a checkpoint, sees the finished
+    step without a host synchronise."""
+
+    def __init__(self, model, engine, batcher, batch_size, warmup=3, stream=None):
+        from .optim import FlatAdam
+        if int(warmup) < 1:
+            raise ValueError("GraphedTrainStep: warmup=%d; at least one eager step builds the "
+                             "constants and buffers the capture reads" % warmup)
+        if not model.training:
+            raise ValueError("GraphedTrainStep: the model is in eval mode; call model.train()")
+        if not isinstance(engine, FlatAdam):
+            raise TypeError("GraphedTrainStep: the engine must be a FlatAdam, got %s"
+                            % type(engine).__name__)
+        if engine.peer_dp:
+            raise NotImplementedError("GraphedTrainStep: FlatAdam(peer_dp=True) is not supported; "
+                                      "data-parallel steps are not captured here")
+        sunk = {id(p) for _, p in model.frontend.named_parameters() if p.requires_grad}
+        if getattr(model.frontend, "grad_sink", None) is None or engine._sunk != sunk:
+            raise ValueError("GraphedTrainStep: call engine.bind_encoder(model.frontend) first")
+        if int(batch_size) < 1:
+            raise ValueError("GraphedTrainStep: batch_size=%d" % batch_size)
+        self.planner = TrainPlanner(model, batcher)
+        params = list(model.parameters())
+        if not params or not all(p.is_cuda for p in params):
+            raise ValueError("GraphedTrainStep: the model must live on a CUDA device")
+        self.model, self.engine, self.batcher = model, engine, batcher
+        self.B, self.warmup = int(batch_size), int(warmup)
+        self.device = params[0].device
+        # total_loss's order: classification workers, then regression workers
+        self.names = ["total"] + [w.name for w in list(model.classification_workers) +
+                                  list(model.regression_workers)]
+        self.stream = stream if stream is not None else torch.cuda.Stream(device=self.device)
+        self.loss_host = torch.zeros(len(self.names), dtype=torch.float32).pin_memory()
+        self.done = torch.cuda.Event()
+        self.table = None                 # the graph's static plan table, sized by the first plan
+        self.graph = None
+        self._plans = []
+        self.calls = 0
+        self._k = 0
+
+    def _alloc(self, n):
+        self.table = torch.zeros(n, dtype=torch.int64, device=self.device)
+        # two page-locked staging tables: the host fills one while the other's copy is queued
+        self._stage = [torch.zeros(n, dtype=torch.int64).pin_memory() for _ in (0, 1)]
+        self._staged = [torch.cuda.Event(), torch.cuda.Event()]
+
+    def _run(self):
+        """The step as it is captured: everything reads the static table."""
+        from .pase import total_loss
+        eng, model = self.engine, self.model
+        nb = self.table.numel() - 3 * len(self.planner.spc)
+        eng.zero_grad(set_to_none=True)
+        batch = self.batcher.run(self.table[:nb])
+        for i, m in enumerate(self.planner.spc):
+            m.frame_table = self.table[nb + 3 * i:nb + 3 * i + 3]
+        try:
+            _, _, preds, labels = model(batch)
+        finally:
+            for m in self.planner.spc:
+                m.frame_table = None
+        tot, losses = total_loss(model, preds, labels)
+        vec = torch.stack([tot.detach()] + [losses[n].detach() for n in self.names[1:]])
+        tot.backward()
+        eng.step()
+        self.loss_host.copy_(vec, non_blocking=True)
+
+    def __call__(self, indices, rng=None):
+        indices = [int(i) for i in indices]
+        if len(indices) != self.B:
+            raise ValueError("GraphedTrainStep: a batch of %d indices, the step was built for %d"
+                             % (len(indices), self.B))
+        _, table = self.planner(indices, rng)
+        if self.table is None:
+            self._alloc(table.size)
+        elif table.size != self.table.numel():
+            raise RuntimeError("GraphedTrainStep: the plan has %d entries, the captured step %d"
+                               % (table.size, self.table.numel()))
+        k = self._k
+        self._staged[k].synchronize()          # the copy that last read this buffer has run
+        self._stage[k].numpy()[:] = table
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            self.table.copy_(self._stage[k], non_blocking=True)
+            self._staged[k].record(self.stream)
+            self.engine._segments()              # lr changes, into the table at its address
+            if self.calls < self.warmup:
+                self._run()
+            else:
+                if self.graph is None:
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g, stream=self.stream):
+                        self._run()
+                    self.graph = g
+                    # the graph holds raw addresses of the encoder's and decoders' plan buffers;
+                    # keep those plans alive when their caches evict them (other shapes run
+                    # eagerly between replays, e.g. validation batches)
+                    self._plans = [p for m in self.model.modules()
+                                   for p in getattr(m, "_plans", {}).values()]
+                self.graph.replay()
+            self.done.record(self.stream)
+        # work the caller queues next (an eager validation pass, reading or saving parameters)
+        # runs after this step on the device; the host does not wait
+        torch.cuda.current_stream(self.device).wait_stream(self.stream)
+        self._k = 1 - k
+        self.calls += 1
+
+    def losses(self):
+        """{'total': ..., worker name: ...} (python floats, each worker's loss times its
+        loss_weight) of the last step issued; waits for that step only."""
+        if self.calls == 0:
+            raise RuntimeError("GraphedTrainStep.losses: no step has run yet")
+        self.done.synchronize()
+        return dict(zip(self.names, self.loss_host.tolist()))
 
 
 class PipelinedDPStep(object):
@@ -278,6 +464,7 @@ class PipelinedDPStep(object):
     def step(self, x_host=None):
         if x_host is not None:
             self.x_host.copy_(x_host)
+        _refresh_hyperparams(self.opt, self.stream)
         with torch.cuda.stream(self.stream):
             self.gA1.replay()
             self._reduce_upper_async()

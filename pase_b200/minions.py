@@ -126,8 +126,11 @@ class MLPMinion(Model):
 
 
 class SPCMinion(MLPMinion):
-    """Future-vs-past frame discrimination (minions.py:575-649).  The frame gather uses
-    Python's ``random`` exactly like the reference (host RNG, three draws per call)."""
+    """Future-vs-past frame discrimination (minions.py:575-649).  The three frames are drawn
+    from Python's ``random`` exactly like the reference (host RNG, three draws per call), unless
+    ``frame_table`` holds a device int64 tensor {t, future_t, past_t}: a captured training step
+    (``pase_b200.graph.GraphedTrainStep``) sets it to its own table, which its planner fills with
+    ``draw_frames`` before every replay."""
 
     def __init__(self, num_inputs, num_outputs, dropout, hidden_size=256, hidden_layers=2,
                  ctxt_frames=5, seq_pad=16, skip=True, loss=None, loss_weight=1., keys=None,
@@ -136,20 +139,33 @@ class SPCMinion(MLPMinion):
                          dropout=dropout, hidden_size=hidden_size, hidden_layers=hidden_layers,
                          skip=skip, loss=loss, loss_weight=loss_weight, keys=keys, name=name)
         self.ctxt_frames, self.seq_pad = ctxt_frames, seq_pad
+        self.frame_table = None
+
+    def frames_ok(self, T):
+        """Whether T frames leave the current frame's range [M + 1, T - M) non-empty (then the
+        future and past ranges are non-empty too)."""
+        M = self.seq_pad + self.ctxt_frames
+        return T - M > M + 1
+
+    def draw_frames(self, T, py=random):
+        """(t, future_t, past_t) for T frames: the reference's three draws from `py`."""
+        N, sp = self.ctxt_frames, self.seq_pad
+        M = sp + N
+        if not self.frames_ok(T):
+            raise ValueError("SPCMinion %s: T'=%d frames leave range(%d, %d) for the current "
+                             "frame empty (ctxt_frames=%d, seq_pad=%d)" % (self.name, T, M + 1,
+                                                                           T - M, N, sp))
+        t = py.choice(list(range(M + 1, T - M)))
+        future_t = py.choice(list(range(t + sp, T - N)))
+        past_t = py.choice(list(range(N, t - sp)))
+        return t, future_t, past_t
 
     def forward(self, x, alpha=1, device=None):
         xin = RowsInput.of(x)
-        B, T, N = xin.B, xin.T, self.ctxt_frames
-        M = self.seq_pad + N
-        t = random.choice(list(range(M + 1, T - M)))
-        future_t = random.choice(list(range(t + self.seq_pad, T - N)))
-        past_t = random.choice(list(range(N, t - self.seq_pad)))
-        v = xin.rows.view(B, T, -1)                                  # (B,T,C)
+        B, T = xin.B, xin.T
+        frames = self.frame_table if self.frame_table is not None else self.draw_frames(T)
         # reference flattens (B,C,N) channel-major: index c*N + n
-        fut = v[:, future_t:future_t + N].transpose(1, 2).reshape(B, -1)
-        past = v[:, past_t - N:past_t].transpose(1, 2).reshape(B, -1)
-        cur = v[:, t]
-        rows = torch.cat([torch.cat([cur, fut], 1), torch.cat([cur, past], 1)], 0).contiguous()
+        rows = Fn.spc_gather(xin.rows, B, T, self.ctxt_frames, self.seq_pad, frames)
         y, h = self.forward_rows(rows)
         pred = rows_to_pred(y, 2 * B, 1, self.num_outputs)
         if self.skip:

@@ -53,6 +53,7 @@ class FlatAdam(torch.optim.Optimizer):
             self._ranges.append((start, off))
         self.n = off
         f32 = dict(dtype=torch.float32, device=dev)
+        self.peer_dp = bool(peer_dp)
         self._peer = None
         if peer_dp:
             import torch.distributed as dist
@@ -162,6 +163,10 @@ class FlatAdam(torch.optim.Optimizer):
 
     # ---- the update ------------------------------------------------------------------
     def _segments(self):
+        """The device table of per-group hyper-parameters.  It is allocated once and keeps its
+        address: a captured ``pase_adam_flat`` launch reads whatever the table holds at replay
+        time, so a changed lr / betas / eps / weight decay is written into the same tensor, by
+        a copy ordered on the current stream after every earlier update that read it."""
         key = tuple((g["lr"], g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"])
                     for g in self.param_groups)
         if key != self._table_key:
@@ -170,8 +175,15 @@ class FlatAdam(torch.optim.Optimizer):
                 struct.pack("<qqffffffq", a, b, float(k[0]), float(k[1]), float(k[2]), float(k[3]),
                             float(k[4]), 0.0, i)
                 for i, ((a, b), k) in enumerate(zip(self._ranges, key)))
-            t = torch.frombuffer(bytearray(raw), dtype=torch.int64).clone()
-            self._table = t.to(self.flat_param.device)
+            src = torch.frombuffer(bytearray(raw), dtype=torch.int64)
+            dev = self.flat_param.device
+            if self._table is None:
+                self._table = torch.empty(src.numel(), dtype=torch.int64, device=dev)
+            if dev.type == "cuda":
+                # page-locked: the copy is asynchronous, and the caching host allocator keeps
+                # the source alive until it has executed
+                src = src.pin_memory()
+            self._table.copy_(src, non_blocking=True)
             self._table_key = key
         return self._table
 
