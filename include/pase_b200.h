@@ -143,7 +143,9 @@ int pase_bound_scale(const float* a4, float* scale_out, void* stream);
  * (m = b*T + t; zero outside [0,T)): never stored as fp32 -- Rhi/Rlo receive the fp16
  * pair of s * residual ([M x ldr], ldr % 128 == 0, columns >= N zero), the operand of
  * the two backward GEMMs; loss_acc += sum residual^2; db_acc[n] += sum_m residual[m,n].
- * scale = device {1/s, s} (pase_bound_scale of the Cauchy-Schwarz bound). */
+ * scale = device {1/s, s} (pase_bound_scale of the Cauchy-Schwarz bound).
+ * Loss only (no gradient will be taken): Rhi, Rlo and db_acc all NULL -- only loss_acc is
+ * written, with the same sum; scale may then be NULL too. */
 int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
                            const void* Bhi, const void* Blo, long ldb,
                            void* Rhi, void* Rlo, long ldr, int M, int N, int K,

@@ -440,11 +440,13 @@ __device__ __forceinline__ void nt_output(float (&v)[NR], const NTArgs& a, float
 // Output stage of the fused regression head (losses.py:15-37 + nn.MSELoss fused into the
 // output GEMM of MLPMinion, minions.py:494-524): row m = (b, t); column n walks the
 // (feature f, context slot j) pairs; label element = label[b][f][t + j - r/2] (zero outside).
-template <int NR>
+// LOSS_ONLY (no gradient will be taken): sum d^2 only -- no residual pair, no bias-gradient
+// column sums.
+template <int NR, bool LOSS_ONLY>
 __device__ __forceinline__ void nt_output_ctx(const float (&v)[NR], const NTArgs& a, float alpha,
                                               const Frag& f, double& loss_acc) {
   const int NV = a.cx_nvalid, T = a.cx_T, F = a.cx_F, r = a.cx_r;
-  const float s = __ldg(a.cx_scale + 1);
+  const float s = LOSS_ONLY ? 0.f : __ldg(a.cx_scale + 1);
   int t[2];
   const float* lab[2];
   bool row_ok[2];
@@ -479,7 +481,7 @@ __device__ __forceinline__ void nt_output_ctx(const float (&v)[NR], const NTArgs
         cs[e] += dd;
         d2 = fmaf(dd, dd, d2);
       }
-      if (row_ok[h]) {
+      if (!LOSS_ONLY && row_ok[h]) {
         __half h0, l0, h1, l1;
         f16_split(d[0] * s, h0, l0);
         f16_split(d[1] * s, h1, l1);
@@ -488,10 +490,12 @@ __device__ __forceinline__ void nt_output_ctx(const float (&v)[NR], const NTArgs
         *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(a.cx_lo) + off) = pack_f16(l0, l1);
       }
     }
+    if constexpr (!LOSS_ONLY) {
 #pragma unroll
-    for (int e = 0; e < 2; ++e) {               // bias gradient: column sums of d
-      const float c = rowgroup_sum(cs[e]);
-      if (f.g == 0 && n + e < NV && c != 0.f) atomicAdd(a.cx_db + n + e, (double)c);
+      for (int e = 0; e < 2; ++e) {             // bias gradient: column sums of d
+        const float c = rowgroup_sum(cs[e]);
+        if (f.g == 0 && n + e < NV && c != 0.f) atomicAdd(a.cx_db + n + e, (double)c);
+      }
     }
   }
   loss_acc += (double)d2;
@@ -523,7 +527,7 @@ struct NTCfg {
   static constexpr int NR = BN / 2;                        // accumulator registers per thread
 };
 
-template <int BN, int MODE, bool OUT16, bool CTX, bool VAR = false>
+template <int BN, int MODE, bool OUT16, bool CTX, bool VAR = false, bool LOSS_ONLY = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo,
@@ -652,8 +656,8 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
     f.m[1] = f.m[0] + 8;
     f.n0 = n0;
     if constexpr (CTX) {
-      if constexpr (MT::SPLIT) nt_output_ctx<NR>(sums, a, alpha, f, cx_loss);
-      else nt_output_ctx<NR>(acc, a, alpha, f, cx_loss);
+      if constexpr (MT::SPLIT) nt_output_ctx<NR, LOSS_ONLY>(sums, a, alpha, f, cx_loss);
+      else nt_output_ctx<NR, LOSS_ONLY>(acc, a, alpha, f, cx_loss);
     } else {
       if constexpr (MT::SPLIT) nt_output<NR, OUT16, VAR>(sums, a, alpha, f, s_stats);
       else nt_output<NR, OUT16, VAR>(acc, a, alpha, f, s_stats);
@@ -986,7 +990,7 @@ int make_map(CUtensorMap* map, const void* base, int mode, int rank, const uint6
     }                                                                      \
   } while (0)
 
-template <int BN, int MODE, bool OUT16, bool CTX, bool VAR = false>
+template <int BN, int MODE, bool OUT16, bool CTX, bool VAR = false, bool LOSS_ONLY = false>
 int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
               const CUtensorMap& bl, NTArgs a, cudaStream_t st) {
   using Cfg = NTCfg<BN, MODE>;
@@ -999,7 +1003,7 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
     return PASE_ERR_UNSUPPORTED;
   }
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt_kernel<BN, MODE, OUT16, CTX, VAR>,
+    cudaError_t e = cudaFuncSetAttribute(tc_gemm_nt_kernel<BN, MODE, OUT16, CTX, VAR, LOSS_ONLY>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) {
       pase_set_error("pase_tc_gemm_nt: smem attribute: %s", cudaGetErrorString(e));
@@ -1009,7 +1013,7 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
   }
   const long tiles = (long)((a.N + BN - 1) / BN) * ((a.M - a.m_base + BM - 1) / BM);
   const int grid = (int)(tiles < pase_num_sms() ? tiles : pase_num_sms());
-  PASE_LAUNCH((tc_gemm_nt_kernel<BN, MODE, OUT16, CTX, VAR>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
+  PASE_LAUNCH((tc_gemm_nt_kernel<BN, MODE, OUT16, CTX, VAR, LOSS_ONLY>), grid, NTHREADS, smem, st, ah, al, bh, bl, a);
   PASE_TC_LAUNCH_CHECK(CTX ? "pase_tc_gemm_nt_ctxmse" : "pase_tc_gemm_nt");
   return PASE_OK;
 }
@@ -1314,14 +1318,18 @@ int pase_tc_gemm_nt_var(const void* Ahi, const void* Alo, long a_rows, int R, co
 // Fused output layer of a regression head (MLPMinion W + ContextualizedLoss MSE,
 // minions.py:494-524, losses.py:15-37): residual = A B^T + bias - ctx(label) is never stored
 // as fp32; the fp16 pair of s * residual (the backward GEMMs' operand), sum residual^2 and
-// the column sums (bias gradient) come out of the GEMM epilogue.  3xF16 operands.
+// the column sums (bias gradient) come out of the GEMM epilogue.  3xF16 operands.  With Rhi,
+// Rlo and db_acc all NULL (no gradient will be taken, e.g. a validation pass) the loss-only
+// epilogue runs: the same sum residual^2, nothing else written.
 int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R, const void* Bhi,
                            const void* Blo, long ldb, void* Rhi, void* Rlo, long ldr, int M,
                            int N, int K, const float* bias, const float* label, int B, int F,
                            int T, int r, const float* scale, double* loss_acc, double* db_acc,
                            void* stream) {
-  PASE_CHECK_ARG(Ahi && Alo && Bhi && Blo && Rhi && Rlo && label && scale && loss_acc && db_acc,
-                 "pase_tc_gemm_nt_ctxmse: null pointer");
+  const bool loss_only = !Rhi && !Rlo && !db_acc;
+  PASE_CHECK_ARG(Ahi && Alo && Bhi && Blo && label && loss_acc &&
+                 (loss_only || (Rhi && Rlo && db_acc && scale)),
+                 "pase_tc_gemm_nt_ctxmse: null pointer (loss only: Rhi, Rlo and db_acc all NULL)");
   PASE_CHECK_ARG(M == B * T && N == F * r && r >= 1 && (r & 1) && K > 0,
                  "pase_tc_gemm_nt_ctxmse: need M == B*T, N == F*r, odd r (M=%d N=%d)", M, N);
   PASE_CHECK_ARG(R >= 64 && (R % 64) == 0 && (K % 8) == 0 && (ldb % 8) == 0 && ldb >= K,
@@ -1351,6 +1359,7 @@ int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
   a.stages = 0; a.stat_cols = 0;
   a.cx_label = label; a.cx_F = F; a.cx_T = T; a.cx_r = r; a.cx_nvalid = N; a.cx_scale = scale;
   a.cx_lo = Rlo; a.cx_loss = loss_acc; a.cx_db = db_acc;
+  if (loss_only) return launch_nt<128, 3, false, true, false, true>(ah, al, bh, bl, a, (cudaStream_t)stream);
   return launch_nt<128, 3, false, true>(ah, al, bh, bl, a, (cudaStream_t)stream);
 }
 

@@ -300,12 +300,15 @@ class _FusedLinearCtxMSE(torch.autograd.Function):
     ctx_r(label))^2) without ever storing the (rows, F*r) prediction in fp32 -- the GEMM
     epilogue emits the fp16 pair of the (power-of-two scaled) residual, which IS the operand
     of the two backward GEMMs, plus sum residual^2 and the bias gradient's column sums.
-    3xF16 precision only (the caller falls back to the unfused path otherwise)."""
+    3xF16 precision only (the caller falls back to the unfused path otherwise).
+
+    ``need_grad`` False (a validation pass): the loss-only epilogue, which writes sum
+    residual^2 and nothing else -- no residual pair, no pool entry, nothing saved."""
 
     _buffers = {}
 
     @staticmethod
-    def forward(ctx, h, weight, bias, label, F, r):
+    def forward(ctx, h, weight, bias, label, F, r, need_grad):
         h, ldh = _rows_ld(h.detach())
         rows, K = h.shape
         N = weight.shape[0]
@@ -317,6 +320,13 @@ class _FusedLinearCtxMSE(torch.autograd.Function):
         ldr = _ru(N, 128)
         hop = gemm.to_operand(_F16X3, _flat_from(h), rows * ldh)
         wop = gemm.to_operand(_F16X3, w2.reshape(-1), N * K, "weight")
+        b = None if bias is None else bias.detach().reshape(-1)
+        if not need_grad:
+            acc = torch.zeros(1, dtype=torch.float64, device=dev)
+            ops.call("pase_tc_gemm_nt_ctxmse", hop.hi, hop.lo, rows, ldh, wop.hi, wop.lo, K,
+                     None, None, ldr, rows, N, K, b, label.reshape(-1), B, F, T, r, None, acc,
+                     None)
+            return _loss_scalar(acc, rows * N)
         # power-of-two scale from the bound |residual| <= max||h_m|| max||W_n|| + max|b| + max|label|
         am = torch.zeros(4, dtype=torch.float32, device=dev)
         ops.call("pase_rownorm_max", _flat_from(h), ldh, rows, K, am[0:1])
@@ -336,8 +346,7 @@ class _FusedLinearCtxMSE(torch.autograd.Function):
         ent["busy"] = True                        # released by backward
         acc = torch.zeros(1 + ldr, dtype=torch.float64, device=dev)
         ops.call("pase_tc_gemm_nt_ctxmse", hop.hi, hop.lo, rows, ldh, wop.hi, wop.lo, K,
-                 ent["hi"], ent["lo"], ldr, rows, N, K,
-                 None if bias is None else bias.detach().reshape(-1), label.reshape(-1),
+                 ent["hi"], ent["lo"], ldr, rows, N, K, b, label.reshape(-1),
                  B, F, T, r, scale, acc[0:1], acc[1:])
         ctx.save_for_backward(h, w2, scale, acc)
         ctx.hop, ctx.ent = hop, ent
@@ -370,11 +379,15 @@ class _FusedLinearCtxMSE(torch.autograd.Function):
             ops.call("pase_cast_d2f", acc[1:], dbf, ldr, coef)
             db = dbf[:N] * g.detach().float()
         ent["busy"] = False
-        return dh, dW, db, None, None, None
+        return dh, dW, db, None, None, None, None
 
 
 def fused_linear_ctx_mse(h, weight, bias, label, F, r):
-    return _FusedLinearCtxMSE.apply(h, weight, bias, label, F, r)
+    # only backward releases a residual pair: without one to come (no_grad, or nothing that
+    # requires grad) the forward must not take a pair
+    need_grad = torch.is_grad_enabled() and any(
+        t is not None and t.requires_grad for t in (h, weight, bias))
+    return _FusedLinearCtxMSE.apply(h, weight, bias, label, F, r, need_grad)
 
 
 def fused_head_ok(K, ldh):

@@ -315,6 +315,157 @@ class GraphedTrainStep(object):
         return dict(zip(self.names, self.loss_host.tolist()))
 
 
+class GraphedEvalStep(object):
+    """The validation pass of the reference trainer (``_eval``, trainer.py:282-337) from a
+    resident corpus, one CUDA-graph replay per batch: batch assembly (``DeviceBatcher``), the
+    encoder in eval mode (BatchNorm on its running statistics) and every worker under
+    ``no_grad``, and each worker's unweighted loss with their fp32 sum (``pase.eval_losses``).
+
+        ev = GraphedEvalStep(model, va_batcher, B)      # model on CUDA
+        model.eval()
+        for indices in BatchSampler(RandomSampler(range(len(va_pool))), B, drop_last=True):
+            ev(indices)                   # plan on the host, upload, replay; does not wait
+        running_loss = ev.losses()        # {worker: [per batch], ..., 'total': [...]}, one D2H
+        ev.reset()                        # before the next pass
+        model.train()
+
+    Batch k of a pass writes row k of a device table of ``max_batches`` rows (default: the
+    drop_last batches of the batcher's pool); the row index travels in the uploaded plan, so a
+    call neither waits nor reads anything back.  ``losses()`` copies the pass's rows to the host
+    once and returns the reference's ``running_loss`` layout (classification workers, regression
+    workers, then 'total'), which its ``eval_logger`` takes as it is.  The host draws are the
+    eager pass's, in its order: the batch, then the three frames of each SPC head
+    (``TrainPlanner``).  Fused regression heads (``model.fuse_regression_loss``) run their
+    loss-only epilogue, as they do eagerly under ``no_grad``.
+
+    The replay reads the parameters and BatchNorm running statistics by address, so a pass sees
+    what the training steps before it wrote, and it writes none of them.  Like
+    ``GraphedTrainStep`` it runs on its own stream, after the caller's earlier work and with the
+    caller's stream ordered after it; it holds every encoder and decoder plan that existed at
+    capture.  A ``GraphedTrainStep`` at the same batch size shares the (3B, T) encoder plan
+    with it: both graphs write its buffers, which is safe because each call is ordered after
+    the caller's earlier work and the caller after it, so the two never run at once.  The first
+    `warmup` calls run eagerly through the code that is captured."""
+
+    def __init__(self, model, batcher, batch_size, max_batches=None, warmup=3, stream=None):
+        if int(warmup) < 1:
+            raise ValueError("GraphedEvalStep: warmup=%d; at least one eager batch builds the "
+                             "constants and buffers the capture reads" % warmup)
+        if int(batch_size) < 1:
+            raise ValueError("GraphedEvalStep: batch_size=%d" % batch_size)
+        self.planner = TrainPlanner(model, batcher)
+        params = list(model.parameters())
+        if not params or not all(p.is_cuda for p in params):
+            raise ValueError("GraphedEvalStep: the model must live on a CUDA device")
+        self.B, self.warmup = int(batch_size), int(warmup)
+        if max_batches is None:
+            max_batches = len(batcher.wavs) // self.B
+        if int(max_batches) < 1:
+            raise ValueError("GraphedEvalStep: max_batches=%d" % max_batches)
+        self.model, self.batcher = model, batcher
+        self.max_batches = int(max_batches)
+        self.device = params[0].device
+        # running_loss's order (trainer.py:306-326)
+        self.names = [w.name for w in list(model.classification_workers) +
+                      list(model.regression_workers)] + ["total"]
+        self.stream = stream if stream is not None else torch.cuda.Stream(device=self.device)
+        self.out = torch.zeros(self.max_batches, len(self.names), dtype=torch.float32,
+                               device=self.device)
+        self.out_host = torch.zeros(self.max_batches, len(self.names),
+                                    dtype=torch.float32).pin_memory()
+        self.done = torch.cuda.Event()
+        self.table = None                 # the graph's static plan table, sized by the first plan
+        self.graph = None
+        self._plans = []
+        self.calls = 0
+        self.k = 0                        # batches of the current pass
+        self._k = 0
+
+    def _alloc(self, n):
+        self.table = torch.zeros(n, dtype=torch.int64, device=self.device)
+        self._stage = [torch.zeros(n, dtype=torch.int64).pin_memory() for _ in (0, 1)]
+        self._staged = [torch.cuda.Event(), torch.cuda.Event()]
+
+    def _run(self):
+        """One batch as it is captured: everything reads the static table [plan | SPC frames |
+        row]."""
+        from .pase import eval_losses
+        model = self.model
+        nb = self.table.numel() - 1 - 3 * len(self.planner.spc)
+        with torch.no_grad():
+            batch = self.batcher.run(self.table[:nb])
+            for i, m in enumerate(self.planner.spc):
+                m.frame_table = self.table[nb + 3 * i:nb + 3 * i + 3]
+            try:
+                _, _, preds, labels = model(batch)
+            finally:
+                for m in self.planner.spc:
+                    m.frame_table = None
+            tot, losses = eval_losses(model, preds, labels)
+            vec = torch.stack([losses[n].reshape(()) for n in self.names[:-1]] +
+                              [tot.reshape(())])
+            self.out.index_copy_(0, self.table[-1:], vec[None])
+
+    def __call__(self, indices, rng=None):
+        if self.model.training:
+            raise ValueError("GraphedEvalStep: the model is in train mode; call model.eval() "
+                             "before the pass (BatchNorm must use its running statistics)")
+        indices = [int(i) for i in indices]
+        if len(indices) != self.B:
+            raise ValueError("GraphedEvalStep: a batch of %d indices, the pass was built for %d"
+                             % (len(indices), self.B))
+        if self.k >= self.max_batches:
+            raise RuntimeError("GraphedEvalStep: the loss table holds %d batches and this pass "
+                               "has filled it; call reset() to start the next pass"
+                               % self.max_batches)
+        _, table = self.planner(indices, rng)
+        table = np.append(table, np.int64(self.k))
+        if self.table is None:
+            self._alloc(table.size)
+        elif table.size != self.table.numel():
+            raise RuntimeError("GraphedEvalStep: the plan has %d entries, the captured pass %d"
+                               % (table.size, self.table.numel()))
+        k = self._k
+        self._staged[k].synchronize()          # the copy that last read this buffer has run
+        self._stage[k].numpy()[:] = table
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            self.table.copy_(self._stage[k], non_blocking=True)
+            self._staged[k].record(self.stream)
+            if self.calls < self.warmup:
+                self._run()
+            else:
+                if self.graph is None:
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g, stream=self.stream):
+                        self._run()
+                    self.graph = g
+                    self._plans = [p for m in self.model.modules()
+                                   for p in getattr(m, "_plans", {}).values()]
+                self.graph.replay()
+            self.done.record(self.stream)
+        torch.cuda.current_stream(self.device).wait_stream(self.stream)
+        self._k = 1 - k
+        self.k += 1
+        self.calls += 1
+
+    def losses(self):
+        """{worker name: [loss of batch 0, 1, ...], ..., 'total': [...]} (python floats) of the
+        batches of the current pass; one device-to-host copy, waits for the pass only."""
+        n = self.k
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            self.out_host[:n].copy_(self.out[:n], non_blocking=True)
+            self.done.record(self.stream)
+        self.done.synchronize()
+        rows = self.out_host[:n].tolist()
+        return {name: [r[j] for r in rows] for j, name in enumerate(self.names)}
+
+    def reset(self):
+        """Start the next pass at row 0 (the draws continue from the generators' state)."""
+        self.k = 0
+
+
 class PipelinedDPStep(object):
     """Data-parallel training step of the encoder with the gradient all-reduce HIDDEN behind
     the tail of backward (SURVEY.md 8e: pure DP, one flat gradient buffer).

@@ -93,3 +93,15 @@ def total_loss(model, preds, labels):
         losses[w.name] = l
         tot = tot + l
     return tot, losses
+
+
+def eval_losses(model, preds, labels):
+    """The losses of a validation batch as the reference trainer's ``_eval`` computes them
+    (trainer.py:303-326): each worker's UNWEIGHTED loss, classification workers first, then
+    regression workers, and their fp32 sum in that order."""
+    tot, losses = 0., {}
+    for w in list(model.classification_workers) + list(model.regression_workers):
+        l = w.loss(preds[w.name], labels[w.name])
+        losses[w.name] = l
+        tot = tot + l
+    return tot, losses
