@@ -331,6 +331,15 @@ int pase_out_affine_nct(const float* y, const float* scale, const float* shift,
  * sum in a fixed order. */
 int pase_out_affine_var(const float* y, const float* scale, const float* shift, float* out,
                         const int* tab, int nseg, int C, int mode, void* stream);
+/* Windowed output of one long recording (WaveFe.extract_long): rows 0..T-1 of y (T,C) as
+ * y*scale+shift (one fmaf, as pase_out_affine_nct) into columns col0 .. col0+T-1 of out (C,ldo),
+ * leading dimension ldo.  64-bit offsets: the output may exceed 2^31 elements. */
+int pase_out_place(const float* y, const float* scale, const float* shift, float* out, long ldo,
+                   long col0, int T, int C, void* stream);
+/* select_output (pase/models/modules.py:62-74) in place over a whole (C,T) output whose rows
+ * 0..C-1 hold h: mode 1 (avg_norm) h - mean_t h; 2 (avg_concat) rows C..2C-1 = mean_t h;
+ * 3 (avg_norm_concat) both.  The mean is a double sum in a fixed order. */
+int pase_out_select(float* out, long T, int C, int mode, void* stream);
 /* g_ntc = dout(N,C,T)^T + dout_ntc; S1 += g, S2 += g*xhat (double[C]) */
 int pase_out_bwd_reduce(const float* dout, const float* dout_ntc, const float* y,
                         const float* mean, const float* invstd, int N, int T, int C,
@@ -354,6 +363,12 @@ int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst,
  * (pase_qrnn_scan_plan), so its result is that of a B=1 scan.  Two launches. */
 int pase_qrnn_scan_fwd_var(const float* Y, float* h, long ldh, float* Cst, const int* tab,
                            int nseg, int H, void* stream);
+/* One recording's sequential scan continued over rows 0..T-1 of Y / h / Cst (B=1): the cell
+ * state enters from c_in[H] (NULL: zero) and the state after row T-1 is written to c_out[H]
+ * (c_out may equal c_in).  The per-step arithmetic is the sequential kernel's, so scanning a
+ * recording piece by piece reproduces pase_qrnn_scan_fwd's bits for T' > 512. */
+int pase_qrnn_scan_fwd_carry(const float* Y, float* h, long ldh, float* Cst, const float* c_in,
+                             float* c_out, int T, int H, void* stream);
 int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long lddh,
                        float* dY, int N, int T, int H, void* stream);
 /* Which kernels the two scans run for T time steps (host only, launches nothing): out1 =

@@ -777,6 +777,54 @@ out_affine_var_kernel(const float* __restrict__ y, const float* __restrict__ sca
   }
 }
 
+// Windowed output (WaveFe.extract_long): rows 0..T-1 of y, as h = y*scale+shift (the fmaf of
+// out_affine_nct_kernel), into columns col0 .. col0+T-1 of the (C, ldo) output.  32x32 tiles.
+__global__ void out_place_kernel(const float* __restrict__ y, const float* __restrict__ scale,
+                                 const float* __restrict__ shift, float* __restrict__ out,
+                                 long ldo, long col0, int T, int C) {
+  pdl_wait();
+  __shared__ float tile[32][33];
+  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int t = t0 + i, c = c0 + threadIdx.x;
+    if (t < T && c < C) tile[i][threadIdx.x] = fmaf(y[(long)t * C + c], scale[c], shift[c]);
+  }
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int c = c0 + i, t = t0 + threadIdx.x;
+    if (t < T && c < C) out[(long)c * ldo + col0 + t] = tile[threadIdx.x][i];
+  }
+}
+
+// select_output over a whole (C, T) output in place: one block per channel.  The time mean is
+// a double sum in a fixed order (per-thread strided sums, then a fixed tree), so it does not
+// depend on how the output was produced.  mode 1: h - mean; 2: rows C+c = mean; 3: both.
+__global__ void __launch_bounds__(256)
+out_select_kernel(float* __restrict__ out, long T, int C, int mode) {
+  pdl_wait();
+  __shared__ double part[256];
+  __shared__ float mean_s;
+  const int c = blockIdx.x, tid = threadIdx.x;
+  float* row = out + (long)c * T;
+  double s = 0.0;
+  for (long t = tid; t < T; t += 256) s += (double)row[t];
+  part[tid] = s;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (tid < w) part[tid] += part[tid + w];
+    __syncthreads();
+  }
+  if (tid == 0) mean_s = (float)(part[0] / (double)T);
+  __syncthreads();
+  const float m = mean_s;
+  const bool sub = mode == 1 || mode == 3, cat = mode >= 2;
+  float* mrow = out + (long)(C + c) * T;
+  for (long t = tid; t < T; t += 256) {
+    if (sub) row[t] -= m;
+    if (cat) mrow[t] = m;
+  }
+}
+
 // g[n,t,c] = dout_nct[n,c,t] (+ dout_ntc[n,t,c]); S1 += g, S2 += g*xhat
 __global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
                                       const float* __restrict__ dout_ntc,
@@ -1433,6 +1481,25 @@ int pase_out_affine_var(const float* y, const float* scale, const float* shift, 
   PASE_LAUNCH((out_affine_var_kernel), dim3((C + 31) / 32, nseg), dim3(32, 8), 0,
               (cudaStream_t)stream, y, scale, shift, out, tab, C, mode);
   PASE_LAUNCH_CHECK("pase_out_affine_var");
+  return PASE_OK;
+}
+
+int pase_out_place(const float* y, const float* scale, const float* shift, float* out, long ldo,
+                   long col0, int T, int C, void* stream) {
+  PASE_CHECK_ARG(y && scale && shift && out && T > 0 && C > 0, "pase_out_place: bad args");
+  PASE_CHECK_ARG(col0 >= 0 && col0 + T <= ldo, "pase_out_place: columns %ld..%ld past ldo=%ld",
+                 col0, col0 + T, ldo);
+  PASE_LAUNCH((out_place_kernel), dim3((T + 31) / 32, (C + 31) / 32), dim3(32, 8), 0,
+              (cudaStream_t)stream, y, scale, shift, out, ldo, col0, T, C);
+  PASE_LAUNCH_CHECK("pase_out_place");
+  return PASE_OK;
+}
+
+int pase_out_select(float* out, long T, int C, int mode, void* stream) {
+  PASE_CHECK_ARG(out && T > 0 && C > 0, "pase_out_select: bad args");
+  PASE_CHECK_ARG(mode >= 1 && mode <= 3, "pase_out_select: mode %d", mode);
+  PASE_LAUNCH((out_select_kernel), dim3(C), 256, 0, (cudaStream_t)stream, out, T, C, mode);
+  PASE_LAUNCH_CHECK("pase_out_select");
   return PASE_OK;
 }
 

@@ -706,6 +706,24 @@ def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None):
     """Eval-mode forward of utterances packed in x (fp32, sum(lengths) samples, plan.wave):
     each one computed as a B=1 forward would.  Launches do not depend on the number of
     utterances.  Returns the list of (1, E, T'_i) features, views of one new buffer."""
+    sz, tab = _packed_front(plan, mod, x, lengths, geoms, params, mode)
+    n = len(lengths)
+    if plan.rnn:
+        ops.call("pase_qrnn_scan_fwd_var", plan.Yg, plan.cat, plan.Kc, plan.Cst, tab("scan"), n,
+                 plan.H)
+    _packed_out_proj(plan, mod, params, sz["rows"])
+    bo = plan.bn_out
+    out = torch.empty(sz["out"], dtype=torch.float32, device=x.device)
+    ops.call("pase_out_affine_var", plan.yout, bo[2], bo[3], out, tab("out"), n, plan.emb,
+             OUT_MODES[mode])
+    E = sz["E"]
+    return [out[o:o + E * t].view(1, E, t) for o, t in zip(sz["offsets"], sz["Tq"])]
+
+
+def _packed_front(plan, mod, x, lengths, geoms, params, mode):
+    """encoder_forward_packed up to the QRNN scan: every conv block, the pooled skips in
+    plan.cat and (rnn configs) the gate pre-activations of every frame in plan.Yg.
+    -> (sizes of packed_layout, section -> device table view)."""
     call = ops.call
     G, n = plan.geoms, len(lengths)
     host, sec, sz = packed_layout(plan, lengths, geoms, mode)
@@ -753,20 +771,236 @@ def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None):
         plan.nt_var("xq", plan.xq, Cq, "Wq", plan.Wq, 2 * Cq, True, plan.Yg, 3 * H,
                     sz["xq_rows"], 3 * H, 2 * Cq, P("rnn.layers.0.linear.bias"), tab("qgemm"), n,
                     1)
-        call("pase_qrnn_scan_fwd_var", plan.Yg, plan.cat, Kc, plan.Cst, tab("scan"), n, H)
+    return sz, tab
 
-    # the output projection is uniform over the sum of the frame counts
+
+def _packed_out_proj(plan, mod, params, rows):
+    """The output projection [W | skips] of `rows` packed frames into plan.yout (uniform over
+    the frames) and the eval-mode norm_out affine into plan.bn_out."""
+    Kc, emb = plan.Kc, plan.emb
     _out_weights(plan, params)
     gemm.nt(plan.precision, plan.cat, Kc, rows * Kc, plan.Wcat, Kc, plan.yout, emb, rows, emb,
-            Kc, 1.0, P("W.bias"), a_op=lambda: plan.operand("cat", plan.cat, True, n=rows * Kc),
+            Kc, 1.0, _flat(params["W.bias"]),
+            a_op=lambda: plan.operand("cat", plan.cat, True, n=rows * Kc),
             b_op=lambda: plan.operand("Wcat", plan.Wcat, True, "weight"))
-    bo = plan.bn_out
     if plan.norm_out:
-        _out_bn_eval_affine(plan, buf)
-    out = torch.empty(sz["out"], dtype=torch.float32, device=x.device)
-    call("pase_out_affine_var", plan.yout, bo[2], bo[3], out, tab("out"), n, emb, OUT_MODES[mode])
-    E = sz["E"]
-    return [out[o:o + E * t].view(1, E, t) for o, t in zip(sz["offsets"], sz["Tq"])]
+        _out_bn_eval_affine(plan, lambda name: _flat(mod.get_buffer(name)))
+
+
+# -- windowed inference of one long recording (DESIGN.md section 15) --------------------------
+# The whole-recording forward runs the sequential QRNN scan for T' > 512 frames (qrnn.cu
+# seg_width); the carried window scan reproduces that one, so a window holds at least 512 frames.
+MIN_WINDOW_FRAMES = 512
+_TAIL_SEARCH_FRAMES = 2048
+_tail_cache = {}
+
+
+def hop_size(cfg):
+    """Samples per output frame: the product of the strides."""
+    return int(np.prod(cfg["strides"]))
+
+
+def min_window(cfg):
+    return MIN_WINDOW_FRAMES * hop_size(cfg)
+
+
+def _block_spans(cfg):
+    """Per block (a, b, R): frame t of block l reads samples R*t - a .. R*t + b (R: its stride
+    product), composed from the kernels, strides and left reflect pads of ConvGeom."""
+    spans, R, a, b = [], 1, 0, 0
+    for g in build_geometry(cfg, 1 << 20):
+        a, b = R * g.padL + a, R * (g.k - 1 - g.padL) + b
+        R *= g.s
+        spans.append((a, b, R))
+    return spans
+
+
+def receptive_field(cfg):
+    """(A, B): final frame j of a recording depends on samples hop*j - A .. hop*j + B only --
+    through the last block and, with dense skips, through the hop/R_l frames of block l pooled
+    into it (fuse_skip at its nominal pool factor)."""
+    hop, spans = hop_size(cfg), _block_spans(cfg)
+    A, B = spans[-1][0], spans[-1][1]
+    if cfg["denseskips"]:
+        for a, b, R in spans[:-1]:
+            A, B = max(A, a), max(B, hop - R + b)
+    return A, B
+
+
+def window_halos(cfg):
+    """(left, right) halo in frames: the left one covers A (plus the QRNN's x_{t-1}), the right
+    one B beyond the hop of a window's last frame."""
+    hop = hop_size(cfg)
+    A, B = receptive_field(cfg)
+    return _cdiv(A, hop) + (1 if cfg["rnn_pool"] else 0), _cdiv(B + 1 - hop, hop)
+
+
+def nominal_pool_factors(cfg):
+    """fuse_skip's d_l = T_out_l // T' for a long recording: the stride product after block l."""
+    s = cfg["strides"]
+    return [int(np.prod(s[l + 1:])) for l in range(len(s) - 1)]
+
+
+def pool_factors(cfg, L):
+    G = build_geometry(cfg, L)
+    return [max(g.T_out // G[-1].T_out, 1) for g in G[:-1]]
+
+
+def _tail_table(cfg):
+    """(tail, residues): segment lengths L with L mod hop in `residues` never get the nominal
+    pool factors (PASE+: L mod 160 >= 151 makes T' = ceil(L/160), so d_0 = 159); in every other
+    residue class each length >= tail has them (and valid reflect pads)."""
+    key = (tuple(cfg["kwidths"]), tuple(cfg["strides"]), bool(cfg["sincnet"]),
+           bool(cfg["denseskips"]))
+    if key in _tail_cache:
+        return _tail_cache[key]
+    hop = hop_size(cfg)
+    lens = np.arange(_TAIL_SEARCH_FRAMES * hop, dtype=np.int64)      # row f, column r: f*hop+r
+    L, ok, outs = lens, lens > 0, []
+    for g in build_geometry(cfg, 1 << 20):
+        ok &= (L > g.padL) & (L > g.padR)
+        L = (L + g.padL + g.padR - g.k) // g.s + 1
+        outs.append(L)
+    if cfg["denseskips"]:
+        Tq = np.maximum(outs[-1], 1)
+        for l, d in enumerate(nominal_pool_factors(cfg)):
+            ok &= np.maximum(outs[l] // Tq, 1) == d
+    ok = ok.reshape(-1, hop)
+    half = ok.shape[0] // 2
+    residues = [r for r in range(hop) if not ok[half:, r].all()]
+    tail = 1
+    for r in range(hop):
+        bad = np.nonzero(~ok[:, r])[0]
+        if r not in residues and bad.size:
+            tail = max(tail, (int(bad[-1]) + 1) * hop + r)
+    _tail_cache[key] = (tail, residues)
+    return tail, residues
+
+
+def tail_length(cfg):
+    """Shortest segment length from which on every longer one (outside the residues of
+    _tail_table) has the nominal pool factors.  A short segment pools skip l over more than d_l
+    frames (7597 samples: d_0 = 161 in PASE+), so a recording's last segment is extended to
+    this length."""
+    return _tail_table(cfg)[0]
+
+
+def check_windowable(cfg, L):
+    """NotImplementedError when a recording of L samples pools its skips at other than the
+    nominal factors: its whole-recording frames then drift against any hop-aligned segment."""
+    if not cfg["denseskips"]:
+        return
+    residues = _tail_table(cfg)[1]
+    if L % hop_size(cfg) in residues or (L >= tail_length(cfg) and
+                                         pool_factors(cfg, L) != nominal_pool_factors(cfg)):
+        raise NotImplementedError(
+            "a recording of %d samples (%d mod %d) pools its dense skips over %s frames, not the "
+            "nominal %s, so no hop-aligned window reproduces its frames; trim or pad it to a "
+            "length mod %d outside %d..%d" % (L, L % hop_size(cfg), hop_size(cfg),
+                                              pool_factors(cfg, L), nominal_pool_factors(cfg),
+                                              hop_size(cfg), min(residues), max(residues)))
+
+
+def window_capacity(cfg, window):
+    """Samples of the longest segment plan_windows / a FeatureStream builds for `window`:
+    window + both halos + one hop + the tail extension, whatever the recording's length."""
+    hl, hr = window_halos(cfg)
+    hop = hop_size(cfg)
+    return hop * (window // hop + hl + hr + 1) + tail_length(cfg)
+
+
+def stream_end(cfg, n):
+    """Where a stream's segment ends once n samples have arrived: n, less the last few samples
+    when n mod hop falls in the residues without nominal pool factors (_tail_table)."""
+    residues, hop = _tail_table(cfg)[1], hop_size(cfg)
+    return n - (n % hop - min(residues) + 1) if n % hop in residues else n
+
+
+def final_frames(cfg, n):
+    """Frames of a stream that are final once its first n samples have arrived: frame j reads
+    up to sample hop*j + B, and the segment that computes it needs tail_length samples (and a
+    length outside the residues of _tail_table: stream_end)."""
+    n = stream_end(cfg, n)
+    if n < tail_length(cfg):
+        return 0
+    _, B = receptive_field(cfg)
+    return max(0, (n - B - 1) // hop_size(cfg) + 1)
+
+
+def make_segment(cfg, f0, f1, end):
+    """Segment computing frames f0 .. f1-1 from samples up to `end`: starts the left halo before
+    f0 on a hop boundary, extended left to tail_length samples (not before 0)."""
+    hop, tail = hop_size(cfg), tail_length(cfg)
+    s = max(0, f0 - window_halos(cfg)[0]) * hop
+    if end - s < tail:
+        s = max(0, (end - tail) // hop * hop)
+    return dict(seg_start=s, seg_len=end - s, crop_f0=f0 - s // hop, crop_n=f1 - f0)
+
+
+def check_segment(cfg, seg, at_end):
+    """Raise NotImplementedError unless the segment's crop is exactly the whole recording's
+    frames (at_end: the segment ends where the recording does)."""
+    hop = hop_size(cfg)
+    s, n, c0, cn = seg["seg_start"], seg["seg_len"], seg["crop_f0"], seg["crop_n"]
+    what = "segment at sample %d (%d samples, frames %d+%d)" % (s, n, c0, cn)
+    if s % hop or s < 0 or cn < 1 or c0 < 0:
+        raise NotImplementedError("%s: not hop-aligned" % what)
+    try:
+        G = build_geometry(cfg, n)
+    except ValueError as e:
+        raise NotImplementedError("%s: %s" % (what, e)) from None
+    if c0 + cn > G[-1].T_out:
+        raise NotImplementedError("%s: only %d frames" % (what, G[-1].T_out))
+    whole = s == 0 and at_end
+    if cfg["denseskips"] and not whole and pool_factors(cfg, n) != nominal_pool_factors(cfg):
+        raise NotImplementedError("%s: pool factors %s, not the nominal %s"
+                                  % (what, pool_factors(cfg, n), nominal_pool_factors(cfg)))
+    A, B = receptive_field(cfg)
+    lead = 1 if cfg["rnn_pool"] else 0
+    if s > 0 and hop * (c0 - lead) - A < 0:
+        raise NotImplementedError("%s: left halo short of the receptive field" % what)
+    if not at_end and hop * (c0 + cn - 1) + B > n - 1:
+        raise NotImplementedError("%s: right halo short of the receptive field" % what)
+
+
+def plan_windows(cfg, L, window):
+    """Segments of a recording of L samples for windows of `window` samples' frames: a list of
+    dict(seg_start, seg_len, crop_f0, crop_n) whose crops tile the recording's frames 0 .. T'-1
+    once, in order (crop_f0: first frame of the crop within the segment).  Host only; raises
+    ValueError for a bad window / a too-short recording and NotImplementedError when a segment
+    could not reproduce the whole-recording frames."""
+    hop = hop_size(cfg)
+    if window < min_window(cfg):
+        raise ValueError("window must be at least %d samples (%d frames), got %d"
+                         % (min_window(cfg), MIN_WINDOW_FRAMES, window))
+    T = build_geometry(cfg, L)[-1].T_out
+    check_windowable(cfg, L)
+    nw, hr = window // hop, window_halos(cfg)[1]
+    segs = []
+    for f0 in range(0, T, nw):
+        f1 = min(f0 + nw, T)
+        end = L if f1 == T else min(L, (f1 + hr) * hop)
+        seg = make_segment(cfg, f0, f1, end)
+        check_segment(cfg, seg, end == L)
+        segs.append(seg)
+    return segs
+
+
+def encoder_forward_window(plan, mod, x, seg, geoms, params, carry, out, ldo, col0):
+    """One segment of a long recording (x: its seg_len samples, fp32): the packed front end as
+    a one-utterance pack, the QRNN scan over the crop's frames only, continuing from the state in
+    `carry` (H floats, updated), the output projection, and the crop's frames as y*scale+shift
+    into columns col0 .. of the (emb, ldo) tensor `out`."""
+    sz, _ = _packed_front(plan, mod, x, [seg["seg_len"]], [geoms], params, None)
+    f0, n = seg["crop_f0"], seg["crop_n"]
+    if plan.rnn:
+        H, Kc = plan.H, plan.Kc
+        ops.call("pase_qrnn_scan_fwd_carry", plan.Yg[f0 * 3 * H:], plan.cat[f0 * Kc:], Kc,
+                 plan.Cst[f0 * H:], carry, carry, n, H)
+    _packed_out_proj(plan, mod, params, sz["rows"])
+    bo = plan.bn_out
+    ops.call("pase_out_place", plan.yout[f0 * plan.emb:], bo[2], bo[3], out, ldo, col0, n,
+             plan.emb)
 
 
 def encoder_backward(plan, mod, params, gout, gntc, training, sink=None):

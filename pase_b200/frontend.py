@@ -19,6 +19,7 @@ import torch.nn as nn
 from .modules import Model, format_frontend_chunk, format_frontend_output
 from . import encoder as _enc
 from . import gemm as _gemm
+from . import ops as _ops
 
 # "3xtf32": wgmma tensor cores with error-compensated TF32 (fp32-equivalent, meets the
 # fp32 parity bar); "fp32": FFMA kernels; "tf32": single-pass TF32 (L2-equivalent only).
@@ -33,6 +34,9 @@ DEFAULT_PRECISION = "auto"
 # this sizes holds 1.35 GB for PASE+ in 3xf16 and 0.75 GB in bf16 (EncoderPlan.nbytes() after a
 # call, operand buffers included).
 EXTRACT_MAX_SAMPLES = 1 << 20
+
+# Samples whose frames one segment of WaveFe.extract_long computes (65.5 s of 16 kHz audio).
+EXTRACT_LONG_WINDOW = 1 << 20
 
 _DEFAULTS = dict(
     num_inputs=1, sincnet=True,
@@ -150,6 +154,7 @@ class WaveFe(Model):
             self.norm_out = nn.BatchNorm1d(emb, affine=False)
         self._plans = OrderedDict()
         self._packed_plans = OrderedDict()
+        self._stagers, self._carries = {}, {}
         # GEMM numerics (gemm.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (wgmma,
         # fp32-equivalent), "tf32" (wgmma), "bf16" (wgmma, bf16 operands and activations)
         self.precision = os.environ.get("PASE_B200_PRECISION", DEFAULT_PRECISION)
@@ -295,6 +300,92 @@ class WaveFe(Model):
                                                      params, mode)
         return feats
 
+    def _eval_device(self, what):
+        if self.training:
+            raise RuntimeError("WaveFe.%s runs the encoder in eval mode; call .eval() first"
+                               % what)
+        device = self.W.weight.device
+        if device.type != "cuda":
+            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; the module lives "
+                               "on %s. There is no CPU path." % device)
+        return device
+
+    def extract_long(self, wav, mode=None, window=None):
+        """Features of one recording of any length in memory bounded by the window: (1, emb',
+        T') CUDA tensor equal to ``self(wav.view(1,1,-1), mode=mode)``.  The recording is cut
+        into segments whose crops hold `window` samples' frames (default EXTRACT_LONG_WINDOW,
+        at least encoder.min_window), each with halos covering the receptive field, and the
+        QRNN state is carried from one to the next (DESIGN.md section 15).  A recording of at
+        most `window` samples runs as one forward of `extract`.  wav: fp32 (T,), (1,T) or
+        (1,1,T) on the CPU (staged segment by segment through pinned memory) or the GPU.
+        Eval mode only."""
+        return self._extract_long(wav, mode, window, self._eval_device("extract_long"))
+
+    def _extract_long(self, wav, mode, window, device):
+        if mode not in _enc.OUT_MODES:
+            raise ValueError("mode must be one of %s, got %r" % (list(_enc.OUT_MODES), mode))
+        x = _recording(wav)
+        win = EXTRACT_LONG_WINDOW if window is None else int(window)
+        cfg, L = self.cfg, x.numel()
+        if win < _enc.min_window(cfg):
+            raise ValueError("window must be at least %d samples, got %d"
+                             % (_enc.min_window(cfg), win))
+        if L <= win:
+            return self._extract([x], mode, win, device)[0]
+        segs = _enc.plan_windows(cfg, L, win)            # every check before the first launch
+        T = _enc.frame_counts(cfg, L)[-1]
+        emb = self.emb_dim
+        E = emb * (2 if mode in ("avg_concat", "avg_norm_concat") else 1)
+        plan = self._packed_plan(_enc.window_capacity(cfg, win), device)
+        fold = plan.precision.sinc_fold
+        stage = None
+        if device.type == "cuda" and not x.is_cuda:
+            stage = self._stager(plan.capacity)
+        elif x.device != device:
+            x = x.to(device)
+        self._sinc_consts(device)
+        params = dict(self.named_parameters())
+        out = torch.empty(E, T, dtype=torch.float32, device=device)
+        carry = self._carry(plan, device)
+        col = 0
+        with torch.no_grad():
+            for seg in segs:
+                s, n = seg["seg_start"], seg["seg_len"]
+                xs = x[s:s + n] if stage is None else stage.put(x[s:s + n], plan.wave)
+                _enc.encoder_forward_window(plan, self, xs, seg,
+                                            _enc.build_geometry(cfg, n, fold), params, carry,
+                                            out, T, col)
+                col += seg["crop_n"]
+            if mode is not None:
+                _ops.call("pase_out_select", out, T, emb, _enc.OUT_MODES[mode])
+        return out.view(1, E, T)
+
+    def stream(self, mode=None, window=None):
+        """A FeatureStream over this encoder: push() samples as they arrive, get back the
+        frames that are already final.  Eval mode only, mode None only (the avg modes need the
+        whole recording)."""
+        device = self._eval_device("stream")
+        if mode is not None:
+            raise ValueError("a FeatureStream returns mode None features only; select_output "
+                             "modes need the whole recording (use extract_long)")
+        return FeatureStream(self, device, window)
+
+    def _stager(self, n):
+        st = self._stagers.get(n)
+        if st is None:
+            st = self._stagers[n] = _PinnedStager(n)
+        return st
+
+    def _carry(self, plan, device):
+        """Zeroed QRNN state of a windowed forward (one buffer per device, reused)."""
+        if not plan.rnn:
+            return None
+        c = self._carries.get(str(device))
+        if c is None or c.numel() != plan.H:
+            c = self._carries[str(device)] = torch.zeros(plan.H, dtype=torch.float32,
+                                                         device=device)
+        return c.zero_()
+
     def forward(self, batch, device=None, mode=None):
         if device is None:
             # Model.parameters() only yields trainable parameters: a frozen encoder (a fixed
@@ -309,3 +400,120 @@ class WaveFe(Model):
 
     def frame_counts(self, T):
         return _enc.frame_counts(self.cfg, T)
+
+
+def _recording(w):
+    """One fp32 recording as (T,), (1,T) or (1,1,T) -> its flat contiguous (T,) view."""
+    if not isinstance(w, torch.Tensor) or w.dtype != torch.float32:
+        raise TypeError("expected an fp32 tensor, got %s" % getattr(w, "dtype", type(w)))
+    if w.dim() == 0 or w.dim() > 3 or any(d != 1 for d in w.shape[:-1]):
+        raise ValueError("expected a (T,), (1,T) or (1,1,T) recording, got %s"
+                         % (tuple(w.shape),))
+    return w.reshape(-1).contiguous()
+
+
+class _PinnedStager(object):
+    """Two pinned host buffers of n floats: a CPU segment is copied into one while the device
+    may still be reading the other, then sent to the device asynchronously."""
+
+    def __init__(self, n):
+        self.bufs = [torch.empty(n, dtype=torch.float32).pin_memory() for _ in range(2)]
+        self.events = [None, None]
+        self.i = 0
+
+    def put(self, src, dst):
+        i, self.i = self.i, self.i ^ 1
+        if self.events[i] is not None:
+            self.events[i].synchronize()          # its last copy to the device has finished
+        n = src.numel()
+        self.bufs[i][:n].copy_(src)
+        d = dst[:n]
+        d.copy_(self.bufs[i][:n], non_blocking=True)
+        self.events[i] = torch.cuda.Event()
+        self.events[i].record()
+        return d
+
+
+class FeatureStream(object):
+    """Online feature extraction of one recording (WaveFe.stream()).  push(samples) returns the
+    (1, emb, n) frames that became final (n may be 0): frame j is final once sample
+    hop*j + B has arrived (B: encoder.receptive_field, 1335 samples for PASE+) and at least
+    encoder.tail_length samples have.  finish() returns the rest, the end of the recording
+    reflect-padded as a whole-recording forward pads it.  The frames concatenate to
+    ``WaveFe.extract_long`` of the whole recording (bit-equal when it has more than 512
+    frames, where both run the sequential QRNN scan).  Between calls the stream holds only the
+    samples its next segment reads again (halo and tail), the QRNN state and frame counters."""
+
+    def __init__(self, model, device, window=None):
+        cfg = model.cfg
+        win = _enc.min_window(cfg) if window is None else int(window)
+        if win < _enc.min_window(cfg):
+            raise ValueError("window must be at least %d samples, got %d"
+                             % (_enc.min_window(cfg), win))
+        self.model, self.device, self.cfg = model, device, cfg
+        self.chunk = win // _enc.hop_size(cfg) * _enc.hop_size(cfg)
+        self.min_len = _enc.min_length(cfg)
+        self.plan = model._packed_plan(_enc.window_capacity(cfg, win), device)
+        self.carry = (torch.zeros(self.plan.H, dtype=torch.float32, device=device)
+                      if self.plan.rnn else None)
+        self.buf = None            # samples buf0 .. n-1 (the ones a later segment reads)
+        self.buf0 = 0
+        self.n = 0                 # samples received
+        self.done = 0              # frames returned
+        self.finished = False
+
+    def push(self, samples):
+        if self.finished:
+            raise RuntimeError("FeatureStream.push after finish()")
+        x = _recording(samples)
+        outs = []
+        for a in range(0, x.numel(), self.chunk):
+            piece = x[a:a + self.chunk]
+            self.buf = piece.clone() if self.buf is None else torch.cat([self.buf,
+                                                                         piece.to(self.buf)])
+            self.n += piece.numel()
+            f1 = _enc.final_frames(self.cfg, self.n)
+            if f1 > self.done:
+                outs.append(self._run(f1, False))
+        if not outs:
+            return torch.empty(1, self.model.emb_dim, 0, dtype=torch.float32, device=self.device)
+        return outs[0] if len(outs) == 1 else torch.cat(outs, 2)
+
+    def finish(self):
+        if self.finished:
+            raise RuntimeError("FeatureStream.finish called twice")
+        if self.n < self.min_len:
+            raise ValueError("a recording of %d samples is shorter than the encoder's minimum "
+                             "of %d" % (self.n, self.min_len))
+        if self.done > 0:
+            _enc.check_windowable(self.cfg, self.n)
+        self.finished = True
+        T = _enc.frame_counts(self.cfg, self.n)[-1]
+        if T > self.done:
+            return self._run(T, True)
+        return torch.empty(1, self.model.emb_dim, 0, dtype=torch.float32, device=self.device)
+
+    def _run(self, f1, at_end):
+        cfg, plan, m = self.cfg, self.plan, self.model
+        seg = _enc.make_segment(cfg, self.done, f1,
+                                self.n if at_end else _enc.stream_end(cfg, self.n))
+        _enc.check_segment(cfg, seg, at_end)
+        s, n = seg["seg_start"], seg["seg_len"]
+        assert s >= self.buf0 and n <= plan.capacity
+        x = plan.wave[:n]
+        x.copy_(self.buf[s - self.buf0:s - self.buf0 + n])
+        out = torch.empty(m.emb_dim, f1 - self.done, dtype=torch.float32, device=self.device)
+        m._sinc_consts(self.device)
+        with torch.no_grad():
+            _enc.encoder_forward_window(
+                plan, m, x, seg, _enc.build_geometry(cfg, n, plan.precision.sinc_fold),
+                dict(m.named_parameters()), self.carry, out, f1 - self.done, 0)
+        self.done = f1
+        # keep what the next segment can read: from its left halo or its tail extension
+        hop = _enc.hop_size(cfg)
+        keep = min(max(0, self.done - _enc.window_halos(cfg)[0]) * hop,
+                   max(0, (_enc.stream_end(cfg, self.n) - _enc.tail_length(cfg)) // hop * hop))
+        if keep > self.buf0:
+            self.buf = self.buf[keep - self.buf0:].clone()
+            self.buf0 = keep
+        return out.view(1, m.emb_dim, -1)
