@@ -336,6 +336,12 @@ int pase_out_affine_var(const float* y, const float* scale, const float* shift, 
  * leading dimension ldo.  64-bit offsets: the output may exceed 2^31 elements. */
 int pase_out_place(const float* y, const float* scale, const float* shift, float* out, long ldo,
                    long col0, int T, int C, void* stream);
+/* pase_out_place for many streams' crops at once (StreamPool): tab (DEVICE, nseg rows of 5
+ * ints) {row0, T, ocol, ldo, col0}: rows row0 .. row0+T-1 of y (rows,C) as y*scale+shift (the
+ * same fmaf) into columns col0 .. col0+T-1 of the (C, ldo) block starting at element ocol*C of
+ * out.  max_T >= every row's T.  64-bit element offsets. */
+int pase_out_place_var(const float* y, const float* scale, const float* shift, float* out,
+                       const int* tab, int nseg, int max_T, int C, void* stream);
 /* select_output (pase/models/modules.py:62-74) in place over a whole (C,T) output whose rows
  * 0..C-1 hold h: mode 1 (avg_norm) h - mean_t h; 2 (avg_concat) rows C..2C-1 = mean_t h;
  * 3 (avg_norm_concat) both.  The mean is a double sum in a fixed order. */
@@ -369,6 +375,13 @@ int pase_qrnn_scan_fwd_var(const float* Y, float* h, long ldh, float* Cst, const
  * recording piece by piece reproduces pase_qrnn_scan_fwd's bits for T' > 512. */
 int pase_qrnn_scan_fwd_carry(const float* Y, float* h, long ldh, float* Cst, const float* c_in,
                              float* c_out, int T, int H, void* stream);
+/* pase_qrnn_scan_fwd_carry for many streams at once (StreamPool): tab (DEVICE, nseg rows of 4
+ * ints) {row0, T, slot, first}: rows row0 .. row0+T-1 of Y / h / Cst continue the scan of the
+ * stream whose state is row `slot` of state (max_streams, H), zero when first != 0; the state
+ * after the last row is written back there.  A slot appears at most once per call.  Same
+ * per-step body, so the same bits as pase_qrnn_scan_fwd_carry. */
+int pase_qrnn_scan_fwd_carry_var(const float* Y, float* h, long ldh, float* Cst, float* state,
+                                 const int* tab, int nseg, int H, void* stream);
 int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long lddh,
                        float* dY, int N, int T, int H, void* stream);
 /* Which kernels the two scans run for T time steps (host only, launches nothing): out1 =
@@ -407,6 +420,15 @@ int pase_spc_gather(const float* x, long ldx, const long* frames, int B, int T, 
  * zeros elsewhere (every element written, no atomics). */
 int pase_spc_gather_bwd(const float* g, const long* frames, int B, int T, int C, int N,
                         int seq_pad, float* dx, void* stream);
+/* ---- StreamPool sample history (csrc/stream.cu) --------------------------- */
+/* tab (DEVICE, nrow rows of 8 ints) {slot, head, nnew, stage_off, ring_s, old, seg_len,
+ * wave_off}: appends staging[stage_off .. +nnew) to ring slot `slot` (ring + slot*ring_cap,
+ * 64-bit) at positions head, head+1, .. mod ring_cap, and writes wave[wave_off .. +seg_len): its
+ * first `old` samples from the ring from position ring_s (mod ring_cap), the rest from
+ * staging[stage_off + i - old].  The positions read and appended must not overlap.  max_len >=
+ * every row's nnew and seg_len.  One launch. */
+int pase_stream_gather(const float* staging, float* ring, long ring_cap, float* wave,
+                       const int* tab, int nrow, int max_len, void* stream);
 /* misc fused vector helpers */
 int pase_axpy(const float* x, float* y, long n, float a, void* stream);
 int pase_scale_dev(float* x, long n, const float* dev_scalar, float host_coef, void* stream);

@@ -796,6 +796,33 @@ __global__ void out_place_kernel(const float* __restrict__ y, const float* __res
   }
 }
 
+// out_place_kernel for many streams' crops at once (StreamPool): segment blockIdx.z's row
+// {row0, T, ocol, ldo, col0} writes rows row0 .. row0+T-1 of y into columns col0 .. col0+T-1 of
+// the (C, ldo) block that starts at element ocol*C of out.  Same fmaf, same 32x32 tiles.
+__global__ void out_place_var_kernel(const float* __restrict__ y, const float* __restrict__ scale,
+                                     const float* __restrict__ shift, float* __restrict__ out,
+                                     const int* __restrict__ tab, int C) {
+  pdl_wait();
+  __shared__ float tile[32][33];
+  const int* row = tab + 5 * blockIdx.z;
+  const long row0 = __ldg(row);
+  const int T = __ldg(row + 1);
+  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  if (t0 >= T) return;                        // uniform over the block
+  const long ldo = __ldg(row + 3), col0 = __ldg(row + 4);
+  float* o = out + (long)__ldg(row + 2) * C;
+  const float* yr = y + row0 * C;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int t = t0 + i, c = c0 + threadIdx.x;
+    if (t < T && c < C) tile[i][threadIdx.x] = fmaf(yr[(long)t * C + c], scale[c], shift[c]);
+  }
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int c = c0 + i, t = t0 + threadIdx.x;
+    if (t < T && c < C) o[(long)c * ldo + col0 + t] = tile[threadIdx.x][i];
+  }
+}
+
 // select_output over a whole (C, T) output in place: one block per channel.  The time mean is
 // a double sum in a fixed order (per-thread strided sums, then a fixed tree), so it does not
 // depend on how the output was produced.  mode 1: h - mean; 2: rows C+c = mean; 3: both.
@@ -1492,6 +1519,17 @@ int pase_out_place(const float* y, const float* scale, const float* shift, float
   PASE_LAUNCH((out_place_kernel), dim3((T + 31) / 32, (C + 31) / 32), dim3(32, 8), 0,
               (cudaStream_t)stream, y, scale, shift, out, ldo, col0, T, C);
   PASE_LAUNCH_CHECK("pase_out_place");
+  return PASE_OK;
+}
+
+int pase_out_place_var(const float* y, const float* scale, const float* shift, float* out,
+                       const int* tab, int nseg, int max_T, int C, void* stream) {
+  PASE_CHECK_ARG(y && scale && shift && out && tab && max_T > 0 && C > 0,
+                 "pase_out_place_var: bad args");
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535, "pase_out_place_var: nseg=%d", nseg);
+  PASE_LAUNCH((out_place_var_kernel), dim3((max_T + 31) / 32, (C + 31) / 32, nseg), dim3(32, 8),
+              0, (cudaStream_t)stream, y, scale, shift, out, tab, C);
+  PASE_LAUNCH_CHECK("pase_out_place_var");
   return PASE_OK;
 }
 

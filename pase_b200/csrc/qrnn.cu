@@ -69,6 +69,27 @@ qrnn_scan_fwd_carry_kernel(const float* __restrict__ Y, float* __restrict__ h, l
   c_out[c] = qrnn_fwd_seq(Y + c, h + c, ldh, Cst + c, T, H, c0);
 }
 
+// Many streams' scans continued at once (StreamPool): segment blockIdx.y's row {row0, T, slot,
+// first} scans rows row0 .. row0+T-1 from state[slot] (0 when first) and writes the state back.
+// A slot appears at most once per launch.
+__global__ void __launch_bounds__(128)
+qrnn_scan_fwd_carry_var_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
+                               float* __restrict__ Cst, float* __restrict__ state,
+                               const int* __restrict__ tab, int H) {
+  pdl_wait();
+  const int* row = tab + 4 * blockIdx.y;
+  const long row0 = __ldg(row);
+  const int T = __ldg(row + 1);
+  const long slot = __ldg(row + 2);
+  const int first = __ldg(row + 3);
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= H) return;
+  float* st = state + slot * H + c;
+  const float c0 = first ? 0.f : *st;
+  *st = qrnn_fwd_seq(Y + row0 * 3 * H + c, h + row0 * ldh + c, ldh, Cst + row0 * H + c, T, H,
+                     c0);
+}
+
 __global__ void __launch_bounds__(128)
 qrnn_scan_bwd_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
                      const float* __restrict__ dh, long lddh, float* __restrict__ dY, int T,
@@ -340,6 +361,17 @@ int pase_qrnn_scan_fwd_carry(const float* Y, float* h, long ldh, float* Cst, con
   PASE_LAUNCH((qrnn_scan_fwd_carry_kernel), dim3((H + 127) / 128), 128, 0, (cudaStream_t)stream,
               Y, h, ldh, Cst, c_in, c_out, T, H);
   PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd_carry");
+  return PASE_OK;
+}
+
+int pase_qrnn_scan_fwd_carry_var(const float* Y, float* h, long ldh, float* Cst, float* state,
+                                 const int* tab, int nseg, int H, void* stream) {
+  PASE_CHECK_ARG(Y && h && Cst && state && tab, "pase_qrnn_scan_fwd_carry_var: null pointer");
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535 && H > 0 && ldh >= H,
+                 "pase_qrnn_scan_fwd_carry_var: nseg=%d H=%d ldh=%ld", nseg, H, ldh);
+  PASE_LAUNCH((qrnn_scan_fwd_carry_var_kernel), dim3((H + 127) / 128, nseg), 128, 0,
+              (cudaStream_t)stream, Y, h, ldh, Cst, state, tab, H);
+  PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd_carry_var");
   return PASE_OK;
 }
 

@@ -724,11 +724,18 @@ def _packed_front(plan, mod, x, lengths, geoms, params, mode):
     """encoder_forward_packed up to the QRNN scan: every conv block, the pooled skips in
     plan.cat and (rnn configs) the gate pre-activations of every frame in plan.Yg.
     -> (sizes of packed_layout, section -> device table view)."""
-    call = ops.call
-    G, n = plan.geoms, len(lengths)
     host, sec, sz = packed_layout(plan, lengths, geoms, mode)
     plan.table[:host.numel()].copy_(host)                    # the one host-to-device copy
     tab = lambda name: plan.table[sec[name]:]
+    _packed_front_launch(plan, mod, x, sz, tab, params)
+    return sz, tab
+
+
+def _packed_front_launch(plan, mod, x, sz, tab, params):
+    """The launches of _packed_front, from a layout already on the device (tab: section ->
+    table view)."""
+    call = ops.call
+    G, n = plan.geoms, len(sz["Tq"])
     P = lambda name: _flat(params[name])
     buf = lambda name: _flat(mod.get_buffer(name))
     fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
@@ -771,7 +778,6 @@ def _packed_front(plan, mod, x, lengths, geoms, params, mode):
         plan.nt_var("xq", plan.xq, Cq, "Wq", plan.Wq, 2 * Cq, True, plan.Yg, 3 * H,
                     sz["xq_rows"], 3 * H, 2 * Cq, P("rnn.layers.0.linear.bias"), tab("qgemm"), n,
                     1)
-    return sz, tab
 
 
 def _packed_out_proj(plan, mod, params, rows):
@@ -961,6 +967,47 @@ def check_segment(cfg, seg, at_end):
         raise NotImplementedError("%s: left halo short of the receptive field" % what)
     if not at_end and hop * (c0 + cn - 1) + B > n - 1:
         raise NotImplementedError("%s: right halo short of the receptive field" % what)
+
+
+def stream_step(cfg, n, done, keep, add, at_end=False):
+    """The host planner of one stream (FeatureStream, StreamPool), as a pure function of its
+    counters: n samples received, frames 0 .. done-1 returned, samples from `keep` on held.
+    `add` more samples arrive (at_end: none, and the recording ends at n).  -> (n, done, keep,
+    seg) after the step, seg the make_segment dict computing the frames that became final (None
+    when none did).  keep is the first sample a later segment can read (its left halo or its
+    tail extension).  Raises before anything changes: ValueError for a finish shorter than
+    min_length, NotImplementedError for a finish at a length no segment can window or a
+    segment that fails check_segment."""
+    n += add
+    if at_end:
+        if n < min_length(cfg):
+            raise ValueError("a recording of %d samples is shorter than the encoder's minimum "
+                             "of %d" % (n, min_length(cfg)))
+        if done > 0:
+            check_windowable(cfg, n)
+        f1 = frame_counts(cfg, n)[-1]
+    else:
+        f1 = final_frames(cfg, n)
+    if f1 <= done:
+        return n, done, keep, None
+    seg = make_segment(cfg, done, f1, n if at_end else stream_end(cfg, n))
+    check_segment(cfg, seg, at_end)
+    hop = hop_size(cfg)
+    k = min(max(0, f1 - window_halos(cfg)[0]) * hop,
+            max(0, (stream_end(cfg, n) - tail_length(cfg)) // hop * hop))
+    return n, f1, max(keep, k), seg
+
+
+def stream_chunk(cfg, window):
+    """Samples of the pieces a stream cuts a longer push into: the window, hop-aligned."""
+    return window // hop_size(cfg) * hop_size(cfg)
+
+
+def stream_ring_capacity(cfg, window):
+    """Samples of one stream's history ring in a StreamPool: every sample a segment reads lies
+    in keep .. n (at most window_capacity of them, by stream_step) and one call's piece adds at
+    most stream_chunk more, so a ring this long never overwrites a sample still to be read."""
+    return window_capacity(cfg, window) + stream_chunk(cfg, window)
 
 
 def plan_windows(cfg, L, window):

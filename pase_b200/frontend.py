@@ -38,6 +38,11 @@ EXTRACT_MAX_SAMPLES = 1 << 20
 # Samples whose frames one segment of WaveFe.extract_long computes (65.5 s of 16 kHz audio).
 EXTRACT_LONG_WINDOW = 1 << 20
 
+# Samples packed into one forward of a StreamPool round: every segment holds at least
+# encoder.tail_length samples (24310 for PASE+), so a pack serves about 43 streams (DESIGN.md
+# section 16).  The plan it sizes is that of WaveFe.extract.
+STREAM_POOL_MAX_SAMPLES = EXTRACT_MAX_SAMPLES
+
 _DEFAULTS = dict(
     num_inputs=1, sincnet=True,
     kwidths=[251, 10, 5, 5, 5, 5, 5, 5], strides=[1, 10, 2, 1, 2, 1, 2, 2],
@@ -370,6 +375,17 @@ class WaveFe(Model):
                              "modes need the whole recording (use extract_long)")
         return FeatureStream(self, device, window)
 
+    def streams(self, max_streams, window=None, max_samples=None, mode=None):
+        """A StreamPool of up to `max_streams` live recordings at once: each push() runs every
+        stream's next segment in one packed forward per round (at most `max_samples` samples
+        per forward, default STREAM_POOL_MAX_SAMPLES), and each stream's frames are those of a
+        FeatureStream fed the same blocks.  Eval mode only, mode None only."""
+        device = self._eval_device("streams")
+        if mode is not None:
+            raise ValueError("a FeatureStream returns mode None features only; select_output "
+                             "modes need the whole recording (use extract_long)")
+        return StreamPool(self, device, max_streams, window, max_samples)
+
     def _stager(self, n):
         st = self._stagers.get(n)
         if st is None:
@@ -451,7 +467,7 @@ class FeatureStream(object):
             raise ValueError("window must be at least %d samples, got %d"
                              % (_enc.min_window(cfg), win))
         self.model, self.device, self.cfg = model, device, cfg
-        self.chunk = win // _enc.hop_size(cfg) * _enc.hop_size(cfg)
+        self.chunk = _enc.stream_chunk(cfg, win)
         self.min_len = _enc.min_length(cfg)
         self.plan = model._packed_plan(_enc.window_capacity(cfg, win), device)
         self.carry = (torch.zeros(self.plan.H, dtype=torch.float32, device=device)
@@ -471,10 +487,10 @@ class FeatureStream(object):
             piece = x[a:a + self.chunk]
             self.buf = piece.clone() if self.buf is None else torch.cat([self.buf,
                                                                          piece.to(self.buf)])
-            self.n += piece.numel()
-            f1 = _enc.final_frames(self.cfg, self.n)
-            if f1 > self.done:
-                outs.append(self._run(f1, False))
+            self.n, f1, keep, seg = _enc.stream_step(self.cfg, self.n, self.done, self.buf0,
+                                                     piece.numel())
+            if seg is not None:
+                outs.append(self._run(seg, f1, keep))
         if not outs:
             return torch.empty(1, self.model.emb_dim, 0, dtype=torch.float32, device=self.device)
         return outs[0] if len(outs) == 1 else torch.cat(outs, 2)
@@ -482,22 +498,14 @@ class FeatureStream(object):
     def finish(self):
         if self.finished:
             raise RuntimeError("FeatureStream.finish called twice")
-        if self.n < self.min_len:
-            raise ValueError("a recording of %d samples is shorter than the encoder's minimum "
-                             "of %d" % (self.n, self.min_len))
-        if self.done > 0:
-            _enc.check_windowable(self.cfg, self.n)
+        _, f1, keep, seg = _enc.stream_step(self.cfg, self.n, self.done, self.buf0, 0, True)
         self.finished = True
-        T = _enc.frame_counts(self.cfg, self.n)[-1]
-        if T > self.done:
-            return self._run(T, True)
+        if seg is not None:
+            return self._run(seg, f1, keep)
         return torch.empty(1, self.model.emb_dim, 0, dtype=torch.float32, device=self.device)
 
-    def _run(self, f1, at_end):
+    def _run(self, seg, f1, keep):
         cfg, plan, m = self.cfg, self.plan, self.model
-        seg = _enc.make_segment(cfg, self.done, f1,
-                                self.n if at_end else _enc.stream_end(cfg, self.n))
-        _enc.check_segment(cfg, seg, at_end)
         s, n = seg["seg_start"], seg["seg_len"]
         assert s >= self.buf0 and n <= plan.capacity
         x = plan.wave[:n]
@@ -509,11 +517,283 @@ class FeatureStream(object):
                 plan, m, x, seg, _enc.build_geometry(cfg, n, plan.precision.sinc_fold),
                 dict(m.named_parameters()), self.carry, out, f1 - self.done, 0)
         self.done = f1
-        # keep what the next segment can read: from its left halo or its tail extension
-        hop = _enc.hop_size(cfg)
-        keep = min(max(0, self.done - _enc.window_halos(cfg)[0]) * hop,
-                   max(0, (_enc.stream_end(cfg, self.n) - _enc.tail_length(cfg)) // hop * hop))
-        if keep > self.buf0:
+        if keep > self.buf0:                    # what the next segment can read (stream_step)
             self.buf = self.buf[keep - self.buf0:].clone()
             self.buf0 = keep
         return out.view(1, m.emb_dim, -1)
+
+
+# table row widths of the pool's kernels (include/pase_b200.h)
+_GATHER_W, _CARRY_W, _PLACE_W = 8, 4, 5
+
+
+class _PoolStream(object):
+    """Host counters of one pooled stream (those of FeatureStream): its ring slot, samples
+    received, frames returned and the first sample it still holds."""
+    __slots__ = ("slot", "n", "done", "keep")
+
+    def __init__(self, slot):
+        self.slot, self.n, self.done, self.keep = slot, 0, 0, 0
+
+
+class StreamPool(object):
+    """Online feature extraction of many live recordings at once (WaveFe.streams()).
+
+    open() returns a stream id; push({id: samples, ...}, finish=(ids...)) returns {id: (1, emb,
+    n) frames} for every id named, n >= 0.  Each stream's frames are exactly those of a
+    FeatureStream fed the same blocks (and finish()ed where named): every stream is planned by
+    the same host planner (encoder.stream_step) and cut into the same pieces.  Round r of a call
+    runs the r-th piece of every stream that has one (then each finishing stream's last
+    segment) as packs of at most max_samples samples; a pack is one packed forward whose
+    launches do not depend on how many streams it holds (DESIGN.md section 16).  Between calls
+    the device holds each stream's recent samples in a ring of an arena and its QRNN state in a
+    (max_streams, H) table; the host holds four counters per stream."""
+
+    def __init__(self, model, device, max_streams, window=None, max_samples=None):
+        cfg = model.cfg
+        win = _enc.min_window(cfg) if window is None else int(window)
+        if win < _enc.min_window(cfg):
+            raise ValueError("window must be at least %d samples, got %d"
+                             % (_enc.min_window(cfg), win))
+        if not 1 <= int(max_streams) <= 65535:           # one grid row per stream
+            raise ValueError("max_streams must be in 1..65535, got %r" % (max_streams,))
+        cap = STREAM_POOL_MAX_SAMPLES if max_samples is None else int(max_samples)
+        if cap < 1:
+            raise ValueError("max_samples must be positive, got %r" % (max_samples,))
+        self.model, self.device, self.cfg = model, device, cfg
+        self.max_streams, self.max_samples = int(max_streams), cap
+        self.chunk = _enc.stream_chunk(cfg, win)
+        self.plan = model._packed_plan(max(cap, _enc.window_capacity(cfg, win)), device)
+        self.ring_cap = _enc.stream_ring_capacity(cfg, win)
+        self.ring = torch.zeros(self.max_streams * self.ring_cap, dtype=torch.float32,
+                                device=device)
+        self.state = (torch.zeros(self.max_streams * self.plan.H, dtype=torch.float32,
+                                  device=device) if self.plan.rnn else None)
+        self._free = list(range(self.max_streams - 1, -1, -1))
+        self._streams, self._next_id = {}, 0
+        # two host staging slots (samples, table, event), as _PinnedStager; device copies
+        self._pin = device.type == "cuda"
+        self._host = [[None, None, None], [None, None, None]]
+        self._hi = 0
+        self._stage = torch.empty(0, dtype=torch.float32, device=device)
+        self._tab = torch.empty(0, dtype=torch.int32, device=device)
+
+    def open(self):
+        """A new stream's id; its slot starts from zero QRNN state and no samples."""
+        if not self._free:
+            raise RuntimeError("StreamPool: %d streams are open already (max_streams); finish "
+                               "one first" % self.max_streams)
+        sid, self._next_id = self._next_id, self._next_id + 1
+        self._streams[sid] = _PoolStream(self._free.pop())
+        return sid
+
+    def __len__(self):
+        return len(self._streams)
+
+    def push(self, blocks, finish=()):
+        """blocks: {id: fp32 (T,), (1,T) or (1,1,T) samples on the CPU or the pool's GPU};
+        finish: ids whose recording ends after this call's samples.  -> {id: (1, emb, n)} for
+        every id in either, views of one buffer.  Every argument is checked, and every segment
+        planned, before the first launch: a call that raises changes no stream."""
+        m, emb = self.model, self.model.emb_dim
+        if m.training:
+            raise RuntimeError("WaveFe.streams runs the encoder in eval mode; call .eval() first")
+        if m.W.weight.device != self.device:
+            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; the module lives "
+                               "on %s, the pool on %s. There is no CPU path."
+                               % (m.W.weight.device, self.device))
+        if not isinstance(blocks, dict):
+            raise TypeError("blocks must map stream ids to sample tensors, got %s"
+                            % type(blocks).__name__)
+        fin = list(dict.fromkeys(finish))
+        ids = list(blocks) + [i for i in fin if i not in blocks]
+        for i in ids:
+            if i not in self._streams:
+                raise KeyError("StreamPool: stream %r is unknown or finished" % (i,))
+        xs = {}
+        for i, b in blocks.items():
+            try:
+                x = _recording(b)
+            except (TypeError, ValueError) as e:
+                raise type(e)("stream %r: %s" % (i, e)) from None
+            if x.device.type != "cpu" and x.device != self.device:
+                raise ValueError("stream %r: samples on %s, the pool runs on %s"
+                                 % (i, x.device, self.device))
+            xs[i] = x
+        steps, new, closing = self._plan(ids, xs, set(fin))
+
+        col, views, ocol = 0, {}, {}
+        total = sum(new[i][1] - self._streams[i].done for i in ids)
+        out = torch.empty(emb * total, dtype=torch.float32, device=self.device)
+        for i in ids:
+            nf = new[i][1] - self._streams[i].done
+            views[i] = out[col * emb:(col + nf) * emb].view(1, emb, nf)
+            ocol[i] = col
+            col += nf
+        if total:
+            m._sinc_consts(self.device)
+        params = dict(m.named_parameters())
+        with torch.no_grad():
+            for r in range(max((len(s) for s in steps.values()), default=0)):
+                entries = [(i, steps[i][r]) for i in ids if r < len(steps[i])]
+                self._round(entries, out, ocol, new, params)
+        for i in ids:                                  # commit
+            st = self._streams[i]
+            st.n, st.done, st.keep = new[i]
+            if i in closing:
+                del self._streams[i]
+                self._free.append(st.slot)
+        return views
+
+    def _plan(self, ids, xs, fin):
+        """Every stream's steps of this call on the host, through encoder.stream_step: per id a
+        list of (piece or None, n before it, done before it, keep before it, segment or None),
+        its counters after the call, and the ids that finish.  Raises before any launch."""
+        cfg, steps, new = self.cfg, {}, {}
+        for i in ids:
+            st = self._streams[i]
+            n, done, keep = st.n, st.done, st.keep
+            out = []
+            x = xs.get(i)
+            L = 0 if x is None else x.numel()
+            for a in range(0, L, self.chunk):
+                piece = x[a:a + self.chunk]
+                n1, d1, k1, seg = _enc.stream_step(cfg, n, done, keep, piece.numel())
+                if n1 - keep > self.ring_cap or (seg is not None and seg["seg_start"] < keep):
+                    raise RuntimeError("StreamPool: stream %r would read samples %d .. %d from a "
+                                       "ring of %d" % (i, keep, n1, self.ring_cap))
+                out.append((piece, n, done, keep, seg))
+                n, done, keep = n1, d1, k1
+            if i in fin:
+                try:
+                    _, d1, k1, seg = _enc.stream_step(cfg, n, done, keep, 0, True)
+                except (ValueError, NotImplementedError) as e:
+                    raise type(e)("stream %r: %s" % (i, e)) from None
+                if seg is not None:
+                    out.append((None, n, done, keep, seg))
+                done, keep = d1, k1
+            steps[i], new[i] = out, (n, done, keep)
+        return steps, new, fin
+
+    def _round(self, entries, out, ocol, new, params):
+        """One round: stage the new samples, upload one table for every pack, then per pack the
+        gather, the packed front end, the carried scan, the output projection and the place."""
+        cfg, plan, emb = self.cfg, self.plan, self.model.emb_dim
+        call = _ops.call
+        # staging: host pieces first (one copy through pinned memory), then device pieces
+        host_p = [(i, e[0]) for i, e in entries if e[0] is not None and
+                  not (self._pin and e[0].is_cuda)]
+        dev_p = [(i, e[0]) for i, e in entries if e[0] is not None and self._pin and e[0].is_cuda]
+        stage_off, a = {}, 0
+        for i, p in host_p + dev_p:
+            stage_off[i] = a
+            a += p.numel()
+        nh = sum(p.numel() for _, p in host_p)
+        # packs over the round's segments; rows that only append go with the first pack
+        segs = [(i, e) for i, e in entries if e[4] is not None]
+        appends = [(i, e) for i, e in entries if e[4] is None and e[0] is not None]
+        lengths = [e[4]["seg_len"] for _, e in segs]
+        packs = _enc.split_packs(lengths, self.max_samples) or [(0, 0)]
+        fold = plan.precision.sinc_fold
+        geoms = _enc.utterance_geometry(cfg, lengths, fold)
+        parts, jobs, off = [], [], 0
+        for p, (a0, b0) in enumerate(packs):
+            g_rows, c_rows, p_rows = [], [], []
+            pk = segs[a0:b0]
+            if pk:
+                host, sec, sz = _enc.packed_layout(plan, lengths[a0:b0], geoms[a0:b0], None)
+                q0 = np.concatenate([[0], np.cumsum(sz["Tq"])])
+                wave_off = 0
+            for k, (i, (piece, n0, d0, k0, seg)) in enumerate(pk):
+                slot = self._streams[i].slot
+                s, sl = seg["seg_start"], seg["seg_len"]
+                nn = 0 if piece is None else piece.numel()
+                g_rows.append([slot, n0 % self.ring_cap, nn, stage_off.get(i, 0),
+                               s % self.ring_cap, n0 - s, sl, wave_off])
+                wave_off += sl
+                r0 = int(q0[k]) + seg["crop_f0"]
+                c_rows.append([r0, seg["crop_n"], slot, int(d0 == 0)])
+                p_rows.append([r0, seg["crop_n"], ocol[i], new[i][1] - self._streams[i].done,
+                               d0 - self._streams[i].done])
+            if p == 0:
+                for i, (piece, n0, _, _, _) in appends:
+                    g_rows.append([self._streams[i].slot, n0 % self.ring_cap, piece.numel(),
+                                   stage_off[i], 0, 0, 0, 0])
+            if not g_rows:
+                continue
+            job = dict(segs=len(pk), gather=(off, len(g_rows)))
+            parts.append(np.asarray(g_rows, dtype=np.int64).reshape(-1))
+            off += parts[-1].size
+            job["max_len"] = max(max(r[2], r[6]) for r in g_rows)
+            if pk:
+                job["sec"] = {k: v + off for k, v in sec.items()}
+                job["sz"] = sz
+                parts.append(host.numpy().astype(np.int64))
+                off += parts[-1].size
+                job["carry"] = off
+                parts.append(np.asarray(c_rows, dtype=np.int64).reshape(-1))
+                off += parts[-1].size
+                job["place"] = off
+                job["max_T"] = max(r[1] for r in p_rows)
+                parts.append(np.asarray(p_rows, dtype=np.int64).reshape(-1))
+                off += parts[-1].size
+            jobs.append(job)
+        if not jobs:
+            return
+        table = np.concatenate(parts)
+        assert np.abs(table).max() < _enc.INDEX_LIMIT     # `old` may be negative
+        stage, tab = self._upload([p for _, p in host_p], nh, a, table)
+        if dev_p:                                       # device blocks: one launch
+            torch.cat([p for _, p in dev_p], out=stage[nh:a])
+
+        bo = plan.bn_out
+        for job in jobs:
+            g0, gn = job["gather"]
+            call("pase_stream_gather", stage, self.ring, self.ring_cap, plan.wave, tab[g0:], gn,
+                 job["max_len"])
+            if not job["segs"]:
+                continue
+            sz, sec = job["sz"], job["sec"]
+            _enc._packed_front_launch(plan, self.model, plan.wave, sz,
+                                      lambda name, sec=sec: tab[sec[name]:], params)
+            if plan.rnn:
+                call("pase_qrnn_scan_fwd_carry_var", plan.Yg, plan.cat, plan.Kc, plan.Cst,
+                     self.state, tab[job["carry"]:], job["segs"], plan.H)
+            _enc._packed_out_proj(plan, self.model, params, sz["rows"])
+            call("pase_out_place_var", plan.yout, bo[2], bo[3], out, tab[job["place"]:],
+                 job["segs"], job["max_T"], emb)
+
+    def _upload(self, host_pieces, nh, n, table):
+        """The round's samples (host pieces into staging[0:nh]) and its table, each with one
+        copy from a pinned slot; the host waits only when it reuses a slot whose copies have
+        not finished.  -> (device staging, device table); both grow, never shrink."""
+        if self._stage.numel() < n:
+            self._stage = torch.empty(_grow(n), dtype=torch.float32, device=self.device)
+        if self._tab.numel() < table.size:
+            self._tab = torch.empty(_grow(table.size), dtype=torch.int32, device=self.device)
+        slot, self._hi = self._host[self._hi], self._hi ^ 1
+        if slot[2] is not None:
+            slot[2].synchronize()               # this slot's last copies have finished
+        if slot[0] is None or slot[0].numel() < nh:
+            slot[0] = _host_buffer(_grow(nh), torch.float32, self._pin)
+        if slot[1] is None or slot[1].numel() < table.size:
+            slot[1] = _host_buffer(_grow(table.size), torch.int32, self._pin)
+        if nh:
+            torch.cat(host_pieces, out=slot[0][:nh])
+            self._stage[:nh].copy_(slot[0][:nh], non_blocking=True)
+        slot[1][:table.size].copy_(torch.from_numpy(table.astype(np.int32)))
+        self._tab[:table.size].copy_(slot[1][:table.size], non_blocking=True)
+        if self._pin:
+            slot[2] = torch.cuda.Event()
+            slot[2].record()
+        return self._stage, self._tab
+
+
+def _grow(n):
+    """Capacity for n elements: the next power of two (at least 1024)."""
+    return max(1024, 1 << (int(n) - 1).bit_length())
+
+
+def _host_buffer(n, dtype, pinned):
+    t = torch.empty(n, dtype=dtype)
+    return t.pin_memory() if pinned else t
