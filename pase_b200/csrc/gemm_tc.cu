@@ -340,7 +340,7 @@ struct NTArgs {
   RowMap rm;
   double* colsum;
   double* colsumsq;
-  int accumulate, flush_kb, stages, stat_cols;
+  int accumulate, flush_kb, stages;
   // contextualised-MSE epilogue (fused regression head, tc_gemm_nt_kernel<.., CTX = true>):
   // C / cx_lo receive the fp16 pair of s * (prediction - label window) instead of the
   // prediction; cx_loss += sum d^2; cx_db[n] += sum_rows d
@@ -352,11 +352,37 @@ struct NTArgs {
   double* cx_db;
 };
 
+// BatchNorm column statistics of one tile: every consumer warp stores the fp32 sums of its 16
+// rows into a slab [8 warps][BN columns][sum y, sum y^2] with plain shared stores; after a
+// consumer barrier, nt_flush_stats adds the 8 partials of each (column, statistic) in fp64 and
+// in warp order, and issues one global fp64 add.  Two slabs alternate by tile parity, so the
+// next tile's stores never race the reads of this one without a second barrier.
+template <int BN>
+struct StatSlab {
+  static constexpr int WARP_BYTES = BN * 2 * 4;
+  static constexpr int TILE_BYTES = 8 * WARP_BYTES;
+  static constexpr int BYTES = 2 * TILE_BYTES;            // double-buffered
+};
+__device__ __forceinline__ void sts_v4(uint32_t addr, float x, float y, float z, float w) {
+  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(x), "f"(y), "f"(z),
+               "f"(w)
+               : "memory");
+}
+__device__ __forceinline__ float lds_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_add_f64(double* p, double v) {
+  asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
+}
+
 // Output stage of the NT kernel: alpha / bias, row map and validity, store (fp32 or bf16),
-// BatchNorm column statistics of the fp32 values (into shared-memory column sums).
+// this warp's partial BatchNorm column statistics of the fp32 values (into its StatSlab row at
+// shared address `slab`).
 template <int NR, bool OUT16, bool VAR>
 __device__ __forceinline__ void nt_output(float (&v)[NR], const NTArgs& a, float alpha,
-                                          const Frag& f, double* s_stats) {
+                                          const Frag& f, uint32_t slab) {
   const int N = a.N;
   long orow[2];
   int nlim[2];                             // columns [0, nlim) of the row are valid
@@ -425,16 +451,26 @@ __device__ __forceinline__ void nt_output(float (&v)[NR], const NTArgs& a, float
       }
     }
     if (want_stats) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const float c1 = rowgroup_sum(s1[e]), c2 = rowgroup_sum(s2[e]);
-        if (f.g == 0 && n + e < N && (c1 != 0.f || c2 != 0.f)) {
-          atomicAdd(&s_stats[n + e], (double)c1);
-          atomicAdd(&s_stats[a.stat_cols + n + e], (double)c2);
-        }
-      }
+      const float c0 = rowgroup_sum(s1[0]), q0 = rowgroup_sum(s2[0]);
+      const float c1 = rowgroup_sum(s1[1]), q1 = rowgroup_sum(s2[1]);
+      if (f.g == 0) sts_v4(slab + (n - f.n0) * 8, c0, q0, c1, q1);
     }
   }
+}
+
+// The tile's column statistics, after the consumer barrier that follows the slab stores: the
+// 256 consumer threads each own one (column, statistic) of the tile.  The 8 warp partials are
+// added in fixed order in fp64; only the order of the global adds across tiles varies, and it
+// moves bits below what the fp32 consumers of the statistics read (DESIGN.md §5).
+template <int BN>
+__device__ __forceinline__ void nt_flush_stats(const NTArgs& a, uint32_t slab, int n0) {
+  const int i = threadIdx.x - 128;
+  const int n = n0 + (i >> 1);
+  if (i >= 2 * BN || n >= a.N) return;
+  double s = 0.0;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) s += (double)lds_f32(slab + w * StatSlab<BN>::WARP_BYTES + 4 * i);
+  if (s != 0.0) red_add_f64(((i & 1) ? a.colsumsq : a.colsum) + n, s);
 }
 
 // Output stage of the fused regression head (losses.py:15-37 + nn.MSELoss fused into the
@@ -501,17 +537,6 @@ __device__ __forceinline__ void nt_output_ctx(const float (&v)[NR], const NTArgs
   loss_acc += (double)d2;
 }
 
-__device__ __forceinline__ void flush_stats(const NTArgs& a, const double* s_stats) {
-  consumer_sync();
-  for (int col = threadIdx.x - 128; col < a.N; col += 256) {
-    const double s = s_stats[col], b2 = s_stats[a.stat_cols + col];
-    if (s != 0.0 || b2 != 0.0) {
-      atomicAdd(a.colsum + col, s);
-      atomicAdd(a.colsumsq + col, b2);
-    }
-  }
-}
-
 // ------------------------------------------------------------------ NT kernel ----
 // Persistent: CTA b processes tiles b, b+grid, ... (n-tile fastest so concurrently running
 // CTAs share A rows in L2).  Stage = [A.hi | B.hi | A.lo | B.lo], each 128-byte K-major rows.
@@ -542,9 +567,7 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
   uint8_t* tiles = smem;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  // column sums in fp64: the order of the warps' additions then only moves bits that the
-  // fp32 consumers of the statistics never see (run-to-run identical results)
-  double* s_stats = reinterpret_cast<double*>(smem + stages * Cfg::STAGE_BYTES + BAR_BYTES);
+  // then the StatSlab of the column statistics, at stages * STAGE_BYTES + BAR_BYTES
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int M = a.M, N = a.N, K = a.K, R = a.R;
@@ -570,8 +593,6 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
       tmap_prefetch(&mBlo);
     }
   }
-  if (want_stats)
-    for (int i = threadIdx.x; i < 2 * a.stat_cols; i += NTHREADS) s_stats[i] = 0.0;
   __syncthreads();
   pdl_wait();
 
@@ -659,15 +680,22 @@ tc_gemm_nt_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
       if constexpr (MT::SPLIT) nt_output_ctx<NR, LOSS_ONLY>(sums, a, alpha, f, cx_loss);
       else nt_output_ctx<NR, LOSS_ONLY>(acc, a, alpha, f, cx_loss);
     } else {
-      if constexpr (MT::SPLIT) nt_output<NR, OUT16, VAR>(sums, a, alpha, f, s_stats);
-      else nt_output<NR, OUT16, VAR>(acc, a, alpha, f, s_stats);
+      // this tile's slab: the CTA's tiles alternate between the two
+      const uint32_t slab = tiles_u32 + stages * Cfg::STAGE_BYTES + BAR_BYTES +
+                            (((tile - blockIdx.x) / gridDim.x) & 1) * StatSlab<BN>::TILE_BYTES;
+      const uint32_t wslab = slab + (cw * 4 + wq) * StatSlab<BN>::WARP_BYTES;
+      if constexpr (MT::SPLIT) nt_output<NR, OUT16, VAR>(sums, a, alpha, f, wslab);
+      else nt_output<NR, OUT16, VAR>(acc, a, alpha, f, wslab);
+      if (want_stats) {
+        consumer_sync();
+        nt_flush_stats<BN>(a, slab, n0);
+      }
     }
   }
   if constexpr (CTX) {
     cx_loss = warp_sum_d(cx_loss);
     if (lane == 0 && cx_loss != 0.0) atomicAdd(a.cx_loss, cx_loss);
   }
-  if (want_stats) flush_stats(a, s_stats);
 }
 
 // ------------------------------------------------------------------ TN kernel ----
@@ -995,9 +1023,9 @@ int launch_nt(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& b
               const CUtensorMap& bl, NTArgs a, cudaStream_t st) {
   using Cfg = NTCfg<BN, MODE>;
   static bool attr = false;
-  a.stat_cols = a.colsum ? ((a.N + 31) / 32) * 32 : 0;
-  a.stages = pick_stages(Cfg::STAGE_BYTES, 2 * a.stat_cols * 8);
-  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, 2 * a.stat_cols * 8);
+  const int slab_bytes = a.colsum ? StatSlab<BN>::BYTES : 0;
+  a.stages = pick_stages(Cfg::STAGE_BYTES, slab_bytes);
+  const int smem = smem_bytes(a.stages, Cfg::STAGE_BYTES, slab_bytes);
   if (a.stages < 2) {
     pase_set_error("pase_tc_gemm_nt: not enough shared memory for 2 pipeline stages");
     return PASE_ERR_UNSUPPORTED;
@@ -1269,7 +1297,7 @@ int tc_gemm_nt_impl(const void* Ahi, const void* Alo, long a_rows, int R, const 
   a.alpha_dev = alpha_dev; a.bias = bias;
   a.rm = RowMap{rows_in, t_valid, rows_out, fold, N / fold, var_tab, var_n};
   a.colsum = colsum; a.colsumsq = colsumsq; a.accumulate = accumulate; a.flush_kb = flush_kb;
-  a.stages = 0; a.stat_cols = 0;
+  a.stages = 0;
   a.cx_label = nullptr; a.cx_F = a.cx_T = a.cx_r = a.cx_nvalid = 0; a.cx_scale = nullptr;
   a.cx_lo = nullptr; a.cx_loss = nullptr; a.cx_db = nullptr;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1356,7 +1384,7 @@ int pase_tc_gemm_nt_ctxmse(const void* Ahi, const void* Alo, long a_rows, int R,
   a.rm = RowMap{M, M, M, 1, (int)ldr, nullptr, 0};
   a.colsum = nullptr; a.colsumsq = nullptr; a.accumulate = 0;
   a.flush_kb = K > 512 ? 2 : 0;
-  a.stages = 0; a.stat_cols = 0;
+  a.stages = 0;
   a.cx_label = label; a.cx_F = F; a.cx_T = T; a.cx_r = r; a.cx_nvalid = N; a.cx_scale = scale;
   a.cx_lo = Rlo; a.cx_loss = loss_acc; a.cx_db = db_acc;
   if (loss_only) return launch_nt<128, 3, false, true, false, true>(ah, al, bh, bl, a, (cudaStream_t)stream);
