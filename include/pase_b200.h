@@ -331,15 +331,11 @@ int pase_out_affine_nct(const float* y, const float* scale, const float* shift,
  * sum in a fixed order. */
 int pase_out_affine_var(const float* y, const float* scale, const float* shift, float* out,
                         const int* tab, int nseg, int C, int mode, void* stream);
-/* Windowed output of one long recording (WaveFe.extract_long): rows 0..T-1 of y (T,C) as
- * y*scale+shift (one fmaf, as pase_out_affine_nct) into columns col0 .. col0+T-1 of out (C,ldo),
- * leading dimension ldo.  64-bit offsets: the output may exceed 2^31 elements. */
-int pase_out_place(const float* y, const float* scale, const float* shift, float* out, long ldo,
-                   long col0, int T, int C, void* stream);
-/* pase_out_place for many streams' crops at once (StreamPool): tab (DEVICE, nseg rows of 5
- * ints) {row0, T, ocol, ldo, col0}: rows row0 .. row0+T-1 of y (rows,C) as y*scale+shift (the
- * same fmaf) into columns col0 .. col0+T-1 of the (C, ldo) block starting at element ocol*C of
- * out.  max_T >= every row's T.  64-bit element offsets. */
+/* Windowed output of many streams' crops at once (StreamPool, so FeatureStream and
+ * WaveFe.extract_long): tab (DEVICE, nseg rows of 5 ints) {row0, T, ocol, ldo, col0}: rows row0
+ * .. row0+T-1 of y (rows,C) as y*scale+shift (one fmaf, as pase_out_affine_nct) into columns
+ * col0 .. col0+T-1 of the (C, ldo) block starting at element ocol*C of out.  max_T >= every
+ * row's T.  64-bit element offsets: the output may exceed 2^31 elements. */
 int pase_out_place_var(const float* y, const float* scale, const float* shift, float* out,
                        const int* tab, int nseg, int max_T, int C, void* stream);
 /* select_output (pase/models/modules.py:62-74) in place over a whole (C,T) output whose rows
@@ -369,17 +365,12 @@ int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst,
  * (pase_qrnn_scan_plan), so its result is that of a B=1 scan.  Two launches. */
 int pase_qrnn_scan_fwd_var(const float* Y, float* h, long ldh, float* Cst, const int* tab,
                            int nseg, int H, void* stream);
-/* One recording's sequential scan continued over rows 0..T-1 of Y / h / Cst (B=1): the cell
- * state enters from c_in[H] (NULL: zero) and the state after row T-1 is written to c_out[H]
- * (c_out may equal c_in).  The per-step arithmetic is the sequential kernel's, so scanning a
- * recording piece by piece reproduces pase_qrnn_scan_fwd's bits for T' > 512. */
-int pase_qrnn_scan_fwd_carry(const float* Y, float* h, long ldh, float* Cst, const float* c_in,
-                             float* c_out, int T, int H, void* stream);
-/* pase_qrnn_scan_fwd_carry for many streams at once (StreamPool): tab (DEVICE, nseg rows of 4
- * ints) {row0, T, slot, first}: rows row0 .. row0+T-1 of Y / h / Cst continue the scan of the
- * stream whose state is row `slot` of state (max_streams, H), zero when first != 0; the state
- * after the last row is written back there.  A slot appears at most once per call.  Same
- * per-step body, so the same bits as pase_qrnn_scan_fwd_carry. */
+/* Sequential scans continued over windows of many streams at once (StreamPool, so FeatureStream
+ * and WaveFe.extract_long): tab (DEVICE, nseg rows of 4 ints) {row0, T, slot, first}: rows row0
+ * .. row0+T-1 of Y / h / Cst continue the scan of the stream whose state is row `slot` of state
+ * (max_streams, H), zero when first != 0; the state after the last row is written back there.
+ * A slot appears at most once per call.  The per-step arithmetic is the sequential kernel's, so
+ * scanning a recording piece by piece reproduces pase_qrnn_scan_fwd's bits for T' > 512. */
 int pase_qrnn_scan_fwd_carry_var(const float* Y, float* h, long ldh, float* Cst, float* state,
                                  const int* tab, int nseg, int H, void* stream);
 int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long lddh,

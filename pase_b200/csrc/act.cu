@@ -777,28 +777,10 @@ out_affine_var_kernel(const float* __restrict__ y, const float* __restrict__ sca
   }
 }
 
-// Windowed output (WaveFe.extract_long): rows 0..T-1 of y, as h = y*scale+shift (the fmaf of
-// out_affine_nct_kernel), into columns col0 .. col0+T-1 of the (C, ldo) output.  32x32 tiles.
-__global__ void out_place_kernel(const float* __restrict__ y, const float* __restrict__ scale,
-                                 const float* __restrict__ shift, float* __restrict__ out,
-                                 long ldo, long col0, int T, int C) {
-  pdl_wait();
-  __shared__ float tile[32][33];
-  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int t = t0 + i, c = c0 + threadIdx.x;
-    if (t < T && c < C) tile[i][threadIdx.x] = fmaf(y[(long)t * C + c], scale[c], shift[c]);
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int c = c0 + i, t = t0 + threadIdx.x;
-    if (t < T && c < C) out[(long)c * ldo + col0 + t] = tile[threadIdx.x][i];
-  }
-}
-
-// out_place_kernel for many streams' crops at once (StreamPool): segment blockIdx.z's row
-// {row0, T, ocol, ldo, col0} writes rows row0 .. row0+T-1 of y into columns col0 .. col0+T-1 of
-// the (C, ldo) block that starts at element ocol*C of out.  Same fmaf, same 32x32 tiles.
+// Windowed output (StreamPool, so FeatureStream and WaveFe.extract_long): segment blockIdx.z's
+// row {row0, T, ocol, ldo, col0} writes rows row0 .. row0+T-1 of y, as h = y*scale+shift (the
+// fmaf of out_affine_nct_kernel), into columns col0 .. col0+T-1 of the (C, ldo) block that
+// starts at element ocol*C of out.  32x32 tiles.
 __global__ void out_place_var_kernel(const float* __restrict__ y, const float* __restrict__ scale,
                                      const float* __restrict__ shift, float* __restrict__ out,
                                      const int* __restrict__ tab, int C) {
@@ -1508,17 +1490,6 @@ int pase_out_affine_var(const float* y, const float* scale, const float* shift, 
   PASE_LAUNCH((out_affine_var_kernel), dim3((C + 31) / 32, nseg), dim3(32, 8), 0,
               (cudaStream_t)stream, y, scale, shift, out, tab, C, mode);
   PASE_LAUNCH_CHECK("pase_out_affine_var");
-  return PASE_OK;
-}
-
-int pase_out_place(const float* y, const float* scale, const float* shift, float* out, long ldo,
-                   long col0, int T, int C, void* stream) {
-  PASE_CHECK_ARG(y && scale && shift && out && T > 0 && C > 0, "pase_out_place: bad args");
-  PASE_CHECK_ARG(col0 >= 0 && col0 + T <= ldo, "pase_out_place: columns %ld..%ld past ldo=%ld",
-                 col0, col0 + T, ldo);
-  PASE_LAUNCH((out_place_kernel), dim3((T + 31) / 32, (C + 31) / 32), dim3(32, 8), 0,
-              (cudaStream_t)stream, y, scale, shift, out, ldo, col0, T, C);
-  PASE_LAUNCH_CHECK("pase_out_place");
   return PASE_OK;
 }
 

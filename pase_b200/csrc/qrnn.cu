@@ -15,7 +15,7 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-
 // cprev is the cell state before it (0 at the start of an utterance).  Returns the state after
 // the last step.  Every step runs the same arithmetic whether it falls in an unrolled group or
 // in the remainder, so a scan cut into pieces that carry the state reproduces the whole scan's
-// bits (pase_qrnn_scan_fwd_carry).
+// bits (pase_qrnn_scan_fwd_carry_var).
 __device__ __forceinline__ float qrnn_fwd_seq(const float* __restrict__ y, float* __restrict__ hp,
                                               long ldh, float* __restrict__ cp, int T, int H,
                                               float cprev) {
@@ -54,19 +54,6 @@ qrnn_scan_fwd_kernel(const float* __restrict__ Y, float* __restrict__ h, long ld
   if (c >= H) return;
   qrnn_fwd_seq(Y + (long)n * T * 3 * H + c, h + (long)n * T * ldh + c, ldh,
                Cst + (long)n * T * H + c, T, H, 0.f);
-}
-
-// One recording's scan continued over T more rows: the state enters from c_in (nullptr: 0) and
-// leaves through c_out (may alias c_in: each thread reads its entry before writing it).
-__global__ void __launch_bounds__(128)
-qrnn_scan_fwd_carry_kernel(const float* __restrict__ Y, float* __restrict__ h, long ldh,
-                           float* __restrict__ Cst, const float* c_in, float* c_out, int T,
-                           int H) {
-  pdl_wait();
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= H) return;
-  const float c0 = c_in ? c_in[c] : 0.f;
-  c_out[c] = qrnn_fwd_seq(Y + c, h + c, ldh, Cst + c, T, H, c0);
 }
 
 // Many streams' scans continued at once (StreamPool): segment blockIdx.y's row {row0, T, slot,
@@ -350,17 +337,6 @@ int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst, int N, in
   dim3 grid((H + 127) / 128, N);
   PASE_LAUNCH((qrnn_scan_fwd_kernel), grid, 128, 0, (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
   PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd");
-  return PASE_OK;
-}
-
-int pase_qrnn_scan_fwd_carry(const float* Y, float* h, long ldh, float* Cst, const float* c_in,
-                             float* c_out, int T, int H, void* stream) {
-  PASE_CHECK_ARG(Y && h && Cst && c_out, "pase_qrnn_scan_fwd_carry: null pointer");
-  PASE_CHECK_ARG(T > 0 && H > 0 && ldh >= H, "pase_qrnn_scan_fwd_carry: T=%d H=%d ldh=%ld", T,
-                 H, ldh);
-  PASE_LAUNCH((qrnn_scan_fwd_carry_kernel), dim3((H + 127) / 128), 128, 0, (cudaStream_t)stream,
-              Y, h, ldh, Cst, c_in, c_out, T, H);
-  PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd_carry");
   return PASE_OK;
 }
 

@@ -908,8 +908,10 @@ def check_windowable(cfg, L):
 
 
 def window_capacity(cfg, window):
-    """Samples of the longest segment plan_windows / a FeatureStream builds for `window`:
-    window + both halos + one hop + the tail extension, whatever the recording's length."""
+    """Samples of the longest segment stream_step builds for pieces of stream_chunk(window)
+    samples (plan_windows, a StreamPool with that window): window + both halos + one hop + the
+    tail extension, whatever the recording's length.  The plan of a FeatureStream and of
+    extract_long holds this many samples."""
     hl, hr = window_halos(cfg)
     hop = hop_size(cfg)
     return hop * (window // hop + hl + hr + 1) + tail_length(cfg)
@@ -1011,43 +1013,23 @@ def stream_ring_capacity(cfg, window):
 
 
 def plan_windows(cfg, L, window):
-    """Segments of a recording of L samples for windows of `window` samples' frames: a list of
-    dict(seg_start, seg_len, crop_f0, crop_n) whose crops tile the recording's frames 0 .. T'-1
-    once, in order (crop_f0: first frame of the crop within the segment).  Host only; raises
-    ValueError for a bad window / a too-short recording and NotImplementedError when a segment
-    could not reproduce the whole-recording frames."""
-    hop = hop_size(cfg)
+    """Segments of a recording of L samples for windows of `window` samples' frames, as
+    WaveFe.extract_long runs them: stream_step over pieces of stream_chunk samples, the last one
+    at the end of the recording.  A list of dict(seg_start, seg_len, crop_f0, crop_n) whose
+    crops tile the recording's frames 0 .. T'-1 once, in order (crop_f0: first frame of the crop
+    within the segment).  Host only; raises ValueError for a bad window / a too-short recording
+    and NotImplementedError when a segment could not reproduce the whole-recording frames."""
     if window < min_window(cfg):
         raise ValueError("window must be at least %d samples (%d frames), got %d"
                          % (min_window(cfg), MIN_WINDOW_FRAMES, window))
-    T = build_geometry(cfg, L)[-1].T_out
-    check_windowable(cfg, L)
-    nw, hr = window // hop, window_halos(cfg)[1]
-    segs = []
-    for f0 in range(0, T, nw):
-        f1 = min(f0 + nw, T)
-        end = L if f1 == T else min(L, (f1 + hr) * hop)
-        seg = make_segment(cfg, f0, f1, end)
-        check_segment(cfg, seg, end == L)
-        segs.append(seg)
+    chunk = stream_chunk(cfg, window)
+    pieces = [min(chunk, L - a) for a in range(0, L, chunk)] or [0]
+    segs, n, done, keep = [], 0, 0, 0
+    for k, add in enumerate(pieces):
+        n, done, keep, seg = stream_step(cfg, n, done, keep, add, k + 1 == len(pieces))
+        if seg is not None:
+            segs.append(seg)
     return segs
-
-
-def encoder_forward_window(plan, mod, x, seg, geoms, params, carry, out, ldo, col0):
-    """One segment of a long recording (x: its seg_len samples, fp32): the packed front end as
-    a one-utterance pack, the QRNN scan over the crop's frames only, continuing from the state in
-    `carry` (H floats, updated), the output projection, and the crop's frames as y*scale+shift
-    into columns col0 .. of the (emb, ldo) tensor `out`."""
-    sz, _ = _packed_front(plan, mod, x, [seg["seg_len"]], [geoms], params, None)
-    f0, n = seg["crop_f0"], seg["crop_n"]
-    if plan.rnn:
-        H, Kc = plan.H, plan.Kc
-        ops.call("pase_qrnn_scan_fwd_carry", plan.Yg[f0 * 3 * H:], plan.cat[f0 * Kc:], Kc,
-                 plan.Cst[f0 * H:], carry, carry, n, H)
-    _packed_out_proj(plan, mod, params, sz["rows"])
-    bo = plan.bn_out
-    ops.call("pase_out_place", plan.yout[f0 * plan.emb:], bo[2], bo[3], out, ldo, col0, n,
-             plan.emb)
 
 
 def encoder_backward(plan, mod, params, gout, gntc, training, sink=None):

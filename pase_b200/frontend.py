@@ -159,7 +159,7 @@ class WaveFe(Model):
             self.norm_out = nn.BatchNorm1d(emb, affine=False)
         self._plans = OrderedDict()
         self._packed_plans = OrderedDict()
-        self._stagers, self._carries = {}, {}
+        self._long_pool = None          # (key, StreamPool) of extract_long
         # GEMM numerics (gemm.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (wgmma,
         # fp32-equivalent), "tf32" (wgmma), "bf16" (wgmma, bf16 operands and activations)
         self.precision = os.environ.get("PASE_B200_PRECISION", DEFAULT_PRECISION)
@@ -260,14 +260,7 @@ class WaveFe(Model):
         equal to ``self(wavs[i].view(1,1,-1), mode=mode)`` (mode as select_output); they are
         views of one buffer per forward.  Eval mode only: train-mode BatchNorm would couple
         the utterances."""
-        if self.training:
-            raise RuntimeError("WaveFe.extract runs the encoder in eval mode; call .eval() first "
-                               "(train-mode BatchNorm statistics would mix the utterances)")
-        device = self.W.weight.device
-        if device.type != "cuda":
-            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; the module lives "
-                               "on %s. There is no CPU path." % device)
-        return self._extract(wavs, mode, max_samples, device)
+        return self._extract(wavs, mode, max_samples, self._eval_device("extract"))
 
     def _extract(self, wavs, mode, max_samples, device):
         if mode not in _enc.OUT_MODES:
@@ -277,13 +270,10 @@ class WaveFe(Model):
             raise ValueError("max_samples must be positive, got %r" % (max_samples,))
         flat = []
         for i, w in enumerate(wavs):
-            if not isinstance(w, torch.Tensor) or w.dtype != torch.float32:
-                raise TypeError("utterance %d: expected an fp32 tensor, got %s"
-                                % (i, getattr(w, "dtype", type(w))))
-            if w.dim() == 0 or w.dim() > 3 or any(d != 1 for d in w.shape[:-1]):
-                raise ValueError("utterance %d: expected (T,), (1,T) or (1,1,T), got %s"
-                                 % (i, tuple(w.shape)))
-            flat.append(w.reshape(-1))
+            try:
+                flat.append(_recording(w))
+            except (TypeError, ValueError) as e:
+                raise type(e)("utterance %d: %s" % (i, e)) from None
         if not flat:
             return []
         lengths = [w.numel() for w in flat]
@@ -320,9 +310,10 @@ class WaveFe(Model):
         T') CUDA tensor equal to ``self(wav.view(1,1,-1), mode=mode)``.  The recording is cut
         into segments whose crops hold `window` samples' frames (default EXTRACT_LONG_WINDOW,
         at least encoder.min_window), each with halos covering the receptive field, and the
-        QRNN state is carried from one to the next (DESIGN.md section 15).  A recording of at
+        QRNN state is carried from one to the next (DESIGN.md section 15): the recording runs
+        as one push of a one-stream StreamPool, finished in the same call.  A recording of at
         most `window` samples runs as one forward of `extract`.  wav: fp32 (T,), (1,T) or
-        (1,1,T) on the CPU (staged segment by segment through pinned memory) or the GPU.
+        (1,1,T) on the CPU (staged piece by piece through pinned memory) or the GPU.
         Eval mode only."""
         return self._extract_long(wav, mode, window, self._eval_device("extract_long"))
 
@@ -337,32 +328,25 @@ class WaveFe(Model):
                              % (_enc.min_window(cfg), win))
         if L <= win:
             return self._extract([x], mode, win, device)[0]
-        segs = _enc.plan_windows(cfg, L, win)            # every check before the first launch
-        T = _enc.frame_counts(cfg, L)[-1]
-        emb = self.emb_dim
-        E = emb * (2 if mode in ("avg_concat", "avg_norm_concat") else 1)
-        plan = self._packed_plan(_enc.window_capacity(cfg, win), device)
-        fold = plan.precision.sinc_fold
-        stage = None
-        if device.type == "cuda" and not x.is_cuda:
-            stage = self._stager(plan.capacity)
-        elif x.device != device:
+        if x.is_cuda and x.device != device:
             x = x.to(device)
-        self._sinc_consts(device)
-        params = dict(self.named_parameters())
+        T, emb = _enc.frame_counts(cfg, L)[-1], self.emb_dim
+        E = emb * (2 if mode in ("avg_concat", "avg_norm_concat") else 1)
+        # one cached one-stream pool (its ring and staging) per (window, device, precision)
+        key = (win, str(device), self.resolved_precision())
+        if self._long_pool is None or self._long_pool[0] != key:
+            self._long_pool = None
+            self._long_pool = (key, StreamPool(self, device, 1, win,
+                                               _enc.window_capacity(cfg, win)))
+        pool = self._long_pool[1]
         out = torch.empty(E, T, dtype=torch.float32, device=device)
-        carry = self._carry(plan, device)
-        col = 0
-        with torch.no_grad():
-            for seg in segs:
-                s, n = seg["seg_start"], seg["seg_len"]
-                xs = x[s:s + n] if stage is None else stage.put(x[s:s + n], plan.wave)
-                _enc.encoder_forward_window(plan, self, xs, seg,
-                                            _enc.build_geometry(cfg, n, fold), params, carry,
-                                            out, T, col)
-                col += seg["crop_n"]
-            if mode is not None:
-                _ops.call("pase_out_select", out, T, emb, _enc.OUT_MODES[mode])
+        sid = pool.open()
+        try:                        # the whole recording as one push: plan_windows' segments
+            pool._push({sid: x}, [sid], out)
+        finally:
+            pool._release(sid)      # a no-op once the push has finished the stream
+        if mode is not None:
+            _ops.call("pase_out_select", out, T, emb, _enc.OUT_MODES[mode])
         return out.view(1, E, T)
 
     def stream(self, mode=None, window=None):
@@ -385,22 +369,6 @@ class WaveFe(Model):
             raise ValueError("a FeatureStream returns mode None features only; select_output "
                              "modes need the whole recording (use extract_long)")
         return StreamPool(self, device, max_streams, window, max_samples)
-
-    def _stager(self, n):
-        st = self._stagers.get(n)
-        if st is None:
-            st = self._stagers[n] = _PinnedStager(n)
-        return st
-
-    def _carry(self, plan, device):
-        """Zeroed QRNN state of a windowed forward (one buffer per device, reused)."""
-        if not plan.rnn:
-            return None
-        c = self._carries.get(str(device))
-        if c is None or c.numel() != plan.H:
-            c = self._carries[str(device)] = torch.zeros(plan.H, dtype=torch.float32,
-                                                         device=device)
-        return c.zero_()
 
     def forward(self, batch, device=None, mode=None):
         if device is None:
@@ -428,28 +396,6 @@ def _recording(w):
     return w.reshape(-1).contiguous()
 
 
-class _PinnedStager(object):
-    """Two pinned host buffers of n floats: a CPU segment is copied into one while the device
-    may still be reading the other, then sent to the device asynchronously."""
-
-    def __init__(self, n):
-        self.bufs = [torch.empty(n, dtype=torch.float32).pin_memory() for _ in range(2)]
-        self.events = [None, None]
-        self.i = 0
-
-    def put(self, src, dst):
-        i, self.i = self.i, self.i ^ 1
-        if self.events[i] is not None:
-            self.events[i].synchronize()          # its last copy to the device has finished
-        n = src.numel()
-        self.bufs[i][:n].copy_(src)
-        d = dst[:n]
-        d.copy_(self.bufs[i][:n], non_blocking=True)
-        self.events[i] = torch.cuda.Event()
-        self.events[i].record()
-        return d
-
-
 class FeatureStream(object):
     """Online feature extraction of one recording (WaveFe.stream()).  push(samples) returns the
     (1, emb, n) frames that became final (n may be 0): frame j is final once sample
@@ -457,79 +403,33 @@ class FeatureStream(object):
     encoder.tail_length samples have.  finish() returns the rest, the end of the recording
     reflect-padded as a whole-recording forward pads it.  The frames concatenate to
     ``WaveFe.extract_long`` of the whole recording (bit-equal when it has more than 512
-    frames, where both run the sequential QRNN scan).  Between calls the stream holds only the
-    samples its next segment reads again (halo and tail), the QRNN state and frame counters."""
+    frames, where both run the sequential QRNN scan).  A stream is one open id of a private
+    one-stream StreamPool whose plan holds the longest segment of its window
+    (encoder.window_capacity): between calls the device holds the samples a later segment reads
+    again and the QRNN state, the host four counters."""
 
     def __init__(self, model, device, window=None):
-        cfg = model.cfg
-        win = _enc.min_window(cfg) if window is None else int(window)
-        if win < _enc.min_window(cfg):
-            raise ValueError("window must be at least %d samples, got %d"
-                             % (_enc.min_window(cfg), win))
-        self.model, self.device, self.cfg = model, device, cfg
-        self.chunk = _enc.stream_chunk(cfg, win)
-        self.min_len = _enc.min_length(cfg)
-        self.plan = model._packed_plan(_enc.window_capacity(cfg, win), device)
-        self.carry = (torch.zeros(self.plan.H, dtype=torch.float32, device=device)
-                      if self.plan.rnn else None)
-        self.buf = None            # samples buf0 .. n-1 (the ones a later segment reads)
-        self.buf0 = 0
-        self.n = 0                 # samples received
-        self.done = 0              # frames returned
+        win = _enc.min_window(model.cfg) if window is None else int(window)
+        self._pool = StreamPool(model, device, 1, win, _enc.window_capacity(model.cfg, win))
+        self._id = self._pool.open()
         self.finished = False
 
     def push(self, samples):
         if self.finished:
             raise RuntimeError("FeatureStream.push after finish()")
-        x = _recording(samples)
-        outs = []
-        for a in range(0, x.numel(), self.chunk):
-            piece = x[a:a + self.chunk]
-            self.buf = piece.clone() if self.buf is None else torch.cat([self.buf,
-                                                                         piece.to(self.buf)])
-            self.n, f1, keep, seg = _enc.stream_step(self.cfg, self.n, self.done, self.buf0,
-                                                     piece.numel())
-            if seg is not None:
-                outs.append(self._run(seg, f1, keep))
-        if not outs:
-            return torch.empty(1, self.model.emb_dim, 0, dtype=torch.float32, device=self.device)
-        return outs[0] if len(outs) == 1 else torch.cat(outs, 2)
+        return self._pool.push({self._id: samples})[self._id]
 
     def finish(self):
         if self.finished:
             raise RuntimeError("FeatureStream.finish called twice")
-        _, f1, keep, seg = _enc.stream_step(self.cfg, self.n, self.done, self.buf0, 0, True)
+        out = self._pool.push({}, finish=[self._id])[self._id]
         self.finished = True
-        if seg is not None:
-            return self._run(seg, f1, keep)
-        return torch.empty(1, self.model.emb_dim, 0, dtype=torch.float32, device=self.device)
-
-    def _run(self, seg, f1, keep):
-        cfg, plan, m = self.cfg, self.plan, self.model
-        s, n = seg["seg_start"], seg["seg_len"]
-        assert s >= self.buf0 and n <= plan.capacity
-        x = plan.wave[:n]
-        x.copy_(self.buf[s - self.buf0:s - self.buf0 + n])
-        out = torch.empty(m.emb_dim, f1 - self.done, dtype=torch.float32, device=self.device)
-        m._sinc_consts(self.device)
-        with torch.no_grad():
-            _enc.encoder_forward_window(
-                plan, m, x, seg, _enc.build_geometry(cfg, n, plan.precision.sinc_fold),
-                dict(m.named_parameters()), self.carry, out, f1 - self.done, 0)
-        self.done = f1
-        if keep > self.buf0:                    # what the next segment can read (stream_step)
-            self.buf = self.buf[keep - self.buf0:].clone()
-            self.buf0 = keep
-        return out.view(1, m.emb_dim, -1)
-
-
-# table row widths of the pool's kernels (include/pase_b200.h)
-_GATHER_W, _CARRY_W, _PLACE_W = 8, 4, 5
+        return out
 
 
 class _PoolStream(object):
-    """Host counters of one pooled stream (those of FeatureStream): its ring slot, samples
-    received, frames returned and the first sample it still holds."""
+    """Host counters of one pooled stream: its ring slot, samples received, frames returned and
+    the first sample it still holds."""
     __slots__ = ("slot", "n", "done", "keep")
 
     def __init__(self, slot):
@@ -540,14 +440,16 @@ class StreamPool(object):
     """Online feature extraction of many live recordings at once (WaveFe.streams()).
 
     open() returns a stream id; push({id: samples, ...}, finish=(ids...)) returns {id: (1, emb,
-    n) frames} for every id named, n >= 0.  Each stream's frames are exactly those of a
-    FeatureStream fed the same blocks (and finish()ed where named): every stream is planned by
-    the same host planner (encoder.stream_step) and cut into the same pieces.  Round r of a call
-    runs the r-th piece of every stream that has one (then each finishing stream's last
-    segment) as packs of at most max_samples samples; a pack is one packed forward whose
-    launches do not depend on how many streams it holds (DESIGN.md section 16).  Between calls
-    the device holds each stream's recent samples in a ring of an arena and its QRNN state in a
-    (max_streams, H) table; the host holds four counters per stream."""
+    n) frames} for every id named, n >= 0.  Every stream is planned by the host planner
+    encoder.stream_step, one piece of at most stream_chunk samples at a time; a stream that
+    finishes in the call that brings its last piece plans that piece as its end.  Round r of a
+    call runs the r-th piece of every stream that has one (or the last segment of a stream that
+    finishes with no samples) as packs of at most max_samples samples; a pack is one packed
+    forward whose launches do not depend on how many streams it holds (DESIGN.md section 16).
+    This is the one windowed engine: a FeatureStream is a one-stream pool, and extract_long one
+    push of a whole recording into one.  Between calls the device holds each stream's recent
+    samples in a ring of an arena and its QRNN state in a (max_streams, H) table; the host holds
+    four counters per stream."""
 
     def __init__(self, model, device, max_streams, window=None, max_samples=None):
         cfg = model.cfg
@@ -563,7 +465,9 @@ class StreamPool(object):
         self.model, self.device, self.cfg = model, device, cfg
         self.max_streams, self.max_samples = int(max_streams), cap
         self.chunk = _enc.stream_chunk(cfg, win)
-        self.plan = model._packed_plan(max(cap, _enc.window_capacity(cfg, win)), device)
+        self.seg_cap = _enc.window_capacity(cfg, win)         # the longest segment
+        self.capacity = max(cap, self.seg_cap)
+        self.plan = model._packed_plan(self.capacity, device)
         self.ring_cap = _enc.stream_ring_capacity(cfg, win)
         self.ring = torch.zeros(self.max_streams * self.ring_cap, dtype=torch.float32,
                                 device=device)
@@ -571,7 +475,7 @@ class StreamPool(object):
                                   device=device) if self.plan.rnn else None)
         self._free = list(range(self.max_streams - 1, -1, -1))
         self._streams, self._next_id = {}, 0
-        # two host staging slots (samples, table, event), as _PinnedStager; device copies
+        # two host staging slots (samples, table, event) and their device copies
         self._pin = device.type == "cuda"
         self._host = [[None, None, None], [None, None, None]]
         self._hi = 0
@@ -590,11 +494,22 @@ class StreamPool(object):
     def __len__(self):
         return len(self._streams)
 
+    def _release(self, sid):
+        """Close stream sid (if open) and free its slot."""
+        st = self._streams.pop(sid, None)
+        if st is not None:
+            self._free.append(st.slot)
+
     def push(self, blocks, finish=()):
         """blocks: {id: fp32 (T,), (1,T) or (1,1,T) samples on the CPU or the pool's GPU};
         finish: ids whose recording ends after this call's samples.  -> {id: (1, emb, n)} for
         every id in either, views of one buffer.  Every argument is checked, and every segment
         planned, before the first launch: a call that raises changes no stream."""
+        return self._push(blocks, finish, None)
+
+    def _push(self, blocks, finish, out):
+        """push(), writing the frames into `out` (None: a new buffer) as consecutive (emb, n)
+        blocks, one per id in the order of blocks then finish."""
         m, emb = self.model, self.model.emb_dim
         if m.training:
             raise RuntimeError("WaveFe.streams runs the encoder in eval mode; call .eval() first")
@@ -620,11 +535,15 @@ class StreamPool(object):
                 raise ValueError("stream %r: samples on %s, the pool runs on %s"
                                  % (i, x.device, self.device))
             xs[i] = x
-        steps, new, closing = self._plan(ids, xs, set(fin))
+        steps, new = self._plan(ids, xs, set(fin))
+        # the plan of the model's LRU, not one this pool pinned when the LRU has moved on
+        self.plan = m._packed_plan(self.capacity, self.device)
 
         col, views, ocol = 0, {}, {}
         total = sum(new[i][1] - self._streams[i].done for i in ids)
-        out = torch.empty(emb * total, dtype=torch.float32, device=self.device)
+        if out is None:
+            out = torch.empty(emb * total, dtype=torch.float32, device=self.device)
+        out = out.view(-1)
         for i in ids:
             nf = new[i][1] - self._streams[i].done
             views[i] = out[col * emb:(col + nf) * emb].view(1, emb, nf)
@@ -638,42 +557,42 @@ class StreamPool(object):
                 entries = [(i, steps[i][r]) for i in ids if r < len(steps[i])]
                 self._round(entries, out, ocol, new, params)
         for i in ids:                                  # commit
-            st = self._streams[i]
-            st.n, st.done, st.keep = new[i]
-            if i in closing:
-                del self._streams[i]
-                self._free.append(st.slot)
+            self._streams[i].n, self._streams[i].done, self._streams[i].keep = new[i]
+        for i in fin:
+            self._release(i)
         return views
 
     def _plan(self, ids, xs, fin):
         """Every stream's steps of this call on the host, through encoder.stream_step: per id a
-        list of (piece or None, n before it, done before it, keep before it, segment or None),
-        its counters after the call, and the ids that finish.  Raises before any launch."""
+        list of (piece or None, n before it, done before it, keep before it, segment or None)
+        and its counters after the call.  A finishing stream's last piece is planned at_end (a
+        finish with no samples is a step of its own).  Raises before any launch."""
         cfg, steps, new = self.cfg, {}, {}
         for i in ids:
             st = self._streams[i]
             n, done, keep = st.n, st.done, st.keep
-            out = []
             x = xs.get(i)
             L = 0 if x is None else x.numel()
-            for a in range(0, L, self.chunk):
-                piece = x[a:a + self.chunk]
-                n1, d1, k1, seg = _enc.stream_step(cfg, n, done, keep, piece.numel())
-                if n1 - keep > self.ring_cap or (seg is not None and seg["seg_start"] < keep):
-                    raise RuntimeError("StreamPool: stream %r would read samples %d .. %d from a "
-                                       "ring of %d" % (i, keep, n1, self.ring_cap))
-                out.append((piece, n, done, keep, seg))
-                n, done, keep = n1, d1, k1
-            if i in fin:
+            pieces = [x[a:a + self.chunk] for a in range(0, L, self.chunk)]
+            if i in fin and not pieces:
+                pieces = [None]
+            out = []
+            for k, piece in enumerate(pieces):
+                end = i in fin and k + 1 == len(pieces)
                 try:
-                    _, d1, k1, seg = _enc.stream_step(cfg, n, done, keep, 0, True)
+                    n1, d1, k1, seg = _enc.stream_step(cfg, n, done, keep,
+                                                       0 if piece is None else piece.numel(), end)
                 except (ValueError, NotImplementedError) as e:
                     raise type(e)("stream %r: %s" % (i, e)) from None
-                if seg is not None:
-                    out.append((None, n, done, keep, seg))
-                done, keep = d1, k1
+                if n1 - keep > self.ring_cap or (seg is not None and (
+                        seg["seg_start"] < keep or seg["seg_len"] > self.seg_cap)):
+                    raise RuntimeError("StreamPool: stream %r would read samples %d .. %d from a "
+                                       "ring of %d" % (i, keep, n1, self.ring_cap))
+                if piece is not None or seg is not None:
+                    out.append((piece, n, done, keep, seg))
+                n, done, keep = n1, d1, k1
             steps[i], new[i] = out, (n, done, keep)
-        return steps, new, fin
+        return steps, new
 
     def _round(self, entries, out, ocol, new, params):
         """One round: stage the new samples, upload one table for every pack, then per pack the

@@ -1,5 +1,5 @@
 """Host side of WaveFe.extract_long / FeatureStream (windowed inference of one long recording)
-on CPU, every kernel launch replaced by its torch emulation (tests/emul_long.py): the window
+on CPU, every kernel launch replaced by its torch emulation (tests/emul_streams.py): the window
 planner, the halos it derives against the float64 oracle, the windowed forward against the
 B=1 forward, the stream against extract_long, and argument errors raised before any launch."""
 import random
@@ -8,7 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import emul_long
+import emul_streams
 import pase_oracle as O
 from helpers import resolve_cfg, fill_state_dict, seeded_randn, assert_close
 import pase_b200.ops as ops
@@ -21,7 +21,7 @@ CPU = torch.device("cpu")
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_long.call)
+    monkeypatch.setattr(ops, "call", emul_streams.call)
     yield
 
 
@@ -62,7 +62,7 @@ def _check_plan(cfg, L, window):
 
 
 @pytest.mark.parametrize("cfg_name", CFGS)
-def test_planner_tiles_the_frames(cfg_name):
+def test_stream_planner_tiles_the_frames(cfg_name):
     cfg = WaveFe(**resolve_cfg(cfg_name)).cfg
     hop, w = enc.hop_size(cfg), enc.min_window(cfg)
     assert hop == 160 and w == 81920
@@ -72,8 +72,8 @@ def test_planner_tiles_the_frames(cfg_name):
         for L in (w + 1 * hop + r, 3 * w + 977 * hop + r, 7 * w + r):
             _check_plan(cfg, L, w)
         _check_plan(cfg, 5 * w + 300 * hop + r, 2 * w + 3 * hop)
-    segs = _check_plan(cfg, w + hop, w)                    # T' = 513: a 1-frame last crop
-    assert segs[-1]["crop_n"] == 1
+    segs = _check_plan(cfg, w + hop, w)                    # T' = 513: a short last crop
+    assert segs[-1]["crop_n"] == 513 - enc.final_frames(cfg, w)
     segs = _check_plan(cfg, 2 * w + 160 * 20 + 5, w)        # a short tail, extended left
     assert segs[-1]["seg_len"] >= enc.tail_length(cfg)
     with pytest.raises(ValueError, match="window"):
@@ -130,7 +130,7 @@ def test_derived_halos_against_oracle():
 
 
 @pytest.mark.parametrize("cfg_name", CFGS)
-def test_extract_long_matches_single(cfg_name, emulated):
+def test_pooled_extract_long_matches_single(cfg_name, emulated):
     model = make_model(cfg_name)
     w = enc.min_window(model.cfg)
     x = seeded_randn((w + 160 * 30 + 77,), 21, 0.5)
@@ -145,7 +145,7 @@ def test_extract_long_matches_single(cfg_name, emulated):
         assert float((g - ref).abs().max()) <= 1e-6 * float(y.abs().max()), mode
 
 
-def test_stream_matches_extract_long(emulated):
+def test_pooled_stream_matches_extract_long(emulated):
     model = make_model("cfg/frontend/PASE+.cfg")
     cfg = model.cfg
     w = enc.min_window(cfg)
@@ -169,7 +169,7 @@ def test_stream_matches_extract_long(emulated):
             st.push(x[:10])
 
 
-def test_argument_errors(emulated, monkeypatch):
+def test_argument_errors_before_any_segment(emulated, monkeypatch):
     model = make_model("cfg/frontend/PASE+.cfg", "3xf16")
     w = enc.min_window(model.cfg)
     calls = []
@@ -190,6 +190,8 @@ def test_argument_errors(emulated, monkeypatch):
         model.stream()
     st = FeatureStream(model, CPU, w)
     assert st.push(torch.zeros(300)).shape == (1, model.emb_dim, 0)
+    assert calls == ["pase_stream_gather"]                # the samples go to the stream's ring
+    del calls[:]
     with pytest.raises(ValueError, match="shorter"):
         st.finish()
     with pytest.raises(ValueError, match="window"):
@@ -199,4 +201,6 @@ def test_argument_errors(emulated, monkeypatch):
         model.extract_long(torch.zeros(3 * w))
     with pytest.raises(RuntimeError, match="eval"):
         model.stream()
+    with pytest.raises(RuntimeError, match="eval"):
+        st.push(torch.zeros(10))
     assert calls == []

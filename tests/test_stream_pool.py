@@ -1,16 +1,21 @@
 """Host side of WaveFe.streams() / StreamPool on CPU, every kernel launch replaced by its torch
-emulation (tests/emul_streams.py): many staggered streams against one FeatureStream each, slot
-reuse, the pack bound, and refusals raised before any launch with no stream changed."""
+emulation (tests/emul_streams.py): many staggered streams against one one-stream pool each fed
+the same blocks, against the recording pushed whole and against the B=1 forward, slot reuse, a
+finish folded into the last block, the pack bound, and refusals raised before any launch with no
+stream changed.  The emulated GEMMs round differently for different segment lengths, so here a
+stream equals another bit for bit only when both are cut into the same segments; that the frames
+do not depend on the cuts is checked on the GPU (tests/test_stream_pool_gpu.py)."""
 import random
 
 import pytest
 import torch
 
 import emul_streams
-from helpers import resolve_cfg, fill_state_dict, seeded_randn
+from helpers import resolve_cfg, fill_state_dict, seeded_randn, assert_close
 import pase_b200.ops as ops
 from pase_b200 import encoder as enc
-from pase_b200.frontend import FeatureStream, StreamPool, WaveFe
+from pase_b200.frontend import StreamPool, WaveFe
+from test_extract_long import single
 
 CFGS = ["cfg/frontend/PASE.cfg", "cfg/frontend/PASE+.cfg"]
 CPU = torch.device("cpu")
@@ -84,19 +89,24 @@ def run_pool(pool, xs, calls, starts):
     return {k: torch.cat(v, 2) for k, v in outs.items()}
 
 
-def run_reference(model, xs, calls):
-    sts = [FeatureStream(model, CPU, W) for _ in xs]
-    outs = {k: [] for k in range(len(xs))}
-    for blocks, fin in calls:
-        for k, (a, b) in blocks.items():
-            outs[k].append(sts[k].push(xs[k][a:b]))
-        for k in fin:
-            outs[k].append(sts[k].finish())
-    return {k: torch.cat(v, 2) for k, v in outs.items()}
+def alone(model, x, calls):
+    """x fed to a fresh one-stream pool in the blocks and finishes of `calls` ({None: (a, b)}
+    blocks, [None] finishing), or whole in one push that also finishes it (calls None)."""
+    pool = StreamPool(model, CPU, 1, W)
+    i = pool.open()
+    if calls is None:
+        return pool.push({i: x}, finish=[i])[i]
+    return torch.cat([pool.push({i: x[a:b] for a, b in blocks.values()}, [i] if fin else [])[i]
+                      for blocks, fin in calls], 2)
+
+
+def calls_of(calls, k):
+    return [({k: c[0][k]} if k in c[0] else {}, [k] if k in c[1] else [])
+            for c in calls if k in c[0] or k in c[1]]
 
 
 @pytest.mark.parametrize("cfg_name", CFGS)
-def test_pool_matches_feature_streams(cfg_name, gathers):
+def test_pool_matches_one_stream_pools(cfg_name, gathers):
     model = make_model(cfg_name)
     lengths = [50000, 100000, 30000, 70000, 120000, 26000]      # 0: < 512 frames
     starts = [0, 0, 1, 2, 2, 4]
@@ -106,12 +116,14 @@ def test_pool_matches_feature_streams(cfg_name, gathers):
     max_samples = 60000
     pool = StreamPool(model, CPU, 6, W, max_samples)
     got = run_pool(pool, xs, calls, starts)
-    ref = run_reference(model, xs, calls)
-    for k in range(len(xs)):
-        assert got[k].shape == ref[k].shape == (1, model.emb_dim,
-                                                enc.frame_counts(model.cfg, lengths[k])[-1])
-        assert torch.equal(got[k], ref[k]), (k, float((got[k] - ref[k]).abs().max()))
     assert len(pool) == 0
+    for k in range(len(xs)):
+        ref = alone(model, xs[k], calls_of(calls, k))
+        assert got[k].shape == ref.shape == (1, model.emb_dim,
+                                             enc.frame_counts(model.cfg, lengths[k])[-1])
+        assert torch.equal(got[k], ref), (k, float((got[k] - ref).abs().max()))
+        assert_close(got[k], alone(model, xs[k], None), 1e-5, 1e-6, "stream %d" % k)
+        assert_close(got[k], single(model, xs[k]), 1e-4, 1e-5, "stream %d" % k)
     # every pack within max_samples (a longer segment alone), no slot twice in one pack
     assert gathers
     for t in gathers:
@@ -130,10 +142,23 @@ def test_reused_slot_equals_fresh_stream(gathers):
     c = pool.open()
     assert pool._streams[c].slot == 0
     outs = [pool.push({c: y[:25000], b: y[30000:]})[c], pool.push({c: y[25000:]}, [b, c])[c]]
-    got = torch.cat(outs, 2)
-    st = FeatureStream(model, CPU, W)
-    ref = torch.cat([st.push(y[:25000]), st.push(y[25000:]), st.finish()], 2)
-    assert torch.equal(got, ref)
+    ref = alone(model, y, [({0: (0, 25000)}, []), ({0: (25000, 40000)}, []), ({}, [0])])
+    assert torch.equal(torch.cat(outs, 2), ref)
+
+
+def test_finish_with_last_block_runs_one_segment(gathers):
+    model = make_model("cfg/frontend/PASE+.cfg")
+    L = W + 160 * 30 + 77
+    x = seeded_randn((L,), 21, 0.5)
+    alone(model, x, None)
+    segs = [int((t[:, 6] > 0).sum()) for t in gathers]
+    assert segs == [1] * len(enc.plan_windows(model.cfg, L, W)) == [1, 1]
+    pool = StreamPool(model, CPU, 1, W)
+    i = pool.open()
+    del gathers[:]
+    pool.push({i: x[:50000]})
+    pool.push({i: x[50000:]}, finish=[i])             # one piece, planned at the end
+    assert [int((t[:, 6] > 0).sum()) for t in gathers] == [1, 1]
 
 
 def _counters(pool):

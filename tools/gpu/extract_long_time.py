@@ -53,7 +53,7 @@ def main():
     L = int(a.minutes * 60 * SR) // 160 * 160
     x = torch.randn(L) * 0.5
     for window in (1 << 20, 1 << 21):
-        m.extract_long(x[:4 * window], window=window)           # warm-up: plan, pinned buffers
+        m.extract_long(x[:4 * window], window=window)           # warm-up: plan, pool, pinned slots
         torch.cuda.synchronize()
         t0 = time.perf_counter()
         y = m.extract_long(x, window=window)
@@ -66,7 +66,8 @@ def main():
     m._packed_plans.clear()
     xs = x[:10 * 60 * SR]
     for window in (81920, 1 << 19, 1 << 20, 1 << 21):
-        m._packed_plans.clear()
+        m._packed_plans.clear()                 # each row measures a call from a cold model
+        m._long_pool = None
         torch.cuda.empty_cache()
         torch.cuda.synchronize()
         torch.cuda.reset_peak_memory_stats()

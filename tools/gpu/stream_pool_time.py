@@ -1,8 +1,9 @@
 """StreamPool round times on one GPU: PASE+ eval, N live streams in {1, 16, 64, 256} fed 10 ms
 (160-sample) or 100 ms (1600-sample) pushes.  Per case: the median and p90 of the synchronised
 round time (one push() serving every stream) over --rounds rounds after warm-up, the same
-rounds served by N independent FeatureStreams pushed one after another (over fewer rounds when
-N is large: they are N times slower), whether the two gave equal frames, and, per push size, the
+rounds served by N independent FeatureStreams (each a one-stream pool whose plan holds one
+window's longest segment) pushed one after another (the "seq" columns, over fewer rounds when N
+is large: they are N times slower), whether the two gave equal frames, and, per push size, the
 largest N whose median round stays below the push duration (real-time capacity).  The card's
 name and power limit are read in the same run.  Prints one JSON line per measurement.
 
