@@ -218,6 +218,26 @@ int pase_reflect_pad_wave(const float* x, void* dst, void* dst_lo, int dst_fmt, 
  * x[x_off, +T) reflect-padded into dst[dst_off, +T+padL+padR); max_T >= every T. */
 int pase_reflect_pad_wave_var(const float* x, const int* tab, int nseg, int max_T, void* dst,
                               void* dst_lo, int dst_fmt, int padL, int padR, void* stream);
+
+/* ---- input (waveform) gradient of the sinc layer: the input gradients of F.conv1d and
+ * F.pad(mode='reflect') in SincConv_fast.forward (modules.py:922-928).  The transposed
+ * band-pass convolution is one polyphase NT GEMM (pase_gemm_nt / pase_tc_gemm_nt):
+ *   dxpad[n, fold v + p] = sum_{r<rows, q<fold, co<C} dyh[n, fold (v + r) + q, co] Wdg[p, (r,q,co)]
+ * with H = (rows-1) fold the left halo (DESIGN.md section 17). ---------------------------- */
+/* dy (N samples of src_frames frames x C channels, esz-byte elements, any operand format; lo
+ * twins optional, both or neither) -> dyh: N samples of dst_frames frames, frame e = dy frame
+ * e - halo, zero outside [0, T_out) -- so no sample reads its neighbours' frames. */
+int pase_sinc_dgrad_pack(const void* src, const void* src_lo, void* dst, void* dst_lo, int esz,
+                         int N, int C, int T_out, long src_frames, int halo, long dst_frames,
+                         void* stream);
+/* band-pass bank filt (C,k) (pase_sinc_make) -> banded operand Wdg (fold x rows*fold*C):
+ * Wdg[p, (r*fold+q)*C+co] = filt[co][H+p-fold*r-q] inside [0,k), else 0; H = (rows-1)*fold. */
+int pase_sinc_dgrad_weight(const float* filt, float* Wdg, int C, int k, int fold, int rows,
+                           void* stream);
+/* adjoint of pase_reflect_pad_wave: dx[n,t] = dpad[n,t+padL] + [1<=t<=padL] dpad[n,padL-t]
+ * + [T-1-padR<=t<=T-2] dpad[n,padL+2(T-1)-t]  (dpad rows of pitch `pitch`, dx (N,T) fp32) */
+int pase_reflect_fold_wave(const float* dpad, long pitch, float* dx, int N, int T, int padL,
+                           int padR, void* stream);
 /* batch statistics -> per-channel affine; updates running stats (training) */
 int pase_bn_finalize(const double* colsum, const double* colsumsq, int C, int fold,
                      double count, const float* gamma, const float* beta,

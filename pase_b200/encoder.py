@@ -66,6 +66,13 @@ class ConvGeom(object):
             self.Nn = sinc_fold * Cout
             self.P = _cdiv(self.Tpad, sinc_fold)       # rows per sample
             self.rows_out = _cdiv(self.T_out, sinc_fold)
+            # input gradient (DESIGN.md section 17): row v of the transposed convolution gives
+            # the padded positions fold*v .. fold*v+fold-1 from the dg_rows folded rows of dy
+            # that start dg_halo frames earlier
+            self.dg_halo = _cdiv(k - 1, sinc_fold) * sinc_fold
+            self.dg_rows = self.dg_halo // sinc_fold + 1
+            self.dg_K = self.dg_rows * sinc_fold * Cout
+            self.dg_P = self.P + self.dg_rows - 1      # rows per sample of the haloed dy copy
         else:
             self.fold = 1
             self.lda = s * Cin
@@ -209,6 +216,7 @@ class EncoderPlan(object):
         self.dYg = self.dsrc = self.WqT = self.dWq = None
         self.dcat = self.WcatT = self.dWcat = self.g = None
         self.stats_b = self.grad_vec = self.amax = None
+        self.dyh = self.dyh_lo = self.filt = self.Wdg = None     # ensure_input_grad
         self.generation = 0
 
     def ensure_backward(self):
@@ -271,6 +279,23 @@ class EncoderPlan(object):
         # running maxima for the 3xF16 gradient scales: 2 floats per use, zeroed per backward
         self.amax = torch.zeros(2 * (self.nblk + 4), **f32) if f16x2 else None
         self.backward_ready = True
+
+    def ensure_input_grad(self):
+        """Allocate the buffers of the sinc layer's input gradient (_sinc_input_grad) on the
+        first backward that returns the waveform gradient: the haloed copy of dy in the GEMM
+        format (zero halos and slack, written only inside), the band-pass bank, its banded
+        dgrad operand and the padded-waveform gradient dxpad[0]."""
+        self.ensure_backward()
+        if self.dyh is not None:
+            return
+        g, N, p, device = self.geoms[0], self.N, self.precision, self.device
+        n = N * g.dg_P * g.Nn + g.dg_rows * g.Nn + 128          # + slack: rows past the last
+        self.dyh = torch.zeros(n, dtype=p.dtype, device=device)
+        self.dyh_lo = torch.zeros(n, dtype=p.dtype, device=device) if p.split else None
+        self._ops[("dyh", 0)] = gemm.Operand(self.dyh, self.dyh_lo, self.gscale[0])
+        self.filt = torch.empty(g.Cout * g.k, dtype=torch.float32, device=device)
+        self.Wdg = torch.empty(g.fold * g.dg_K, dtype=torch.float32, device=device)
+        self.dxpad[0] = torch.empty(N * g.P * g.fold, dtype=torch.float32, device=device)
 
     # -- GEMM operands -----------------------------------------------------------------
     def operand(self, name, buf, fresh=True, kind="act", n=None):
@@ -1032,10 +1057,12 @@ def plan_windows(cfg, L, window):
     return segs
 
 
-def encoder_backward(plan, mod, params, gout, gntc, training, sink=None):
+def encoder_backward(plan, mod, params, gout, gntc, training, sink=None, dx=None,
+                     param_grads=True):
     """Returns dict name -> gradient tensor (fp32, parameter shape); see
     encoder_backward_steps (this runs it to completion)."""
-    gen = encoder_backward_steps(plan, mod, params, gout, gntc, training, sink)
+    gen = encoder_backward_steps(plan, mod, params, gout, gntc, training, sink, dx=dx,
+                                 param_grads=param_grads)
     try:
         while True:
             next(gen)
@@ -1043,9 +1070,16 @@ def encoder_backward(plan, mod, params, gout, gntc, training, sink=None):
         return done.value
 
 
-def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, split=None):
+def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, split=None,
+                           dx=None, param_grads=True):
     """Generator form of the backward sweep.  Returns (StopIteration.value) dict name ->
     gradient tensor (fp32, parameter shape).
+
+    dx (optional): (N,1,T) fp32 tensor that receives the gradient of the input waveform
+    (_sinc_input_grad).  param_grads=False (a frozen encoder, dx given) runs the data-gradient
+    sweep only: no weight-gradient GEMM, pase_sinc_grad, bias colsum, weight re-layout, cast or
+    sink write; it returns {}.  The BatchNorm/PReLU reductions stay: in train mode their sums
+    enter the data gradient.
 
     split (sink mode only): block index s.  The generator yields ONCE, after every gradient
     of the output layer, the QRNN and blocks >= s has been written to its sink destination
@@ -1060,7 +1094,15 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     conv weight gradients by the batched re-layout, the sinc cut-offs by pase_sinc_grad,
     everything else by one batched strided copy -- and {} is returned: no per-parameter
     clones, no autograd accumulation kernels, no packing before the all-reduce."""
+    if not param_grads and dx is None:
+        raise ValueError("encoder_backward_steps: nothing to compute (no parameter gradients, "
+                         "no dx)")
     plan.ensure_backward()
+    if dx is not None:
+        plan.ensure_input_grad()
+    if not param_grads:
+        sink = None
+    pg = param_grads
     call = ops.call
     cfg, G, N = plan.cfg, plan.geoms, plan.N
     Tq, Kc, rows, emb = plan.Tq, plan.Kc, plan.rows, plan.emb
@@ -1091,22 +1133,24 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     use_stats = 1 if (plan.norm_out and training) else 0
     call("pase_out_bwd_apply", plan.g, plan.yout, bo[0], bo[1], bo[2], S1o, S2o, float(rows),
          use_stats, rows, emb)
-    call("pase_colsum", plan.g, emb, rows, emb, sb[plan.bs_bw:plan.bs_bw + emb])
-    plan.tn("g", plan.g, emb, rows, 0, True, "cat", plan.cat, Kc, rows, False, plan.dWcat, Kc,
-            emb, Kc, 1, rows, 1.0, 0)
+    if pg:
+        call("pase_colsum", plan.g, emb, rows, emb, sb[plan.bs_bw:plan.bs_bw + emb])
+        plan.tn("g", plan.g, emb, rows, 0, True, "cat", plan.cat, Kc, rows, False, plan.dWcat,
+                Kc, emb, Kc, 1, rows, 1.0, 0)
     call("pase_transpose_pad", plan.Wcat, Kc, plan.WcatT, emb, emb, Kc)
-    plan.nt("g", plan.g, emb, False, "WcatT", plan.WcatT, emb, True, plan.dcat, Kc, rows, Kc,
+    # the weight-gradient GEMM above converted g into the GEMM format; without it, this one does
+    plan.nt("g", plan.g, emb, not pg, "WcatT", plan.WcatT, emb, True, plan.dcat, Kc, rows, Kc,
             emb, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad")
     dWcat = plan.dWcat.view(emb, Kc)
     first = plan.H if plan.rnn else plan.Clast
     copies = []          # sink mode: (src tensor view, rows, cols, src_ld, destination name)
-    if sink is not None:
+    if pg and sink is not None:
         copies.append((dWcat, emb, first, Kc, "W.weight"))
         if plan.skips:
             for i in range(plan.nblk - 1):
                 copies.append((dWcat[:, plan.col_off[i]:], emb, G[i].Cout, Kc,
                                "denseskips.%d.weight" % i))
-    else:
+    elif pg:
         # gradients handed to autograd must not alias plan-owned buffers (the next backward
         # would overwrite them): copy the slices out
         grads["W.weight"] = dWcat[:, :first].clone().reshape(params["W.weight"].shape)
@@ -1121,18 +1165,19 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     if plan.rnn:
         Cq, H = Cl, plan.H
         call("pase_qrnn_scan_bwd", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg, N, Tq, H)
-        call("pase_colsum", plan.dYg, 3 * H, rows, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
-        plan.tn("dYg", plan.dYg, 3 * H, Tq, 0, True, "xq", plan.xq, Cq, Tq + 1, False,
-                plan.dWq, 2 * Cq, 3 * H, 2 * Cq, N, Tq, 1.0, 0)
-        dWq = plan.dWq.view(3 * H, 2 * Cq)
-        if sink is not None:        # [x_{t-1} | x_t] GEMM order -> the parameter's [x_t | x_{t-1}]
+        if pg:
+            call("pase_colsum", plan.dYg, 3 * H, rows, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
+            plan.tn("dYg", plan.dYg, 3 * H, Tq, 0, True, "xq", plan.xq, Cq, Tq + 1, False,
+                    plan.dWq, 2 * Cq, 3 * H, 2 * Cq, N, Tq, 1.0, 0)
+            dWq = plan.dWq.view(3 * H, 2 * Cq)
+        if pg and sink is not None:   # [x_{t-1} | x_t] GEMM order -> the parameter's [x_t | x_{t-1}]
             dst = sink["rnn.layers.0.linear.weight"].view(3 * H, 2 * Cq)
             copies.append((dWq[:, Cq:], 3 * H, Cq, 2 * Cq, dst))
             copies.append((dWq, 3 * H, Cq, 2 * Cq, dst[:, Cq:]))
-        else:
+        elif pg:
             grads["rnn.layers.0.linear.weight"] = torch.cat([dWq[:, Cq:], dWq[:, :Cq]], 1)
         call("pase_transpose_pad", plan.Wq, 2 * Cq, plan.WqT, 3 * H, 3 * H, 2 * Cq)
-        plan.nt("dYg", plan.dYg, 3 * H, False, "WqT", plan.WqT, 3 * H, True, plan.dsrc, 2 * Cq,
+        plan.nt("dYg", plan.dYg, 3 * H, not pg, "WqT", plan.WqT, 3 * H, True, plan.dsrc, 2 * Cq,
                 rows, 2 * Cq, 3 * H, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad")
         last_src = dict(A=plan.dsrc[Cq:], a_ss=Tq * 2 * Cq, a_rs=2 * Cq,
                         B=plan.dsrc, b_ss=Tq * 2 * Cq, b_rs=2 * Cq, b_shift=1)
@@ -1185,7 +1230,7 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
              P(pre + "norm.weight"), scale, shift, P(pre + "act.weight"), a1, a2,
              float(N * g.T_out), *src, dst, dst_lo, fmt, d_ss, None if g.sinc else dbi, amax,
              plan.gscale[l])
-        if g.sinc:
+        if g.sinc and pg:
             plan.tn(("dyz", l), plan.dyz[l], g.Nn, g.rows_out, 0, False, ("apad", l), plan.apad[l],
                     g.lda, g.P, False, plan.dWt[l], g.K, g.Nn, g.K, N, g.rows_out, 1.0, 0)
             if sink is not None:
@@ -1199,14 +1244,20 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
             if sink is None:
                 grads[pre + "conv.low_hz_"] = dlow
                 grads[pre + "conv.band_hz_"] = dband
-        else:
-            plan.tn(("dyz", l), plan.dyz[l], C, g.Pd, g.taps - 1, False, ("apad", l), plan.apad[l],
-                    g.lda, g.P, False, plan.dWt[l], g.K, C, g.K, N, g.T_out, 1.0, 0)
+        elif not g.sinc:
+            if pg:
+                plan.tn(("dyz", l), plan.dyz[l], C, g.Pd, g.taps - 1, False, ("apad", l),
+                        plan.apad[l], g.lda, g.P, False, plan.dWt[l], g.K, C, g.K, N, g.T_out,
+                        1.0, 0)
             if l > 0:
                 plan.nt(("dyz", l), plan.dyz[l], C, False, ("Wd", l), plan.Wd[l], g.taps * C, False,
                         plan.dxpad[l], g.s * g.Cin, N * g.Pd, g.s * g.Cin, g.taps * C, 1.0, None,
                         g.Pd, g.P, g.P, 1, None, None, 0, akind="grad")
+        if g.sinc and dx is not None:
+            _sinc_input_grad(plan, mod, P, g, dx)
 
+    if not pg:
+        return {}
     if sink is not None:
         if split is not None:
             _emit_sunk_grads(plan, G, sink, copies, range(0, split), False, "lo")
@@ -1234,6 +1285,24 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     call("pase_cast_d2f", sb, gv, sb.numel(), 1.0)
     grads.update(_small_grad_views(plan, G, gv, range(plan.nblk), True))
     return grads
+
+
+def _sinc_input_grad(plan, mod, P, g, dx):
+    """dx (N,1,T) fp32 = the waveform gradient, from the sinc layer's output gradient in
+    plan.dyz[0] (DESIGN.md section 17): the band-pass bank regenerated from low_hz_ / band_hz_,
+    its banded dgrad operand, a copy of dy with a zero halo around every sample, one polyphase
+    GEMM into the padded-waveform gradient and the reflect fold-back."""
+    call, N, f, p = ops.call, plan.N, g.fold, plan.precision
+    call("pase_sinc_make", P("blocks.0.conv.low_hz_"), P("blocks.0.conv.band_hz_"), mod._sinc_n,
+         mod._sinc_win, plan.filt, plan.Wt[0], g.Cout, g.k, f, g.K, 50.0, 50.0,
+         float(plan.cfg["sr"]))
+    call("pase_sinc_dgrad_weight", plan.filt, plan.Wdg, g.Cout, g.k, f, g.dg_rows)
+    call("pase_sinc_dgrad_pack", plan.dyz[0], plan.dyz_lo[0], plan.dyh, plan.dyh_lo, p.esz, N,
+         g.Cout, g.T_out, g.Ty, g.dg_halo, g.dg_P * f)
+    plan.nt(("dyh", 0), plan.dyh, g.Nn, False, "Wdg", plan.Wdg, g.dg_K, True, plan.dxpad[0], f,
+            N * g.dg_P, f, g.dg_K, 1.0, None, g.dg_P, g.P, g.P, 1, None, None, 0, akind="grad")
+    call("pase_reflect_fold_wave", plan.dxpad[0], g.P * f, dx.reshape(-1), N, plan.T, g.padL,
+         g.padR)
 
 
 def _small_grad_views(plan, G, gv, layers, top):
@@ -1322,5 +1391,11 @@ class _EncoderFn(torch.autograd.Function):
         if sink is not None and any(n not in sink for n in ctx.names):
             raise RuntimeError("pase_b200: WaveFe.grad_sink must name every parameter "
                                "(missing %s)" % [n for n in ctx.names if n not in sink][:3])
-        grads = encoder_backward(plan, ctx.mod, params, gout, gntc, ctx.training, sink)
-        return (None, None, None, None, None) + tuple(grads.get(n) for n in ctx.names)
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty(plan.N, 1, plan.T, dtype=torch.float32, device=plan.device)
+        # all or nothing: one parameter that needs a gradient runs the full sweep
+        param_grads = any(ctx.needs_input_grad[5:])
+        grads = encoder_backward(plan, ctx.mod, params, gout, gntc, ctx.training, sink, dx=dx,
+                                 param_grads=param_grads)
+        return (dx, None, None, None, None) + tuple(grads.get(n) for n in ctx.names)

@@ -237,7 +237,11 @@ class WaveFe(Model):
         if not x.is_cuda:
             raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; got a %s tensor. "
                                "There is no CPU path." % x.device)
-        x = x.contiguous().float()
+        return self._encode(x.contiguous().float())
+
+    def _encode(self, x):
+        """encode past its checks on the input: differentiated (the _EncoderFn node) when grad
+        mode is on and the waveform or a parameter needs a gradient, else the forward alone."""
         self._sinc_consts(x.device)
         plan = self._plan(x.shape[0], x.shape[2], x.device)
         named = [(n, p) for n, p in self.named_parameters()]
@@ -246,7 +250,8 @@ class WaveFe(Model):
         if tensors and tensors[0].device != x.device:
             raise RuntimeError("WaveFe parameters live on %s but the input is on %s"
                                % (tensors[0].device, x.device))
-        if torch.is_grad_enabled() and any(p.requires_grad for p in tensors):
+        if torch.is_grad_enabled() and (x.requires_grad or
+                                        any(p.requires_grad for p in tensors)):
             plan.ensure_backward()
             return _enc._EncoderFn.apply(x, self, plan, self.training, names, *tensors)
         with torch.no_grad():
