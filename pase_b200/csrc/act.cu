@@ -2,11 +2,14 @@
 // All HBM-bound: channel-last float4 accesses, one pass per tensor.
 #include "common.cuh"
 #include "bn_stream.cuh"
-#include <cstdlib>
 
 namespace {
 
 constexpr int THREADS = 256;
+// time steps per thread of the register-resident BatchNorm / PReLU kernels (measured 3.31 vs
+// 3.42 ms/step against 4 steps per thread with 2-3 resident blocks per SM: loads in flight per
+// thread matter more than occupancy here)
+constexpr int RUN = 8;
 
 // DF: operand format of the padded waveform (block 0's GEMM operand)
 template <int DF>
@@ -118,7 +121,7 @@ __device__ __forceinline__ float prelu1(float u, float a) { return u > 0.f ? u :
 //   has one writer and comes out the same on every run.
 // One sample: yn its raw conv output, dst / pool offsets d_base / p_base; thread idx owns the
 // channel quad idx % (C/4) over RUN time steps of the padded output.
-template <typename YT, int DF, int RUN>
+template <typename YT, int DF>
 __device__ __forceinline__ void bn_prelu_pad_fwd_sample(
     const YT* __restrict__ yn, long idx, int T, int C, const float* __restrict__ scale,
     const float* __restrict__ shift, const float* __restrict__ alpha, void* __restrict__ dst_v,
@@ -184,7 +187,7 @@ __device__ __forceinline__ void bn_prelu_pad_fwd_sample(
   }
 }
 
-template <typename YT, int DF, int RUN>
+template <typename YT, int DF>
 __global__ void __launch_bounds__(THREADS)
 bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                         const float* __restrict__ scale, const float* __restrict__ shift,
@@ -193,16 +196,16 @@ bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                         long p_rs, int pool_d, int pool_T, void* __restrict__ dst_lo_v) {
   pdl_wait();
   const int n = blockIdx.y;
-  bn_prelu_pad_fwd_sample<YT, DF, RUN>(y + (long)n * y_ss,
-                                       (long)blockIdx.x * blockDim.x + threadIdx.x, T, C, scale,
-                                       shift, alpha, dst_v, (long)n * d_ss, d_rs, padL, Tp, pool,
-                                       (long)n * p_ss, p_rs, pool_d, pool_T, dst_lo_v);
+  bn_prelu_pad_fwd_sample<YT, DF>(y + (long)n * y_ss,
+                                  (long)blockIdx.x * blockDim.x + threadIdx.x, T, C, scale,
+                                  shift, alpha, dst_v, (long)n * d_ss, d_rs, padL, Tp, pool,
+                                  (long)n * p_ss, p_rs, pool_d, pool_T, dst_lo_v);
 }
 
 // Packed variable-length form: blockIdx.y = utterance, tab row {T, y_off, dst_off, pool_off,
 // pool_d, pool_T} (elements).  sep != 0: the row ahead of each utterance's output (dst_off -
 // d_rs, C elements) is written zero (the QRNN input's x_{-1} row).
-template <typename YT, int DF, int RUN>
+template <typename YT, int DF>
 __global__ void __launch_bounds__(THREADS)
 bn_prelu_pad_fwd_var_kernel(const YT* __restrict__ y, const int* __restrict__ tab, int C,
                             const float* __restrict__ scale, const float* __restrict__ shift,
@@ -226,9 +229,9 @@ bn_prelu_pad_fwd_var_kernel(const YT* __restrict__ y, const int* __restrict__ ta
       st4_f16x2(reinterpret_cast<__half*>(dst_v) + o, reinterpret_cast<__half*>(dst_lo_v) + o, z);
     }
   }
-  bn_prelu_pad_fwd_sample<YT, DF, RUN>(y + __ldg(r + 1), idx, T, C, scale, shift, alpha, dst_v,
-                                       d_base, d_rs, padL, T + padL + padR, pool, __ldg(r + 3),
-                                       p_rs, pool_d, __ldg(r + 5), dst_lo_v);
+  bn_prelu_pad_fwd_sample<YT, DF>(y + __ldg(r + 1), idx, T, C, scale, shift, alpha, dst_v,
+                                  d_base, d_rs, padL, T + padL + padR, pool, __ldg(r + 3),
+                                  p_rs, pool_d, __ldg(r + 5), dst_lo_v);
 }
 
 // ---- backward pass 1: du + reductions ----
@@ -239,7 +242,7 @@ bn_prelu_pad_fwd_var_kernel(const YT* __restrict__ y, const int* __restrict__ ta
 // back at the two sequence ends), the optional shifted source B (QRNN) and the broadcast of
 // the mean-pooled dense-skip gradient.  Straight-line loads first (no branch between a load
 // and the next one, so all DRAM requests of the run are in flight together).
-template <typename GT, int RUN>
+template <typename GT>
 __device__ __forceinline__ void load_grad_run(const BwdSrc& s, int n, int T, long t0, int nvalid,
                                               int c, float4 (&gs)[RUN]) {
   const GT* an = reinterpret_cast<const GT*>(s.A) + (long)n * s.a_ss + c;
@@ -292,8 +295,8 @@ __device__ __forceinline__ void load_grad_run(const BwdSrc& s, int n, int T, lon
 // next layer's input gradient as its dgrad GEMM wrote it).  amax (optional, float[2]):
 // running maxima of |du| and |xhat| (bit-pattern atomicMax), from which pass 2 derives the
 // power-of-two scale of the fp16 gradient operand (3xF16 mode).
-template <typename YT, typename GT, int RUN>
-__global__ void __launch_bounds__(THREADS, RUN <= 4 ? 2 : 1)
+template <typename YT, typename GT>
+__global__ void __launch_bounds__(THREADS, 1)
 bn_prelu_bwd_reduce_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                            const float* __restrict__ mean, const float* __restrict__ invstd,
                            const float* __restrict__ scale, const float* __restrict__ shift,
@@ -330,7 +333,7 @@ bn_prelu_bwd_reduce_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
       const int t = (int)t0 + (i < nvalid ? i : 0);
       ys[i] = ld4t(yn + (long)t * C + c);
     }
-    load_grad_run<GT, RUN>(s, n, T, t0, nvalid, c, gs);
+    load_grad_run<GT>(s, n, T, t0, nvalid, c, gs);
     const float scv[4] = {sc.x, sc.y, sc.z, sc.w}, shv[4] = {sh.x, sh.y, sh.z, sh.w};
     const float alv[4] = {al.x, al.y, al.z, al.w};
     const float muv[4] = {mu.x, mu.y, mu.z, mu.w}, isv[4] = {is.x, is.y, is.z, is.w};
@@ -406,8 +409,8 @@ bn_prelu_bwd_reduce_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
 //     |dy| <= max_c |gamma_c invstd_c| (max|du| + |S1_c/M| + max|xhat| |S2_c/M|)
 // (amax from pass 1), every block computes the same scale; block (0,0) publishes
 // scale_out = {1/s, s} for the consuming GEMMs (alpha_dev).
-template <typename YT, int DF, int RUN>
-__global__ void __launch_bounds__(THREADS, RUN <= 4 ? 3 : 2)
+template <typename YT, int DF>
+__global__ void __launch_bounds__(THREADS, 2)
 bn_prelu_bwd_apply_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                           const float* __restrict__ mean, const float* __restrict__ invstd,
                           const float* __restrict__ gamma, const double* __restrict__ S1,
@@ -513,7 +516,7 @@ bn_prelu_bwd_apply_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
 // sources (same arithmetic as pass 1, so the sums S1 / S2 it is centred with are exactly its
 // own) -- pass 1 then writes nothing but its 3C sums, and the du tensor (one write + one read
 // of the layer's activation size) disappears from the step.
-template <typename YT, typename GT, int DF, int RUN>
+template <typename YT, typename GT, int DF>
 __global__ void __launch_bounds__(THREADS, 1)
 bn_prelu_bwd_apply_src_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                               const float* __restrict__ mean, const float* __restrict__ invstd,
@@ -577,7 +580,7 @@ bn_prelu_bwd_apply_src_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
         const int t = (int)t0 + (i < nvalid ? i : 0);
         vs[i] = ld4t(yn + (long)t * C + c);
       }
-      load_grad_run<GT, RUN>(s, n, T, t0, nvalid, c, gs);
+      load_grad_run<GT>(s, n, T, t0, nvalid, c, gs);
 #pragma unroll
       for (int i = 0; i < RUN; ++i) {
         if (i >= nvalid) break;
@@ -942,18 +945,6 @@ __global__ void scale_dev_kernel(float* __restrict__ x, long n, const float* __r
     x[i] *= f;
 }
 
-// time steps per thread of the BatchNorm / PReLU passes: 8 (default; measured 3.31 vs 3.42
-// ms/step against 4 steps per thread with 2-3 resident blocks per SM: loads in flight per
-// thread matter more than occupancy here); PASE_B200_BN_RUN=4 selects the other variant
-inline int bn_run() {
-  static int r = 0;
-  if (r == 0) {
-    const char* e = getenv("PASE_B200_BN_RUN");
-    r = (e && atoi(e) == 4) ? 4 : 8;
-  }
-  return r;
-}
-
 inline unsigned blocks_for(long total, int threads, int cap_mult = 8) {
   long b = (total + threads - 1) / threads;
   long cap = (long)pase_num_sms() * cap_mult;
@@ -1005,11 +996,10 @@ BnBwdPlan bn_bwd_plan(const BnStreamArgs& a, int pass) {
     p.path = 1; p.rows = sp.TT; p.items = sp.total; p.gx = sp.grid; p.blocks = sp.grid;
     return p;
   }
-  const int RUN = bn_run();
   const long threads = (long)(a.C / 4) * ((a.T + RUN - 1) / RUN);
   long gx = (threads + THREADS - 1) / THREADS;
   if ((THREADS % (a.C / 4)) == 0) {          // stride keeps the channel quad: cap the grid
-    long cap = ((RUN == 8 ? 8L : 16L) * pase_num_sms() + a.N - 1) / a.N;
+    long cap = (8L * pase_num_sms() + a.N - 1) / a.N;
     if (cap < 1) cap = 1;
     if (gx > cap) gx = cap;
   }
@@ -1162,16 +1152,14 @@ int pase_bn_prelu_pad_fwd(const void* y, int y_bf16, long y_sample_stride, int N
   }
   if (pool == nullptr) pool_d = 0;
   const int Tp = T + padL + padR;
-  const int RUN = bn_run();
   const long threads = (long)(C / 4) * ((Tp + RUN - 1) / RUN);
   dim3 grid((unsigned)((threads + THREADS - 1) / THREADS), N);
   cudaStream_t st = (cudaStream_t)stream;
-#define PASE_FWD_R(YT, DF, RV)                                                                 \
-  PASE_LAUNCH((bn_prelu_pad_fwd_kernel<YT, DF, RV>), grid, THREADS, 0, st,                                \
+#define PASE_FWD(YT, DF)                                                                       \
+  PASE_LAUNCH((bn_prelu_pad_fwd_kernel<YT, DF>), grid, THREADS, 0, st,                         \
       reinterpret_cast<const YT*>(y), y_sample_stride, T, C, scale, shift, alpha, dst,         \
-      dst_sample_stride, dst_row_stride, padL, Tp, pool, pool_sample_stride, pool_row_stride, \
+      dst_sample_stride, dst_row_stride, padL, Tp, pool, pool_sample_stride, pool_row_stride,  \
       pool_d, pool_T, dst_lo)
-#define PASE_FWD(YT, DF) do { if (RUN == 8) PASE_FWD_R(YT, DF, 8); else PASE_FWD_R(YT, DF, 4); } while (0)
   if (y_bf16) {
     if (dst_fmt == PASE_FMT_F32) PASE_FWD(__nv_bfloat16, PASE_FMT_F32);
     else if (dst_fmt == PASE_FMT_BF16) PASE_FWD(__nv_bfloat16, PASE_FMT_BF16);
@@ -1182,7 +1170,6 @@ int pase_bn_prelu_pad_fwd(const void* y, int y_bf16, long y_sample_stride, int N
     else PASE_FWD(float, PASE_FMT_F16X2);
   }
 #undef PASE_FWD
-#undef PASE_FWD_R
   PASE_LAUNCH_CHECK("pase_bn_prelu_pad_fwd");
   return PASE_OK;
 }
@@ -1210,15 +1197,13 @@ int pase_bn_prelu_pad_fwd_var(const void* y, int y_bf16, const int* tab, int nse
       PASE_CHECK_STRIDE(fn, pool_row_stride, "pool_row_stride");
     }
   }
-  const int RUN = bn_run();
   const long threads = (long)(C / 4) * (((long)max_T + padL + padR + RUN - 1) / RUN);
   dim3 grid((unsigned)((threads + THREADS - 1) / THREADS), nseg);
   cudaStream_t st = (cudaStream_t)stream;
-#define PASE_FWD_R(YT, DF, RV)                                                                 \
-  PASE_LAUNCH((bn_prelu_pad_fwd_var_kernel<YT, DF, RV>), grid, THREADS, 0, st,                \
+#define PASE_FWD(YT, DF)                                                                       \
+  PASE_LAUNCH((bn_prelu_pad_fwd_var_kernel<YT, DF>), grid, THREADS, 0, st,                     \
       reinterpret_cast<const YT*>(y), tab, C, scale, shift, alpha, dst, dst_row_stride, padL,  \
       padR, pool, pool_row_stride, sep, dst_lo)
-#define PASE_FWD(YT, DF) do { if (RUN == 8) PASE_FWD_R(YT, DF, 8); else PASE_FWD_R(YT, DF, 4); } while (0)
   if (y_bf16) {
     if (dst_fmt == PASE_FMT_F32) PASE_FWD(__nv_bfloat16, PASE_FMT_F32);
     else if (dst_fmt == PASE_FMT_BF16) PASE_FWD(__nv_bfloat16, PASE_FMT_BF16);
@@ -1229,7 +1214,6 @@ int pase_bn_prelu_pad_fwd_var(const void* y, int y_bf16, const int* tab, int nse
     else PASE_FWD(float, PASE_FMT_F16X2);
   }
 #undef PASE_FWD
-#undef PASE_FWD_R
   PASE_LAUNCH_CHECK(fn);
   return PASE_OK;
 }
@@ -1261,21 +1245,19 @@ int pase_bn_prelu_bwd_reduce(const void* y, int y_bf16, long y_sample_stride, in
     sa.S1 = S1; sa.S2 = S2; sa.dalpha = dalpha; sa.amax = amax;
     return pase_bn_stream_reduce(sa, (cudaStream_t)stream);
   }
-  const int RUN = plan.rows;
   dim3 grid((unsigned)plan.gx, N);
   const size_t sm = 3 * C * sizeof(double) + 2 * sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
   // C >= 2048: the block sums need more than the default 48 KB of dynamic shared memory
-#define PASE_RED_R(YT, GT, RV)                                                               \
+#define PASE_RED(YT, GT)                                                                     \
   do {                                                                                       \
     if (sm > 48 * 1024)                                                                      \
-      cudaFuncSetAttribute(bn_prelu_bwd_reduce_kernel<YT, GT, RV>,                           \
+      cudaFuncSetAttribute(bn_prelu_bwd_reduce_kernel<YT, GT>,                               \
                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);            \
-    bn_prelu_bwd_reduce_kernel<YT, GT, RV><<<grid, THREADS, sm, st>>>(                       \
+    bn_prelu_bwd_reduce_kernel<YT, GT><<<grid, THREADS, sm, st>>>(                           \
         reinterpret_cast<const YT*>(y), y_sample_stride, T, C, mean, invstd, scale, shift,   \
         alpha, s, reinterpret_cast<YT*>(dst), dst_sample_stride, S1, S2, dalpha, amax);      \
   } while (0)
-#define PASE_RED(YT, GT) do { if (RUN == 8) PASE_RED_R(YT, GT, 8); else PASE_RED_R(YT, GT, 4); } while (0)
   if (y_bf16) {
     if (a_bf16) PASE_RED(__nv_bfloat16, __nv_bfloat16);
     else PASE_RED(__nv_bfloat16, float);
@@ -1284,7 +1266,6 @@ int pase_bn_prelu_bwd_reduce(const void* y, int y_bf16, long y_sample_stride, in
     else PASE_RED(float, float);
   }
 #undef PASE_RED
-#undef PASE_RED_R
   PASE_LAUNCH_CHECK("pase_bn_prelu_bwd_reduce");
   return PASE_OK;
 }
@@ -1311,21 +1292,18 @@ int pase_bn_prelu_bwd_apply(const void* y, int y_bf16, long y_sample_stride, int
   const int rc = bn_bwd_check("pase_bn_prelu_bwd_apply", sa, 2, du);
   if (rc != PASE_OK) return rc;
   const BnBwdPlan plan = bn_bwd_plan(sa, 2);          // always the register kernel
-  const int RUN = plan.rows;
   dim3 grid((unsigned)plan.gx, N);
   const size_t sm = C * sizeof(double) + sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
-#define PASE_APP_R(YT, DF, RV)                                                                \
-  bn_prelu_bwd_apply_kernel<YT, DF, RV><<<grid, THREADS, sm, st>>>(                           \
+#define PASE_APP(YT, DF)                                                                      \
+  bn_prelu_bwd_apply_kernel<YT, DF><<<grid, THREADS, sm, st>>>(                               \
       reinterpret_cast<const YT*>(y), y_sample_stride, T, C, mean, invstd, gamma, S1, S2,     \
       1.0 / count, reinterpret_cast<const YT*>(du), dst, dst_sample_stride, dbias_acc,        \
       dst_lo, amax, scale_out)
-#define PASE_APP(YT, DF) do { if (RUN == 8) PASE_APP_R(YT, DF, 8); else PASE_APP_R(YT, DF, 4); } while (0)
   if (dst_fmt == PASE_FMT_BF16) PASE_APP(__nv_bfloat16, PASE_FMT_BF16);
   else if (dst_fmt == PASE_FMT_F16X2) PASE_APP(float, PASE_FMT_F16X2);
   else PASE_APP(float, PASE_FMT_F32);
 #undef PASE_APP
-#undef PASE_APP_R
   PASE_LAUNCH_CHECK("pase_bn_prelu_bwd_apply");
   return PASE_OK;
 }
@@ -1367,15 +1345,13 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
     sa.dbias = dbias_acc; sa.amax = const_cast<float*>(amax); sa.scale_out = scale_out;
     return pase_bn_stream_apply(sa, (cudaStream_t)stream);
   }
-  const int RUN = plan.rows;
   dim3 grid((unsigned)plan.gx, N);
   const size_t sm = C * sizeof(double) + sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
-#define PASE_APS_R(YT, GT, DF, RV)                                                             \
-  bn_prelu_bwd_apply_src_kernel<YT, GT, DF, RV><<<grid, THREADS, sm, st>>>(                    \
+#define PASE_APS(YT, GT, DF)                                                                   \
+  bn_prelu_bwd_apply_src_kernel<YT, GT, DF><<<grid, THREADS, sm, st>>>(                        \
       reinterpret_cast<const YT*>(y), y_sample_stride, T, C, mean, invstd, gamma, scale, shift, \
       alpha, S1, S2, 1.0 / count, s, dst, dst_sample_stride, dbias_acc, dst_lo, amax, scale_out)
-#define PASE_APS(YT, GT, DF) do { if (RUN == 8) PASE_APS_R(YT, GT, DF, 8); else PASE_APS_R(YT, GT, DF, 4); } while (0)
   if (dst_fmt == PASE_FMT_BF16) {
     if (a_bf16) PASE_APS(__nv_bfloat16, __nv_bfloat16, PASE_FMT_BF16);
     else PASE_APS(__nv_bfloat16, float, PASE_FMT_BF16);
@@ -1385,7 +1361,6 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
     PASE_APS(float, float, PASE_FMT_F32);
   }
 #undef PASE_APS
-#undef PASE_APS_R
   PASE_LAUNCH_CHECK("pase_bn_prelu_bwd_apply_src");
   return PASE_OK;
 }

@@ -8,14 +8,15 @@
 // mbarrier): the bytes in flight per SM (2 blocks x 2 stages x 32 KB) no longer depend on
 // registers, and the per-block reductions happen once per SM instead of once per 70 KB.
 #include "bn_stream.cuh"
-#include <cstdlib>
 
 namespace {
 
 constexpr int THREADS = 256;
-// tile configuration: TE = TT * C elements per tensor per stage, NS stages
-//   <4096, 3>: 32 KB (fp32 y + g) per stage, 2 in flight per block
-//   <2048, 6>: 16 KB per stage, 5 in flight per block (same shared memory, deeper queue)
+// tile geometry: ELEMS = TT * C elements per tensor and stage (32 KB of fp32 y + g), STAGES
+// stages (2 in flight per block), ITEMS float4 quads per thread and tile
+struct Tile {
+  static constexpr int ELEMS = 4096, STAGES = 3, ITEMS = ELEMS / 4 / THREADS;
+};
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
@@ -60,14 +61,8 @@ struct Geo {
   int TT;
 };
 
-template <int TE_, int NS_>
-struct TileCfg {
-  static constexpr int TE = TE_, NS = NS_;
-  static constexpr int ITEMS = TE_ / 4 / THREADS;   // float4 quads per thread per tile
-};
-
 // One tile of y and of gradient source A into stage `st` (called by one thread).
-template <typename YT, typename GT, int TILE_ELEMS>
+template <typename YT, typename GT>
 __device__ __forceinline__ void issue_tile(const BnStreamArgs& a, const Geo& g, long tile,
                                            uint8_t* stage, uint64_t* bar) {
   const int n = (int)(tile / g.tps);
@@ -78,7 +73,7 @@ __device__ __forceinline__ void issue_tile(const BnStreamArgs& a, const Geo& g, 
   bar_expect_tx(bar, by + bg);
   const YT* ysrc = reinterpret_cast<const YT*>(a.y) + (long)n * a.y_ss + (long)t0 * C;
   bulk_g2s(stage, ysrc, by, bar);
-  uint8_t* sg = stage + TILE_ELEMS * sizeof(YT);
+  uint8_t* sg = stage + Tile::ELEMS * sizeof(YT);
   const GT* gsrc = reinterpret_cast<const GT*>(a.s.A) + (long)n * a.s.a_ss +
                    (long)(t0 + a.s.padL) * a.s.a_rs;
   if (a.s.a_rs == C) {
@@ -90,10 +85,10 @@ __device__ __forceinline__ void issue_tile(const BnStreamArgs& a, const Geo& g, 
 }
 
 // APPLY = false: pass 1 (S1, S2, dalpha, amax).  APPLY = true: pass 2 (dy in format DF, db).
-template <typename YT, typename GT, int DF, bool APPLY, typename TC>
+template <typename YT, typename GT, int DF, bool APPLY>
 __global__ void __launch_bounds__(THREADS, 2)
 bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
-  constexpr int TILE_ELEMS = TC::TE, STAGES = TC::NS, ITEMS = TC::ITEMS;
+  constexpr int TILE_ELEMS = Tile::ELEMS, STAGES = Tile::STAGES, ITEMS = Tile::ITEMS;
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr int STAGE_BYTES = TILE_ELEMS * (sizeof(YT) + sizeof(GT));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
@@ -118,7 +113,7 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       const long tile = first + (long)s * stride;
-      if (tile < g.total) issue_tile<YT, GT, TILE_ELEMS>(a, g, tile, smem + s * STAGE_BYTES, &bars[s]);
+      if (tile < g.total) issue_tile<YT, GT>(a, g, tile, smem + s * STAGE_BYTES, &bars[s]);
     }
   }
   float gs_scale = 1.f;
@@ -275,7 +270,7 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
     __syncthreads();                               // every thread is done with this stage
     if (tid == 0) {
       const long nxt = tile + (long)STAGES * stride;
-      if (nxt < g.total) issue_tile<YT, GT, TILE_ELEMS>(a, g, nxt, smem + stage * STAGE_BYTES, &bars[stage]);
+      if (nxt < g.total) issue_tile<YT, GT>(a, g, nxt, smem + stage * STAGE_BYTES, &bars[stage]);
     }
     if (++stage == STAGES) {
       stage = 0;
@@ -320,20 +315,21 @@ bn_bwd_stream_kernel(const BnStreamArgs a, const Geo g) {
   }
 }
 
-template <typename YT, typename GT, int DF, bool APPLY, typename TC>
-int launch_cfg(const BnStreamArgs& a, const BnStreamPlan& p, cudaStream_t st) {
+template <typename YT, typename GT, int DF, bool APPLY>
+int launch(const BnStreamArgs& a, cudaStream_t st) {
+  const BnStreamPlan p = pase_bn_stream_plan(a);
   Geo g;
   g.TT = p.TT;
   g.tps = p.tps;
   g.total = p.total;
-  const size_t smem = (size_t)TC::NS * TC::TE * (sizeof(YT) + sizeof(GT)) +
-                      TC::NS * sizeof(uint64_t) + (size_t)3 * a.C * sizeof(double) +
+  const size_t smem = (size_t)Tile::STAGES * Tile::ELEMS * (sizeof(YT) + sizeof(GT)) +
+                      Tile::STAGES * sizeof(uint64_t) + (size_t)3 * a.C * sizeof(double) +
                       2 * sizeof(float);
-  auto kern = bn_bwd_stream_kernel<YT, GT, DF, APPLY, TC>;
+  auto kern = bn_bwd_stream_kernel<YT, GT, DF, APPLY>;
   static bool attr_done = false;
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(TC::NS * TC::TE * 8 + 64 + 3 * 1024 * 8 + 8));
+                                         (int)(Tile::STAGES * Tile::ELEMS * 8 + 64 + 3 * 1024 * 8 + 8));
     if (e != cudaSuccess) {
       pase_set_error("bn_stream: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
       return (int)e;
@@ -349,35 +345,9 @@ int launch_cfg(const BnStreamArgs& a, const BnStreamPlan& p, cudaStream_t st) {
   return PASE_OK;
 }
 
-int tile_elems() {
-  static int v = 0;
-  if (v == 0) {
-    const char* e = getenv("PASE_B200_BN_TILE");
-    v = (e && atoi(e) == 2048) ? 2048 : 4096;
-  }
-  return v;
-}
-
-template <typename YT, typename GT, int DF, bool APPLY>
-int launch(const BnStreamArgs& a, cudaStream_t st) {
-  const BnStreamPlan p = pase_bn_stream_plan(a);
-  if (p.TE == 2048) return launch_cfg<YT, GT, DF, APPLY, TileCfg<2048, 6>>(a, p, st);
-  return launch_cfg<YT, GT, DF, APPLY, TileCfg<4096, 3>>(a, p, st);
-}
-
-bool stream_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("PASE_B200_BN_STREAM");
-    v = (e && atoi(e) == 0) ? 0 : 1;
-  }
-  return v == 1;
-}
-
 }  // namespace
 
 bool pase_bn_stream_ok(const BnStreamArgs& a) {
-  if (!stream_enabled()) return false;
   const int C = a.C;
   if (C < 32 || C > 1024 || (C & (C - 1)) != 0) return false;       // C/4 must divide 256
   if (a.a_bf16 && !a.y_bf16) return false;
@@ -396,8 +366,7 @@ bool pase_bn_stream_ok(const BnStreamArgs& a) {
 
 BnStreamPlan pase_bn_stream_plan(const BnStreamArgs& a) {
   BnStreamPlan p;
-  p.TE = (tile_elems() == 2048 && a.C <= 512) ? 2048 : 4096;
-  p.TT = p.TE / a.C;
+  p.TT = Tile::ELEMS / a.C;
   p.tps = (a.T + p.TT - 1) / p.TT;
   p.total = (long)a.N * p.tps;
   p.grid = 2L * pase_num_sms();

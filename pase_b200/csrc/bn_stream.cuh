@@ -21,9 +21,9 @@ struct BnStreamArgs {
   void *dst, *dst_lo; int dst_fmt; long d_ss; double* dbias; float* scale_out;
 };
 
-// how the staged kernels cut a call: TE elements per tile and tensor (TT = TE / C time steps),
-// tps tiles per sample, total = N * tps tiles, shared by grid persistent blocks
-struct BnStreamPlan { int TE, TT, tps; long total, grid; };
+// how the staged kernels cut a call: tiles of TT = 4096 / C time steps, tps tiles per sample,
+// total = N * tps tiles, shared by grid persistent blocks
+struct BnStreamPlan { int TT, tps; long total, grid; };
 
 // true when the staged kernels support the shape / alignment (else: register kernels)
 bool pase_bn_stream_ok(const BnStreamArgs& a);
