@@ -238,6 +238,10 @@ int pase_sinc_dgrad_weight(const float* filt, float* Wdg, int C, int k, int fold
  * + [T-1-padR<=t<=T-2] dpad[n,padL+2(T-1)-t]  (dpad rows of pitch `pitch`, dx (N,T) fp32) */
 int pase_reflect_fold_wave(const float* dpad, long pitch, float* dx, int N, int T, int padL,
                            int padR, void* stream);
+/* Packed form of pase_reflect_fold_wave: tab (DEVICE, nseg rows of 3 ints) {x_off, T, dst_off}
+ * (pase_reflect_pad_wave_var's table): dx[x_off + t] from dpad[dst_off ..]; max_T >= every T. */
+int pase_reflect_fold_wave_var(const float* dpad, const int* tab, int nseg, int max_T, float* dx,
+                               int padL, int padR, void* stream);
 /* batch statistics -> per-channel affine; updates running stats (training) */
 int pase_bn_finalize(const double* colsum, const double* colsumsq, int C, int fold,
                      double count, const float* gamma, const float* beta,
@@ -312,6 +316,32 @@ int pase_bn_prelu_bwd_apply_src(const void* y, int y_bf16, long y_sample_stride,
                                 void* dst, void* dst_lo, int dst_fmt, long dst_sample_stride,
                                 double* dbias_acc, const float* amax, float* scale_out,
                                 void* stream);
+/* Packed variable-length forms of the two passes above in eval mode (WaveFe.encode_packed,
+ * DESIGN.md section 18).  tab (DEVICE, nseg rows of 9 ints) {T, y_off, a_off, b_off, pool_off,
+ * pool_d, pool_T, d_off, d_span}: utterance i is a B=1 call with y + y_off, srcA + a_off,
+ * srcB + b_off, pool + pool_off (element offsets; the sample strides unused), so its gradient
+ * sources are summed as in the uniform kernels.  max_T >= every T.
+ * pase_bn_prelu_bwd_reduce_var: pase_bn_prelu_bwd_reduce's sums and maxima over all utterances.
+ * pase_bn_prelu_bwd_apply_src_var: pase_bn_prelu_bwd_apply_src with S1 = S2 = 0 (dy = gamma
+ * invstd du); utterance i's frame t goes to dst[d_off + t*C ..] (dst rows of C elements), frames
+ * T .. d_span-1 after it are written zero and so are the `lead` frames before the first
+ * utterance, on every call; max_span >= every d_span.  The fp16-pair scale comes from amax over
+ * the whole pack.  dbias_acc (may be NULL) += sum dy. */
+int pase_bn_prelu_bwd_reduce_var(const void* y, int y_bf16, const int* tab, int nseg, int max_T,
+                                 int C, const float* mean, const float* invstd,
+                                 const float* scale, const float* shift, const float* alpha,
+                                 const void* srcA, int a_bf16, long a_row_stride, int padL,
+                                 int padR, const float* srcB, long b_row_stride, int b_shift,
+                                 const float* pool, long pool_row_stride, double* S1, double* S2,
+                                 double* dalpha, float* amax, void* stream);
+int pase_bn_prelu_bwd_apply_src_var(const void* y, int y_bf16, const int* tab, int nseg,
+                                    int max_span, int C, const float* invstd, const float* gamma,
+                                    const float* scale, const float* shift, const float* alpha,
+                                    const void* srcA, int a_bf16, long a_row_stride, int padL,
+                                    int padR, const float* srcB, long b_row_stride, int b_shift,
+                                    const float* pool, long pool_row_stride, void* dst,
+                                    void* dst_lo, int dst_fmt, int lead, double* dbias_acc,
+                                    const float* amax, float* scale_out, void* stream);
 /* The three backward entry points above read and write y, srcA, srcB, pool, dst, dst_lo and du
  * in quads of channels: fp32 operands must be 16-byte aligned, 16-bit ones 8-byte aligned,
  * every row and sample stride a multiple of 4 elements, a/b_row_stride >= C and
@@ -366,6 +396,11 @@ int pase_out_select(float* out, long T, int C, int mode, void* stream);
 int pase_out_bwd_reduce(const float* dout, const float* dout_ntc, const float* y,
                         const float* mean, const float* invstd, int N, int T, int C,
                         float* g_ntc, double* S1, double* S2, void* stream);
+/* Packed form of pase_out_bwd_reduce's layout change (eval mode: no statistics): tab (DEVICE,
+ * nseg rows of 3 ints) {row0, T, o_off}: g_ntc[(row0 + t)*C + c] = dout[o_off + c*T + t];
+ * max_T >= every T. */
+int pase_out_bwd_gather_var(const float* dout, const int* tab, int nseg, int max_T, int C,
+                            float* g_ntc, void* stream);
 /* in place: g = scale*(g - use_stats*(S1/M + xhat*S2/M)) */
 int pase_out_bwd_apply(float* g, const float* y, const float* mean, const float* invstd,
                        const float* scale, const double* S1, const double* S2,
@@ -395,6 +430,13 @@ int pase_qrnn_scan_fwd_carry_var(const float* Y, float* h, long ldh, float* Cst,
                                  const int* tab, int nseg, int H, void* stream);
 int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long lddh,
                        float* dY, int N, int T, int H, void* stream);
+/* Packed variable-length form of pase_qrnn_scan_bwd: tab (DEVICE, nseg rows of 3 ints)
+ * {row0, T, drow0}: rows row0 .. row0+T-1 of Y / Cst / dh are one utterance; its gate gradients
+ * go to rows drow0 .. drow0+T-1 of dY and row drow0+T of dY is written zero.  Each utterance
+ * runs the kernel its own T selects (pase_qrnn_scan_plan), so it gets a B=1 backward's bits.
+ * Two launches. */
+int pase_qrnn_scan_bwd_var(const float* Y, const float* Cst, const float* dh, long lddh, float* dY,
+                           const int* tab, int nseg, int H, void* stream);
 /* Which kernels the two scans run for T time steps (host only, launches nothing): out1 =
  * segments per block of the time-segmented kernels (16, 24 or 32; T <= 512), or 0 for the
  * sequential kernels (T > 512). */

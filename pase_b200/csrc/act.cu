@@ -624,6 +624,245 @@ bn_prelu_bwd_apply_src_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
   }
 }
 
+// ---- packed variable-length backward (eval BatchNorm; pase_bn_prelu_bwd_*_var) ----
+// Table row (ints) of utterance blockIdx.y: {T, y_off, a_off, b_off, pool_off, pool_d, pool_T,
+// d_off, d_span}.  The gradient sources of one utterance are those of a B=1 call at the row's
+// offsets, so load_grad_run (n = 0) gives the uniform kernels' sums in their order.
+constexpr int BWD_ROW = 9;
+
+template <typename GT>
+__device__ __forceinline__ BwdSrc var_src(const int* r, const void* A, long a_rs, int padL,
+                                          int padR, const float* B, long b_rs, int b_shift,
+                                          const float* pool, long p_rs) {
+  BwdSrc s;
+  s.A = reinterpret_cast<const GT*>(A) + __ldg(r + 2); s.a_ss = 0; s.a_rs = a_rs;
+  s.padL = padL; s.padR = padR;
+  s.B = B ? B + __ldg(r + 3) : nullptr; s.b_ss = 0; s.b_rs = b_rs; s.b_shift = b_shift;
+  s.P = pool ? pool + __ldg(r + 4) : nullptr; s.p_ss = 0; s.p_rs = p_rs;
+  s.pool_d = pool ? __ldg(r + 5) : 0; s.pool_T = __ldg(r + 6);
+  return s;
+}
+
+// pass 1 of pase_bn_prelu_bwd_reduce for every utterance: S1, S2, dalpha and the maxima
+template <typename YT, typename GT>
+__global__ void __launch_bounds__(THREADS)
+bn_prelu_bwd_reduce_var_kernel(const YT* __restrict__ y, const int* __restrict__ tab, int C,
+                               const float* __restrict__ mean, const float* __restrict__ invstd,
+                               const float* __restrict__ scale, const float* __restrict__ shift,
+                               const float* __restrict__ alpha, const void* A, long a_rs,
+                               int padL, int padR, const float* B, long b_rs, int b_shift,
+                               const float* pool, long p_rs, double* __restrict__ S1,
+                               double* __restrict__ S2, double* __restrict__ dalpha,
+                               float* __restrict__ amax) {
+  pdl_wait();
+  extern __shared__ double red[];
+  float* redm = reinterpret_cast<float*>(red + 3 * C);
+  for (int i = threadIdx.x; i < 3 * C; i += blockDim.x) red[i] = 0.0;
+  if (threadIdx.x < 2) redm[threadIdx.x] = 0.f;
+  __syncthreads();
+  const int* r = tab + BWD_ROW * blockIdx.y;
+  const int T = __ldg(r);
+  const BwdSrc s = var_src<GT>(r, A, a_rs, padL, padR, B, b_rs, b_shift, pool, p_rs);
+  const int C4 = C >> 2;
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long nthreads = (long)C4 * ((T + RUN - 1) / RUN);
+  const int c = (int)(idx % C4) * 4;
+  float a1[4] = {0, 0, 0, 0}, a2[4] = {0, 0, 0, 0}, a3[4] = {0, 0, 0, 0};
+  float mx_du = 0.f, mx_xh = 0.f;
+  if (idx < nthreads) {
+    const YT* yn = y + __ldg(r + 1);
+    const long t0 = (idx / C4) * RUN;
+    const int nvalid = (T - (int)t0) < RUN ? (T - (int)t0) : RUN;
+    float4 gs[RUN], ys[RUN];
+#pragma unroll
+    for (int i = 0; i < RUN; ++i) ys[i] = ld4t(yn + (long)((int)t0 + (i < nvalid ? i : 0)) * C + c);
+    load_grad_run<GT>(s, 0, T, t0, nvalid, c, gs);
+#pragma unroll
+    for (int i = 0; i < RUN; ++i) {
+      if (i >= nvalid) break;
+      const float gg[4] = {gs[i].x, gs[i].y, gs[i].z, gs[i].w};
+      const float vv[4] = {ys[i].x, ys[i].y, ys[i].z, ys[i].w};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float u = fmaf(vv[k], scale[c + k], shift[c + k]);
+        const bool pos = u > 0.f;
+        const float du = pos ? gg[k] : alpha[c + k] * gg[k];
+        a3[k] += pos ? 0.f : u * gg[k];
+        const float xh = (vv[k] - mean[c + k]) * invstd[c + k];
+        a1[k] += du;
+        a2[k] += du * xh;
+        mx_du = fmaxf(mx_du, fabsf(du));
+        mx_xh = fmaxf(mx_xh, fabsf(xh));
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      atomicAdd(&red[0 * C + c + k], (double)a1[k]);
+      atomicAdd(&red[1 * C + c + k], (double)a2[k]);
+      atomicAdd(&red[2 * C + c + k], (double)a3[k]);
+    }
+  }
+  if (amax != nullptr) {
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) {
+      mx_du = fmaxf(mx_du, __shfl_xor_sync(0xffffffffu, mx_du, off));
+      mx_xh = fmaxf(mx_xh, __shfl_xor_sync(0xffffffffu, mx_xh, off));
+    }
+    if ((threadIdx.x & 31) == 0) {
+      atomic_max_pos(&redm[0], mx_du);
+      atomic_max_pos(&redm[1], mx_xh);
+    }
+  }
+  __syncthreads();
+  if ((long)blockIdx.x * blockDim.x < nthreads) {
+    for (int i = threadIdx.x; i < C; i += blockDim.x) {
+      atomicAdd(S1 + i, red[0 * C + i]);
+      atomicAdd(S2 + i, red[1 * C + i]);
+      atomicAdd(dalpha + i, red[2 * C + i]);
+    }
+  }
+  if (amax != nullptr && threadIdx.x == 0) {
+    atomic_max_pos(amax, redm[0]);
+    atomic_max_pos(amax + 1, redm[1]);
+  }
+}
+
+template <int DF>
+__device__ __forceinline__ void store_grad4(void* dst_v, void* dst_lo_v, long off, float4 o,
+                                            float gs_scale) {
+  if constexpr (DF == PASE_FMT_F32) {
+    st4(reinterpret_cast<float*>(dst_v) + off, o);
+    if (dst_lo_v != nullptr)
+      st4(reinterpret_cast<float*>(dst_lo_v) + off,
+          make_float4(tf32_residual(o.x), tf32_residual(o.y), tf32_residual(o.z),
+                      tf32_residual(o.w)));
+  } else if constexpr (DF == PASE_FMT_BF16) {
+    st4t(reinterpret_cast<__nv_bfloat16*>(dst_v) + off, o);
+  } else {
+    st4_f16x2(reinterpret_cast<__half*>(dst_v) + off, reinterpret_cast<__half*>(dst_lo_v) + off,
+              make_float4(o.x * gs_scale, o.y * gs_scale, o.z * gs_scale, o.w * gs_scale));
+  }
+}
+
+// pass 2 of pase_bn_prelu_bwd_apply_src in eval mode (S1 = S2 = 0: dy = gamma invstd du) for
+// every utterance, into frames d_off/C + f of dst, f < d_span: the utterance's T frames, zeros
+// in [T, d_span) and, for the first utterance, zeros in the `lead` frames before it.  Work item
+// j < C/4 * ceil(T/RUN) computes a run; the others write the zero frames.
+template <typename YT, typename GT, int DF>
+__global__ void __launch_bounds__(THREADS)
+bn_prelu_bwd_apply_src_var_kernel(const YT* __restrict__ y, const int* __restrict__ tab, int C,
+                                  const float* __restrict__ invstd,
+                                  const float* __restrict__ gamma,
+                                  const float* __restrict__ scale, const float* __restrict__ shift,
+                                  const float* __restrict__ alpha, const void* A, long a_rs,
+                                  int padL, int padR, const float* B, long b_rs, int b_shift,
+                                  const float* pool, long p_rs, void* dst_v, void* dst_lo_v,
+                                  int lead, double* __restrict__ dbias,
+                                  const float* __restrict__ amax, float* __restrict__ scale_out) {
+  pdl_wait();
+  extern __shared__ double red[];
+  float* redm = reinterpret_cast<float*>(red + C);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) red[i] = 0.0;
+  if (threadIdx.x == 0) redm[0] = 0.f;
+  __syncthreads();
+  float gs_scale = 1.f;
+  if constexpr (DF == PASE_FMT_F16X2) {     // pase_bn_prelu_bwd_apply_src's bound, S1 = S2 = 0
+    const float mdu = amax[0];
+    float b = 0.f;
+    for (int i = threadIdx.x; i < C; i += blockDim.x)
+      b = fmaxf(b, fabsf((gamma ? gamma[i] : 1.f) * invstd[i]) * mdu);
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, off));
+    if ((threadIdx.x & 31) == 0) atomic_max_pos(&redm[0], b);
+    __syncthreads();
+    gs_scale = f16_grad_scale(redm[0] * 1.0001f);
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
+      scale_out[0] = 1.f / gs_scale;
+      scale_out[1] = gs_scale;
+    }
+  }
+  const int* r = tab + BWD_ROW * blockIdx.y;
+  const int T = __ldg(r);
+  const long d_off = __ldg(r + 7);
+  const int span = __ldg(r + 8), pre = blockIdx.y == 0 ? lead : 0;
+  const int C4 = C >> 2;
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int c = (int)(idx % C4) * 4;
+  const long run = idx / C4;
+  const long nruns = (T + RUN - 1) / RUN;
+  float acc[4] = {0, 0, 0, 0};
+  if (run < nruns) {
+    const BwdSrc s = var_src<GT>(r, A, a_rs, padL, padR, B, b_rs, b_shift, pool, p_rs);
+    const YT* yn = y + __ldg(r + 1);
+    const long t0 = run * RUN;
+    const int nvalid = (T - (int)t0) < RUN ? (T - (int)t0) : RUN;
+    float4 vs[RUN], gs[RUN];
+#pragma unroll
+    for (int i = 0; i < RUN; ++i) vs[i] = ld4t(yn + (long)((int)t0 + (i < nvalid ? i : 0)) * C + c);
+    load_grad_run<GT>(s, 0, T, t0, nvalid, c, gs);
+    float gi[4], scv[4], shv[4], alv[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      gi[k] = (gamma ? gamma[c + k] : 1.f) * invstd[c + k];
+      scv[k] = scale[c + k];
+      shv[k] = shift[c + k];
+      alv[k] = alpha[c + k];
+    }
+#pragma unroll
+    for (int i = 0; i < RUN; ++i) {
+      if (i >= nvalid) break;
+      const float vv[4] = {vs[i].x, vs[i].y, vs[i].z, vs[i].w};
+      const float gg[4] = {gs[i].x, gs[i].y, gs[i].z, gs[i].w};
+      float o[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float u = fmaf(vv[k], scv[k], shv[k]);
+        const float du = u > 0.f ? gg[k] : alv[k] * gg[k];
+        o[k] = gi[k] * du;
+        acc[k] += o[k];
+      }
+      store_grad4<DF>(dst_v, dst_lo_v, d_off + ((long)t0 + i) * C + c,
+                      make_float4(o[0], o[1], o[2], o[3]), gs_scale);
+    }
+    if (dbias) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) atomicAdd(&red[c + k], (double)acc[k]);
+    }
+  } else {
+    // zero frames: [T, span), then [-pre, 0)
+    const long z0 = (run - nruns) * RUN, tail = span - T;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int i = 0; i < RUN; ++i) {
+      const long j = z0 + i;
+      const long f = j < tail ? T + j : j - tail - pre;
+      if (j < tail + pre) store_grad4<DF>(dst_v, dst_lo_v, d_off + f * C + c, zero, gs_scale);
+    }
+  }
+  if (dbias) {
+    __syncthreads();
+    if ((long)blockIdx.x * blockDim.x < (long)C4 * nruns)
+      for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, red[i]);
+  }
+}
+
+// g[row0 + t, c] = dout[o_off + c T + t] for tab rows {row0, T, o_off} (pase_out_bwd_reduce's
+// layout change, one utterance per blockIdx.y)
+__global__ void __launch_bounds__(256)
+out_bwd_gather_var_kernel(const float* __restrict__ dout, const int* __restrict__ tab, int C,
+                          float* __restrict__ g) {
+  pdl_wait();
+  const int* r = tab + 3 * blockIdx.y;
+  const long row0 = __ldg(r), o = __ldg(r + 2);
+  const int T = __ldg(r + 1);
+  const long total = (long)T * C;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i / T), t = (int)(i - (long)c * T);
+    g[(row0 + t) * C + c] = dout[o + i];
+  }
+}
+
 // ---- plain PReLU on (rows, C) ----
 __global__ void prelu_fwd_kernel(const float* __restrict__ u, float* __restrict__ h,
                                  const float* __restrict__ alpha, long rows, int C, long ldu,
@@ -1541,6 +1780,124 @@ int pase_scale_dev(float* x, long n, const float* dev_scalar, float host_coef, v
   scale_dev_kernel<<<blocks_for(n, 256), 256, 0, (cudaStream_t)stream>>>(x, n, dev_scalar,
                                                                         host_coef);
   PASE_LAUNCH_CHECK("pase_scale_dev");
+  return PASE_OK;
+}
+
+// ---- packed variable-length backward ------------------------------------------------------
+static int bn_bwd_var_check(const char* fn, const void* y, int y_bf16, const int* tab, int nseg,
+                            int max_T, int C, const void* srcA, int a_bf16, long a_row_stride,
+                            const float* srcB, long b_row_stride, const float* pool,
+                            long pool_row_stride) {
+  PASE_CHECK_ARG(y && tab && srcA, "%s: null pointer", fn);
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535 && max_T > 0 && C > 0 && (C % 4) == 0 && C <= 4096,
+                 "%s: nseg=%d max_T=%d C=%d", fn, nseg, max_T, C);
+  PASE_CHECK_ARG(!a_bf16 || y_bf16, "%s: bf16 srcA needs bf16 y", fn);
+  PASE_CHECK_QUAD(fn, y, y_bf16 ? 2 : 4, "y");
+  PASE_CHECK_QUAD(fn, srcA, a_bf16 ? 2 : 4, "srcA");
+  PASE_CHECK_STRIDE(fn, a_row_stride, "a_row_stride");
+  PASE_CHECK_ARG(a_row_stride >= C, "%s: a_row_stride < C", fn);
+  if (srcB) {
+    PASE_CHECK_QUAD(fn, srcB, 4, "srcB");
+    PASE_CHECK_STRIDE(fn, b_row_stride, "b_row_stride");
+  }
+  if (pool) {
+    PASE_CHECK_QUAD(fn, pool, 4, "pool");
+    PASE_CHECK_STRIDE(fn, pool_row_stride, "pool_row_stride");
+  }
+  return PASE_OK;
+}
+
+int pase_bn_prelu_bwd_reduce_var(const void* y, int y_bf16, const int* tab, int nseg, int max_T,
+                                 int C, const float* mean, const float* invstd,
+                                 const float* scale, const float* shift, const float* alpha,
+                                 const void* srcA, int a_bf16, long a_row_stride, int padL,
+                                 int padR, const float* srcB, long b_row_stride, int b_shift,
+                                 const float* pool, long pool_row_stride, double* S1, double* S2,
+                                 double* dalpha, float* amax, void* stream) {
+  const char* fn = "pase_bn_prelu_bwd_reduce_var";
+  PASE_CHECK_ARG(mean && invstd && scale && shift && alpha && S1 && S2 && dalpha,
+                 "%s: null pointer", fn);
+  const int rc = bn_bwd_var_check(fn, y, y_bf16, tab, nseg, max_T, C, srcA, a_bf16,
+                                  a_row_stride, srcB, b_row_stride, pool, pool_row_stride);
+  if (rc != PASE_OK) return rc;
+  const long items = (long)(C / 4) * ((max_T + RUN - 1) / RUN);
+  dim3 grid((unsigned)((items + THREADS - 1) / THREADS), nseg);
+  const size_t sm = 3 * C * sizeof(double) + 2 * sizeof(float);
+  cudaStream_t st = (cudaStream_t)stream;
+#define PASE_REDV(YT, GT)                                                                     \
+  do {                                                                                        \
+    if (sm > 48 * 1024)                                                                       \
+      cudaFuncSetAttribute(bn_prelu_bwd_reduce_var_kernel<YT, GT>,                            \
+                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);             \
+    PASE_LAUNCH((bn_prelu_bwd_reduce_var_kernel<YT, GT>), grid, THREADS, sm, st,              \
+                reinterpret_cast<const YT*>(y), tab, C, mean, invstd, scale, shift, alpha,    \
+                srcA, a_row_stride, padL, padR, srcB, b_row_stride, b_shift, pool,            \
+                pool_row_stride, S1, S2, dalpha, amax);                                       \
+  } while (0)
+  if (y_bf16) {
+    if (a_bf16) PASE_REDV(__nv_bfloat16, __nv_bfloat16);
+    else PASE_REDV(__nv_bfloat16, float);
+  } else {
+    PASE_REDV(float, float);
+  }
+#undef PASE_REDV
+  PASE_LAUNCH_CHECK(fn);
+  return PASE_OK;
+}
+
+int pase_bn_prelu_bwd_apply_src_var(const void* y, int y_bf16, const int* tab, int nseg,
+                                    int max_span, int C, const float* invstd, const float* gamma,
+                                    const float* scale, const float* shift, const float* alpha,
+                                    const void* srcA, int a_bf16, long a_row_stride, int padL,
+                                    int padR, const float* srcB, long b_row_stride, int b_shift,
+                                    const float* pool, long pool_row_stride, void* dst,
+                                    void* dst_lo, int dst_fmt, int lead, double* dbias_acc,
+                                    const float* amax, float* scale_out, void* stream) {
+  const char* fn = "pase_bn_prelu_bwd_apply_src_var";
+  PASE_CHECK_ARG(invstd && scale && shift && alpha && dst && lead >= 0, "%s: null pointer / lead",
+                 fn);
+  const int rc = bn_bwd_var_check(fn, y, y_bf16, tab, nseg, max_span, C, srcA, a_bf16,
+                                  a_row_stride, srcB, b_row_stride, pool, pool_row_stride);
+  if (rc != PASE_OK) return rc;
+  PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2, "%s: bad dst_fmt %d", fn, dst_fmt);
+  PASE_CHECK_ARG(dst_fmt != PASE_FMT_F16X2 || (dst_lo && amax && scale_out && !y_bf16),
+                 "%s: the fp16-pair format needs dst_lo, amax, scale_out and fp32 y", fn);
+  PASE_CHECK_ARG((dst_fmt == PASE_FMT_BF16) == (y_bf16 != 0),
+                 "%s: bf16 y goes with bf16 dst (and only with it)", fn);
+  PASE_CHECK_QUAD(fn, dst, dst_fmt == PASE_FMT_F32 ? 4 : 2, "dst");
+  // runs of the T frames + zero runs of [T, span) and the lead: at most this many per row
+  const long items = (long)(C / 4) * ((max_span + RUN - 1) / RUN + (lead + RUN - 1) / RUN + 1);
+  dim3 grid((unsigned)((items + THREADS - 1) / THREADS), nseg);
+  const size_t sm = C * sizeof(double) + sizeof(float);
+  cudaStream_t st = (cudaStream_t)stream;
+#define PASE_APSV(YT, GT, DF)                                                                  \
+  PASE_LAUNCH((bn_prelu_bwd_apply_src_var_kernel<YT, GT, DF>), grid, THREADS, sm, st,          \
+              reinterpret_cast<const YT*>(y), tab, C, invstd, gamma, scale, shift, alpha, srcA, \
+              a_row_stride, padL, padR, srcB, b_row_stride, b_shift, pool, pool_row_stride,     \
+              dst, dst_lo, lead, dbias_acc, amax, scale_out)
+  if (dst_fmt == PASE_FMT_BF16) {
+    if (a_bf16) PASE_APSV(__nv_bfloat16, __nv_bfloat16, PASE_FMT_BF16);
+    else PASE_APSV(__nv_bfloat16, float, PASE_FMT_BF16);
+  } else if (dst_fmt == PASE_FMT_F16X2) {
+    PASE_APSV(float, float, PASE_FMT_F16X2);
+  } else {
+    PASE_APSV(float, float, PASE_FMT_F32);
+  }
+#undef PASE_APSV
+  PASE_LAUNCH_CHECK(fn);
+  return PASE_OK;
+}
+
+int pase_out_bwd_gather_var(const float* dout, const int* tab, int nseg, int max_T, int C,
+                            float* g_ntc, void* stream) {
+  PASE_CHECK_ARG(dout && tab && g_ntc && nseg > 0 && nseg <= 65535 && max_T > 0 && C > 0,
+                 "pase_out_bwd_gather_var: bad args");
+  const long total = (long)max_T * C;
+  long bx = (total + 255) / 256;
+  if (bx > 1024) bx = 1024;
+  PASE_LAUNCH((out_bwd_gather_var_kernel), dim3((unsigned)bx, nseg), 256, 0, (cudaStream_t)stream,
+              dout, tab, C, g_ntc);
+  PASE_LAUNCH_CHECK("pase_out_bwd_gather_var");
   return PASE_OK;
 }
 

@@ -70,6 +70,23 @@ reflect_fold_wave_kernel(const float* __restrict__ dpad, long pitch, float* __re
   }
 }
 
+// pase_reflect_fold_wave for utterance blockIdx.y of a packed waveform: tab row {x_off, T, dst_off}
+__global__ void __launch_bounds__(THREADS)
+reflect_fold_wave_var_kernel(const float* __restrict__ dpad, const int* __restrict__ tab,
+                             float* __restrict__ dx, int padL, int padR) {
+  pdl_wait();
+  const int* r = tab + 3 * blockIdx.y;
+  const int T = __ldg(r + 1);
+  const float* d = dpad + __ldg(r + 2);
+  float* o = dx + __ldg(r);
+  for (int t = blockIdx.x * THREADS + threadIdx.x; t < T; t += gridDim.x * THREADS) {
+    float v = d[t + padL];
+    if (t >= 1 && t <= padL) v += d[padL - t];                               // left mirror
+    if (t >= T - 1 - padR && t <= T - 2) v += d[padL + 2 * (T - 1) - t];     // right mirror
+    o[t] = v;
+  }
+}
+
 inline unsigned grid_for(long total) {
   long b = (total + THREADS - 1) / THREADS;
   const long cap = (long)pase_num_sms() * 16;
@@ -133,5 +150,16 @@ int pase_reflect_fold_wave(const float* dpad, long pitch, float* dx, int N, int 
   PASE_LAUNCH((reflect_fold_wave_kernel), grid, THREADS, 0, (cudaStream_t)stream, dpad, pitch, dx,
               T, padL, padR);
   PASE_LAUNCH_CHECK("pase_reflect_fold_wave");
+  return PASE_OK;
+}
+
+int pase_reflect_fold_wave_var(const float* dpad, const int* tab, int nseg, int max_T, float* dx,
+                               int padL, int padR, void* stream) {
+  PASE_CHECK_ARG(dpad && tab && dx && nseg > 0 && nseg <= 65535 && max_T > 0 && padL >= 0 &&
+                     padR >= 0, "pase_reflect_fold_wave_var: bad args");
+  dim3 grid((unsigned)((max_T + THREADS - 1) / THREADS), nseg);
+  PASE_LAUNCH((reflect_fold_wave_var_kernel), grid, THREADS, 0, (cudaStream_t)stream, dpad, tab,
+              dx, padL, padR);
+  PASE_LAUNCH_CHECK("pase_reflect_fold_wave_var");
   return PASE_OK;
 }

@@ -296,6 +296,135 @@ qrnn_scan_fwd_seq_var_kernel(const float* __restrict__ Y, float* __restrict__ h,
   qrnn_fwd_seq(Y + row0 * 3 * H + c, h + row0 * ldh + c, ldh, Cst + row0 * H + c, T, H, 0.f);
 }
 
+// Packed variable-length backward: blockIdx.y = utterance, tab row {row0, T, drow0}: rows row0 ..
+// row0+T-1 of Y / Cst / dh are one utterance, its gate gradients go to rows drow0 .. drow0+T-1
+// of dY and row drow0+T of dY is written zero (the QRNN input's rows, one separator row per
+// utterance: DESIGN.md section 18).  As in the forward, each utterance runs the kernel its own T
+// selects, with the arithmetic of qrnn_scan_bwd_seg_kernel / qrnn_scan_bwd_kernel.
+__global__ void __launch_bounds__(32 * MAX_SEGS, 1)
+qrnn_scan_bwd_seg_var_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
+                             const float* __restrict__ dh, long lddh, float* __restrict__ dY,
+                             const int* __restrict__ tab, int H) {
+  pdl_wait();
+  __shared__ float sA[MAX_SEGS][33], sB[MAX_SEGS][33];
+  const int* r = tab + 3 * blockIdx.y;
+  const int T = __ldg(r + 1);
+  if (T > SEG * MAX_SEGS) return;
+  const long row0 = __ldg(r), drow0 = __ldg(r + 2);
+  const int lane = threadIdx.x, seg = threadIdx.y, nseg = blockDim.y;
+  const int c = blockIdx.x * 32 + lane;
+  const bool live = c < H;
+  if (live && seg == 0) {
+    float* zr = dY + (drow0 + T) * 3 * H + c;
+    zr[0] = 0.f; zr[H] = 0.f; zr[2 * H] = 0.f;
+  }
+  const int t0 = seg * SEG;
+  const int len = (T - t0) < SEG ? (T - t0) : SEG;
+  const float* y = Y + (row0 + t0) * 3 * H + c;
+  const float* cp = Cst + (row0 + t0) * H + c;
+  const float* dhp = dh + (row0 + t0) * lddh + c;
+  float* dy = dY + (drow0 + t0) * 3 * H + c;
+  float z[SEG], f[SEG], o[SEG], cs[SEG], g[SEG];
+#pragma unroll
+  for (int i = 0; i < SEG; ++i) {
+    const bool ok = live && i < len;
+    const float* yr = y + (long)i * 3 * H;
+    z[i] = ok ? yr[0] : 0.f;
+    f[i] = ok ? yr[H] : 0.f;
+    o[i] = ok ? yr[2 * H] : 0.f;
+    cs[i] = ok ? cp[(long)i * H] : 0.f;
+    g[i] = ok ? dhp[(long)i * lddh] : 0.f;
+  }
+  const float cm0 = (live && t0 > 0 && len > 0) ? cp[-(long)H] : 0.f;
+  float carry = 0.f, Q = 1.f;
+#pragma unroll
+  for (int i = SEG - 1; i >= 0; --i) {
+    const float zz = tanhf(z[i]), ff = sigmoidf_(f[i]), oo = sigmoidf_(o[i]);
+    const float cm = i > 0 ? cs[i - 1] : cm0;
+    const float ct = cs[i];
+    const bool in = i < len;
+    const float dc = in ? fmaf(g[i], oo, carry) : 0.f;
+    if (live && in) dy[(long)i * 3 * H + 2 * H] = g[i] * ct * oo * (1.f - oo);
+    z[i] = ff * (1.f - zz * zz);
+    f[i] = (zz - cm) * ff * (1.f - ff);
+    cs[i] = dc;
+    o[i] = Q;
+    if (in) {
+      carry = dc * (1.f - ff);
+      Q *= (1.f - ff);
+    }
+  }
+  sA[seg][lane] = Q;
+  sB[seg][lane] = carry;
+  __syncthreads();
+  float kin = 0.f;
+  for (int s2 = nseg - 1; s2 > seg; --s2) kin = sA[s2][lane] * kin + sB[s2][lane];
+  if (!live) return;
+#pragma unroll
+  for (int i = 0; i < SEG; ++i) {
+    if (i < len) {
+      const float dc = fmaf(o[i], kin, cs[i]);
+      dy[(long)i * 3 * H] = dc * z[i];
+      dy[(long)i * 3 * H + H] = dc * f[i];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(128)
+qrnn_scan_bwd_seq_var_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
+                             const float* __restrict__ dh, long lddh, float* __restrict__ dY,
+                             const int* __restrict__ tab, int H) {
+  pdl_wait();
+  const int* r = tab + 3 * blockIdx.y;
+  const int T = __ldg(r + 1);
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (T <= SEG * MAX_SEGS || c >= H) return;
+  const long row0 = __ldg(r), drow0 = __ldg(r + 2);
+  const float* y = Y + row0 * 3 * H + c;
+  const float* cp = Cst + row0 * H + c;
+  const float* dhp = dh + row0 * lddh + c;
+  float* dy = dY + drow0 * 3 * H + c;
+  dy[(long)T * 3 * H] = 0.f; dy[(long)T * 3 * H + H] = 0.f; dy[(long)T * 3 * H + 2 * H] = 0.f;
+  float carry = 0.f;
+  int t = T - 1;
+  for (; t - (UNROLL - 1) >= 0; t -= UNROLL) {
+    float z[UNROLL], f[UNROLL], o[UNROLL], c[UNROLL], cm[UNROLL], g[UNROLL];
+#pragma unroll
+    for (int i = 0; i < UNROLL; ++i) {
+      const int tt = t - i;
+      const float* yr = y + (long)tt * 3 * H;
+      z[i] = yr[0]; f[i] = yr[H]; o[i] = yr[2 * H];
+      c[i] = cp[(long)tt * H];
+      cm[i] = tt > 0 ? cp[(long)(tt - 1) * H] : 0.f;
+      g[i] = dhp[(long)tt * lddh];
+    }
+#pragma unroll
+    for (int i = 0; i < UNROLL; ++i) {
+      const int tt = t - i;
+      const float zz = tanhf(z[i]), ff = sigmoidf_(f[i]), oo = sigmoidf_(o[i]);
+      const float dc = g[i] * oo + carry;
+      carry = dc * (1.f - ff);
+      float* dr = dy + (long)tt * 3 * H;
+      dr[0] = dc * ff * (1.f - zz * zz);
+      dr[H] = dc * (zz - cm[i]) * ff * (1.f - ff);
+      dr[2 * H] = g[i] * c[i] * oo * (1.f - oo);
+    }
+  }
+  for (; t >= 0; --t) {
+    const float* yr = y + (long)t * 3 * H;
+    const float zz = tanhf(yr[0]), ff = sigmoidf_(yr[H]), oo = sigmoidf_(yr[2 * H]);
+    const float ct = cp[(long)t * H];
+    const float cm1 = t > 0 ? cp[(long)(t - 1) * H] : 0.f;
+    const float g = dhp[(long)t * lddh];
+    const float dc = g * oo + carry;
+    carry = dc * (1.f - ff);
+    float* dr = dy + (long)t * 3 * H;
+    dr[0] = dc * ff * (1.f - zz * zz);
+    dr[H] = dc * (zz - cm1) * ff * (1.f - ff);
+    dr[2 * H] = g * ct * oo * (1.f - oo);
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -373,6 +502,21 @@ int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long l
   dim3 grid((H + 127) / 128, N);
   PASE_LAUNCH((qrnn_scan_bwd_kernel), grid, 128, 0, (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
   PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd");
+  return PASE_OK;
+}
+
+int pase_qrnn_scan_bwd_var(const float* Y, const float* Cst, const float* dh, long lddh, float* dY,
+                           const int* tab, int nseg, int H, void* stream) {
+  PASE_CHECK_ARG(Y && Cst && dh && dY && tab, "pase_qrnn_scan_bwd_var: null pointer");
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535 && H > 0 && lddh >= H,
+                 "pase_qrnn_scan_bwd_var: nseg=%d H=%d lddh=%ld", nseg, H, lddh);
+  cudaStream_t st = (cudaStream_t)stream;
+  PASE_LAUNCH((qrnn_scan_bwd_seg_var_kernel), dim3((H + 31) / 32, nseg), dim3(32, MAX_SEGS), 0,
+              st, Y, Cst, dh, lddh, dY, tab, H);
+  PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd_var");
+  PASE_LAUNCH((qrnn_scan_bwd_seq_var_kernel), dim3((H + 127) / 128, nseg), 128, 0, st, Y, Cst, dh,
+              lddh, dY, tab, H);
+  PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd_var");
   return PASE_OK;
 }
 

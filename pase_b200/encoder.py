@@ -226,7 +226,17 @@ class EncoderPlan(object):
         warm-up steps and never inside a CUDA-graph capture."""
         if self.backward_ready:
             return
-        G, N, p, device = self.geoms, self.N, self.precision, self.device
+        N = self.N
+        self._alloc_backward(
+            [N * g.rows_out * g.Nn + 128 if g.sinc else N * g.Pd * g.Cout + g.taps * g.Cout + 128
+             for g in self.geoms],
+            [N * g.apad_floats for g in self.geoms], self.rows, self.rows)
+
+    def _alloc_backward(self, n_dyz, n_dxpad, rows, yg_rows):
+        """Backward buffers: each block's output gradient of n_dyz[l] elements in the GEMM
+        format, its input gradient of n_dxpad[l] (blocks > 0), `rows` output frames and `yg_rows`
+        rows of the QRNN gate gradients."""
+        G, p, device = self.geoms, self.precision, self.device
         f32 = dict(dtype=torch.float32, device=device)
         f64 = dict(dtype=torch.float64, device=device)
         opd = dict(dtype=p.dtype, device=device)
@@ -237,26 +247,23 @@ class EncoderPlan(object):
         zlo = lambda n: torch.zeros(int(n), **opd) if p.split else None
         f16x2 = p.fmt == gemm.FMT_F16X2           # gradients carry power-of-two scales
         self.dWt, self.Wd, self.dyz, self.dyz_lo, self.dxpad, self.gscale = [], [], [], [], [], []
-        for g in G:
+        for g, nd, nx in zip(G, n_dyz, n_dxpad):
             self.dWt.append(e(g.Nn * g.K))
             gs = torch.ones(2, **f32) if f16x2 else None
             self.gscale.append(gs)
             if g.sinc:
-                n_dyz = N * g.rows_out * g.Nn + 128
                 self.Wd.append(None)
                 self.dxpad.append(None)
             else:
-                n_dyz = N * g.Pd * g.Cout + g.taps * g.Cout + 128
                 self.Wd.append(e(g.s * g.Cin * g.taps * g.Cout))
-                self.dxpad.append(torch.empty(int(N * g.apad_floats), **yd) if g.idx > 0 else None)
-            self.dyz.append(zo(n_dyz))
-            self.dyz_lo.append(zlo(n_dyz))
+                self.dxpad.append(torch.empty(int(nx), **yd) if g.idx > 0 else None)
+            self.dyz.append(zo(nd))
+            self.dyz_lo.append(zlo(nd))
             self._ops[("dyz", g.idx)] = gemm.Operand(self.dyz[-1], self.dyz_lo[-1], gs)
-        rows = self.rows
         if self.rnn:
             Cq, H = self.Clast, self.H
-            self.dYg = z(rows * 3 * H + 64)
-            self.dsrc = e(rows * 2 * Cq)
+            self.dYg = z(yg_rows * 3 * H + 64)
+            self.dsrc = e(yg_rows * 2 * Cq)
             self.WqT = e(2 * Cq * 3 * H)
             self.dWq = e(3 * H * 2 * Cq)
         self.dcat = e(rows * self.Kc)
@@ -354,12 +361,12 @@ class EncoderPlan(object):
             ops.call("pase_conv_w_batch", ent[1], len(rows), start, op, dst_base, fmt)
 
     def nt(self, an, A, lda, afresh, bn, B, ldb, bfresh, C, ldc, M, N, K, alpha, bias,
-           rows_in, t_valid, rows_out, fold, cs, cq, acc, akind="act"):
+           rows_in, t_valid, rows_out, fold, cs, cq, acc, akind="act", a_n=None):
         """C = alpha * A B^T (+ bias) in the plan's precision (gemm.nt) over the operands
-        `an` / `bn` of buffers A / B."""
+        `an` / `bn` of buffers A / B (a_n: convert only the first a_n elements of A)."""
         return gemm.nt(self.precision, A, lda, A.numel(), B, ldb, C, ldc, M, N, K, alpha, bias,
                        rows_in, t_valid, rows_out, fold, cs, cq, acc, akind,
-                       lambda: self.operand(an, A, afresh, akind),
+                       lambda: self.operand(an, A, afresh, akind, a_n),
                        lambda: self.operand(bn, B, bfresh, "weight"))
 
     def nt_var(self, an, A, lda, bn, B, ldb, bfresh, C, ldc, M, N, K, bias, tab, n, fold):
@@ -370,11 +377,11 @@ class EncoderPlan(object):
                            lambda: self.operand(bn, B, bfresh, "weight"))
 
     def tn(self, an, A, lda, pitchA, offA, afresh, bn, B, ldb, pitchB, bfresh, C, ldc, I, J,
-           groups, rpg, alpha, acc, akind="grad"):
+           groups, rpg, alpha, acc, akind="grad", a_n=None):
         """C = alpha * A^T B in the plan's precision (gemm.tn)."""
         return gemm.tn(self.precision, A, lda, A.numel(), B, ldb, B.numel(), C, ldc, I, J, rpg,
                        groups, pitchA, offA, pitchB, alpha, acc, akind,
-                       lambda: self.operand(an, A, afresh, akind),
+                       lambda: self.operand(an, A, afresh, akind, a_n),
                        lambda: self.operand(bn, B, bfresh, "act"))
 
     def tensors(self):
@@ -727,11 +734,15 @@ def packed_layout(plan, lengths, geoms, mode):
     return torch.from_numpy(table.astype(np.int32)), sec, sizes
 
 
-def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None):
+def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None, layout=None):
     """Eval-mode forward of utterances packed in x (fp32, sum(lengths) samples, plan.wave):
     each one computed as a B=1 forward would.  Launches do not depend on the number of
-    utterances.  Returns the list of (1, E, T'_i) features, views of one new buffer."""
-    sz, tab = _packed_front(plan, mod, x, lengths, geoms, params, mode)
+    utterances.  Returns the list of (1, E, T'_i) features, views of one new buffer.
+    layout: the table builder (default packed_layout; packed_grad_layout also uploads the
+    backward's sections).  Every forward bumps plan.generation: a backward saved against an
+    earlier forward of the plan raises instead of reading these activations."""
+    plan.generation += 1
+    sz, tab = _packed_front(plan, mod, x, lengths, geoms, params, mode, layout)
     n = len(lengths)
     if plan.rnn:
         ops.call("pase_qrnn_scan_fwd_var", plan.Yg, plan.cat, plan.Kc, plan.Cst, tab("scan"), n,
@@ -745,11 +756,11 @@ def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None):
     return [out[o:o + E * t].view(1, E, t) for o, t in zip(sz["offsets"], sz["Tq"])]
 
 
-def _packed_front(plan, mod, x, lengths, geoms, params, mode):
+def _packed_front(plan, mod, x, lengths, geoms, params, mode, layout=None):
     """encoder_forward_packed up to the QRNN scan: every conv block, the pooled skips in
     plan.cat and (rnn configs) the gate pre-activations of every frame in plan.Yg.
     -> (sizes of packed_layout, section -> device table view)."""
-    host, sec, sz = packed_layout(plan, lengths, geoms, mode)
+    host, sec, sz = (layout or packed_layout)(plan, lengths, geoms, mode)
     plan.table[:host.numel()].copy_(host)                    # the one host-to-device copy
     tab = lambda name: plan.table[sec[name]:]
     _packed_front_launch(plan, mod, x, sz, tab, params)
@@ -816,6 +827,303 @@ def _packed_out_proj(plan, mod, params, rows):
             b_op=lambda: plan.operand("Wcat", plan.Wcat, True, "weight"))
     if plan.norm_out:
         _out_bn_eval_affine(plan, lambda name: _flat(mod.get_buffer(name)))
+
+
+# -- packed variable-length backward (DESIGN.md section 18) -----------------------------------
+_BWD_ROW = 9            # {T, y_off, a_off, b_off, pool_off, pool_d, pool_T, d_off, d_span}
+
+
+def _grad_table_size(nblk, n):
+    return nblk * _BWD_ROW * n + 3 * n
+
+
+class PackedGradPlan(PackedPlan):
+    """The PackedPlan of WaveFe.encode_packed: the forward buffers of WaveFe.extract, the
+    backward's table sections, and backward buffers sized by the capacity bounds, allocated on
+    the first differentiated call (the input-gradient ones on the first call returning dx).
+
+    Backward layout: block l's output gradient dyz[l] is the forward operand's row layout
+    shifted by `lead` zero rows (taps - 1; sinc: the dgrad halo), so utterance i's frames sit
+    at lead + row0[i] and every utterance's zero tail (P_i - T_out_i >= taps - 1 rows) is the
+    next one's leading halo.  The dgrad GEMMs then run uniform over sum(P_i) rows into the
+    forward operand's layout, and the weight-gradient GEMMs over the same rows as one
+    sequence.  The QRNN gate gradient dYg uses the QRNN input's rows: one zero row per
+    utterance where the forward reads its separator."""
+
+    def __init__(self, cfg, capacity, device, prec="fp32"):
+        super().__init__(cfg, capacity, device, prec)
+        G = self.geoms
+        n_apad, _, _ = packed_bounds(G, self.capacity, self.max_utts)
+        self.n_dxpad = n_apad
+        self.grad_rows = [na // g.lda for g, na in zip(G, n_apad)]
+        self.yg_rows = self.rows_cap + self.max_utts
+        self.n_dyz = [(R + 2 * g.dg_rows) * g.Nn + 128 if g.sinc else
+                      (R + 2 * g.taps) * g.Cout + 128 for g, R in zip(G, self.grad_rows)]
+        sizes = [("block %d output gradient" % g.idx, nd) for g, nd in zip(G, self.n_dyz)]
+        if self.rnn:
+            sizes.append(("QRNN gate gradient", self.yg_rows * 3 * self.H + 64))
+        for what, n in sizes:
+            if n >= INDEX_LIMIT:
+                raise ValueError(
+                    "a pack of %d samples needs %d elements for the %s, beyond the 32-bit indices "
+                    "of the packed kernels: split it into shorter utterances"
+                    % (self.capacity, n, what))
+        self.table = torch.zeros(_table_size(self.nblk, self.max_utts)
+                                 + _grad_table_size(self.nblk, self.max_utts),
+                                 dtype=torch.int32, device=device)
+        self.layout = None            # (sections, sizes) of the last differentiated forward
+        self.gflat = self.gzero = None
+
+    def ensure_backward(self):
+        if self.backward_ready:
+            return
+        self._alloc_backward(self.n_dyz, self.n_dxpad, self.rows_cap, self.yg_rows)
+        n = self.rows_cap * self.emb
+        self.gflat = torch.empty(n, dtype=torch.float32, device=self.device)
+        self.gzero = torch.zeros(n, dtype=torch.float32, device=self.device)
+
+    def ensure_input_grad(self):
+        self.ensure_backward()
+        if self.filt is not None:
+            return
+        g = self.geoms[0]
+        f32 = dict(dtype=torch.float32, device=self.device)
+        self.filt = torch.empty(g.Cout * g.k, **f32)
+        self.Wdg = torch.empty(g.fold * g.dg_K, **f32)
+        self.dxpad[0] = torch.empty(self.grad_rows[0] * g.fold, **f32)
+
+
+def packed_grad_layout(plan, lengths, geoms, mode=None):
+    """packed_layout plus the sections encoder_backward_packed reads: per block ("bwd", l) rows
+    of _BWD_ROW ints, and "qbwd" {row0, T, dY row0} of the QRNN scan.  Uploaded with the
+    forward's sections in one copy; the plan keeps (sections, sizes) for the backward."""
+    host, sec, sz = packed_layout(plan, lengths, geoms, mode)
+    G, n = plan.geoms, len(lengths)
+    P = np.array([[g.P for g in gi] for gi in geoms], dtype=np.int64).reshape(n, plan.nblk)
+    RO = np.array([[g.rows_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
+    TO = np.array([[g.T_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
+    cum = lambda a: np.concatenate([np.zeros((1,) + a.shape[1:], np.int64), np.cumsum(a, 0)])
+    row0, orow0 = cum(P), cum(RO)
+    Tq = TO[:, -1]
+    q0, xr0 = cum(Tq), cum(Tq + 1)
+    Kc, parts, base = plan.Kc, [host.numpy().astype(np.int64)], host.numel()
+    zero = np.zeros(n, np.int64)
+
+    def put(name, *cols):
+        sec[name] = base + sum(p.size for p in parts[1:])
+        parts.append(np.stack(cols, 1).reshape(-1))
+
+    lead = []
+    for l, g in enumerate(G):
+        C = g.Cout
+        if l + 1 < plan.nblk:
+            a, b = row0[:n, l + 1] * G[l + 1].lda, zero
+        elif plan.rnn:
+            a, b = xr0[:n] * 2 * C + C, xr0[:n] * 2 * C
+        else:
+            a, b = q0[:n] * Kc, zero
+        if g.sinc:
+            ld = g.dg_halo
+            d, span = (ld + g.fold * row0[:n, l]) * C, g.fold * P[:, l]
+        else:
+            ld = g.taps - 1
+            d, span = (ld + row0[:n, l]) * C, P[:, l]
+        lead.append(ld)
+        put(("bwd", l), TO[:, l], orow0[:n, l] * g.Nn, a, b, q0[:n] * Kc,
+            np.maximum(TO[:, l] // Tq, 1), Tq, d, span)
+    put("qbwd", q0[:n], Tq, xr0[:n])
+    table = np.concatenate(parts)
+    assert table.size <= plan.table.numel() and table.max() < INDEX_LIMIT
+    sz.update(lead=lead, total=int(sum(lengths)), lengths=[int(T) for T in lengths],
+              max_span=[int(m) for m in (np.max(P, 0) * np.array([g.fold for g in G]))])
+    plan.layout = (sec, sz)
+    return torch.from_numpy(table.astype(np.int32)), sec, sz
+
+
+def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_grads=True):
+    """Backward of the last packed_grad_layout forward on `plan` (eval mode), the packed mirror
+    of encoder_backward_steps.  gflat: the upstream gradients of the (1, emb, T'_i) outputs,
+    concatenated in output order.  dx (optional): the packed (sum T_i,) waveform gradient.
+    param_grads / sink / the returned dict as in encoder_backward_steps; the parameter
+    gradients are summed over the utterances.  Launches do not depend on the number of
+    utterances."""
+    if not param_grads and dx is None:
+        raise ValueError("encoder_backward_packed: nothing to compute (no parameter gradients, "
+                         "no dx)")
+    plan.ensure_backward()
+    if dx is not None:
+        plan.ensure_input_grad()
+    if not param_grads:
+        sink = None
+    pg = param_grads
+    call = ops.call
+    sec, sz = plan.layout
+    tab = lambda name: plan.table[sec[name]:]
+    cfg, G, n = plan.cfg, plan.geoms, len(sz["Tq"])
+    rows, Kc, emb = sz["rows"], plan.Kc, plan.emb
+    P = lambda name: _flat(params[name])
+    grads, copies = {}, []
+    sb = plan.stats_b
+    sb.zero_()
+    if plan.amax is not None:
+        plan.amax.zero_()
+    fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
+    jobs = []
+    for l, g in enumerate(G):
+        if not g.sinc and l > 0:
+            hi, lo = plan.w_operand(("Wd", l), plan.Wd[l])
+            dst = plan.Wd[l] if fmt == gemm.FMT_F32 else None
+            jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
+                         g.s, g.taps, g.s * g.Cin * g.taps * g.Cout))
+    if jobs:
+        plan.w_batch(1, jobs)
+    bo = plan.bn_out
+    o = plan.bs_out
+    call("pase_out_bwd_gather_var", gflat, tab("out"), n, max(sz["Tq"]), emb, plan.g)
+    call("pase_out_bwd_apply", plan.g, plan.yout, bo[0], bo[1], bo[2], sb[o:o + emb],
+         sb[o + emb:o + 2 * emb], float(rows), 0, rows, emb)
+    if pg:
+        call("pase_colsum", plan.g, emb, rows, emb, sb[plan.bs_bw:plan.bs_bw + emb])
+        plan.tn("g", plan.g, emb, rows, 0, True, "cat", plan.cat, Kc, rows, False, plan.dWcat,
+                Kc, emb, Kc, 1, rows, 1.0, 0, a_n=rows * emb)
+        _out_weight_grads(plan, G, params, sink, copies, grads)
+    call("pase_transpose_pad", plan.Wcat, Kc, plan.WcatT, emb, emb, Kc)
+    plan.nt("g", plan.g, emb, not pg, "WcatT", plan.WcatT, emb, True, plan.dcat, Kc, rows, Kc,
+            emb, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad", a_n=rows * emb)
+
+    if plan.rnn:
+        Cq, H, R = plan.Clast, plan.H, sz["xq_rows"]
+        call("pase_qrnn_scan_bwd_var", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg, tab("qbwd"),
+             n, H)
+        if pg:
+            call("pase_colsum", plan.dYg, 3 * H, R, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
+            plan.tn("dYg", plan.dYg, 3 * H, R, 0, True, "xq", plan.xq, Cq, R, False, plan.dWq,
+                    2 * Cq, 3 * H, 2 * Cq, 1, R, 1.0, 0, a_n=R * 3 * H)
+            _qrnn_weight_grads(plan, sink, copies, grads)
+        call("pase_transpose_pad", plan.Wq, 2 * Cq, plan.WqT, 3 * H, 3 * H, 2 * Cq)
+        plan.nt("dYg", plan.dYg, 3 * H, not pg, "WqT", plan.WqT, 3 * H, True, plan.dsrc, 2 * Cq,
+                R, 2 * Cq, 3 * H, 1.0, None, R, R, R, 1, None, None, 0, akind="grad",
+                a_n=R * 3 * H)
+        top = (plan.dsrc, 0, 2 * Cq, 0, 0, plan.dsrc, 2 * Cq, 1)
+    else:
+        top = (plan.dcat, 0, Kc, 0, 0, None, 0, 0)
+
+    for l in range(plan.nblk - 1, -1, -1):
+        g = G[l]
+        C, pre, M = g.Cout, "blocks.%d." % l, sz["gemm_rows"][l]
+        mean, invstd, scale, shift = plan.bn[l][0], plan.bn[l][1], plan.bn[l][2], plan.bn[l][3]
+        if l == plan.nblk - 1:
+            src = top
+        else:
+            nx = G[l + 1]
+            src = (plan.dxpad[l + 1], ybf, C, nx.padL, nx.padR, None, 0, 0)
+        pool = plan.dcat[plan.col_off[l]:] if plan.skips and l + 1 < plan.nblk else None
+        src = src + (pool, Kc)
+        amax = None if plan.amax is None else plan.amax[2 * l:2 * l + 2]
+        o = plan.bs_off[l]
+        t, mT = tab(("bwd", l)), sz["max_Tout"][l]
+        if pg or amax is not None:       # eval mode: the sums feed parameter gradients only
+            call("pase_bn_prelu_bwd_reduce_var", plan.y[l], ybf, t, n, mT, C, mean, invstd,
+                 scale, shift, P(pre + "act.weight"), *src, sb[o:o + C], sb[o + C:o + 2 * C],
+                 sb[o + 2 * C:o + 3 * C], amax)
+        call("pase_bn_prelu_bwd_apply_src_var", plan.y[l], ybf, t, n, sz["max_span"][l], C, invstd,
+             P(pre + "norm.weight"), scale, shift, P(pre + "act.weight"), *src, plan.dyz[l],
+             plan.dyz_lo[l], fmt, sz["lead"][l],
+             sb[o + 3 * C:o + 4 * C] if pg and not g.sinc else None, amax, plan.gscale[l])
+        if g.sinc:
+            if pg:
+                plan.tn(("dyz", l), plan.dyz[l], g.Nn, M, g.dg_rows - 1, False, ("apad", l),
+                        plan.apad[l], g.lda, M, False, plan.dWt[l], g.K, g.Nn, g.K, 1, M, 1.0, 0)
+                if sink is not None:
+                    dlow, dband = sink[pre + "conv.low_hz_"], sink[pre + "conv.band_hz_"]
+                else:
+                    dlow = torch.empty_like(params[pre + "conv.low_hz_"])
+                    dband = torch.empty_like(params[pre + "conv.band_hz_"])
+                call("pase_sinc_grad", plan.dWt[l], P(pre + "conv.low_hz_"),
+                     P(pre + "conv.band_hz_"), mod._sinc_n, mod._sinc_win, dlow.reshape(-1),
+                     dband.reshape(-1), g.Cout, g.k, g.fold, g.K, 50.0, 50.0, float(cfg["sr"]))
+                if sink is None:
+                    grads[pre + "conv.low_hz_"] = dlow
+                    grads[pre + "conv.band_hz_"] = dband
+            if dx is not None:
+                f = g.fold
+                call("pase_sinc_make", P(pre + "conv.low_hz_"), P(pre + "conv.band_hz_"),
+                     mod._sinc_n, mod._sinc_win, plan.filt, plan.Wt[0], g.Cout, g.k, f, g.K,
+                     50.0, 50.0, float(cfg["sr"]))
+                call("pase_sinc_dgrad_weight", plan.filt, plan.Wdg, g.Cout, g.k, f, g.dg_rows)
+                plan.nt(("dyz", l), plan.dyz[l], g.Nn, False, "Wdg", plan.Wdg, g.dg_K, True,
+                        plan.dxpad[0], f, M, f, g.dg_K, 1.0, None, M, M, M, 1, None, None, 0,
+                        akind="grad")
+                call("pase_reflect_fold_wave_var", plan.dxpad[0], tab("wave"), n,
+                     sz["max_T"], dx, g.padL, g.padR)
+        else:
+            if pg:
+                plan.tn(("dyz", l), plan.dyz[l], C, M, g.taps - 1, False, ("apad", l),
+                        plan.apad[l], g.lda, M, False, plan.dWt[l], g.K, C, g.K, 1, M, 1.0, 0)
+            if l > 0:
+                plan.nt(("dyz", l), plan.dyz[l], C, False, ("Wd", l), plan.Wd[l], g.taps * C,
+                        False, plan.dxpad[l], g.s * g.Cin, M, g.s * g.Cin, g.taps * C, 1.0, None,
+                        M, M, M, 1, None, None, 0, akind="grad")
+
+    if not pg:
+        return {}
+    if sink is not None:
+        _emit_sunk_grads(plan, G, sink, copies, range(0, plan.nblk), True, "all")
+        return {}
+    return _autograd_grads(plan, G, grads)
+
+
+class _PackedEncoderFn(torch.autograd.Function):
+    """Autograd node of WaveFe.encode_packed: one packed eval-mode forward of n utterances
+    (tensors = the n flat CUDA waveforms, then the parameters) and one packed backward sweep.
+    The outputs are views of one buffer."""
+
+    @staticmethod
+    def forward(ctx, mod, plan, lengths, geoms, names, n, *tensors):
+        params = dict(zip(names, tensors[n:]))
+        plan.ensure_backward()
+        x = plan.wave[:sum(lengths)]
+        torch.cat(tensors[:n], out=x)
+        feats = encoder_forward_packed(plan, mod, x, lengths, geoms, params, None,
+                                       packed_grad_layout)
+        ctx.set_materialize_grads(False)
+        ctx.mod, ctx.plan, ctx.names, ctx.n = mod, plan, names, n
+        ctx.generation = plan.generation
+        ctx.save_for_backward(*tensors[n:])
+        return tuple(feats)
+
+    @staticmethod
+    def backward(ctx, *gouts):
+        plan, n = ctx.plan, ctx.n
+        if plan.generation != ctx.generation:
+            raise RuntimeError(
+                "pase_b200: the activation buffers of encode_packed were overwritten by a later "
+                "encode_packed forward on the same plan before this backward ran; run backward "
+                "before the next forward.")
+        params = dict(zip(ctx.names, ctx.saved_tensors))
+        need_x = ctx.needs_input_grad[6:6 + n]
+        param_grads = any(ctx.needs_input_grad[6 + n:])        # all or nothing, as _EncoderFn
+        none = (None,) * 6
+        if not param_grads and not any(need_x):
+            return none + (None,) * (n + len(ctx.names))
+        sink = getattr(ctx.mod, "grad_sink", None)
+        if sink is not None and any(nm not in sink for nm in ctx.names):
+            raise RuntimeError("pase_b200: WaveFe.grad_sink must name every parameter "
+                               "(missing %s)" % [nm for nm in ctx.names if nm not in sink][:3])
+        sec, sz = plan.layout
+        emb = plan.emb
+        gflat = plan.gflat[:sz["out"]]
+        torch.cat([plan.gzero[:emb * T] if g is None else g.reshape(-1)
+                   for g, T in zip(gouts, sz["Tq"])], out=gflat)
+        dx = None
+        if any(need_x):
+            dx = torch.empty(sz["total"], dtype=torch.float32, device=plan.device)
+        grads = encoder_backward_packed(plan, ctx.mod, params, gflat, sink, dx, param_grads)
+        dxs, o = [], 0
+        for T, need in zip(sz["lengths"], need_x):
+            dxs.append(dx[o:o + T] if need else None)
+            o += T
+        return none + tuple(dxs) + tuple(grads.get(nm) for nm in ctx.names)
 
 
 # -- windowed inference of one long recording (DESIGN.md section 15) --------------------------
@@ -1141,25 +1449,9 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     # the weight-gradient GEMM above converted g into the GEMM format; without it, this one does
     plan.nt("g", plan.g, emb, not pg, "WcatT", plan.WcatT, emb, True, plan.dcat, Kc, rows, Kc,
             emb, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad")
-    dWcat = plan.dWcat.view(emb, Kc)
-    first = plan.H if plan.rnn else plan.Clast
     copies = []          # sink mode: (src tensor view, rows, cols, src_ld, destination name)
-    if pg and sink is not None:
-        copies.append((dWcat, emb, first, Kc, "W.weight"))
-        if plan.skips:
-            for i in range(plan.nblk - 1):
-                copies.append((dWcat[:, plan.col_off[i]:], emb, G[i].Cout, Kc,
-                               "denseskips.%d.weight" % i))
-    elif pg:
-        # gradients handed to autograd must not alias plan-owned buffers (the next backward
-        # would overwrite them): copy the slices out
-        grads["W.weight"] = dWcat[:, :first].clone().reshape(params["W.weight"].shape)
-        if plan.skips:
-            for i in range(plan.nblk - 1):
-                c0 = plan.col_off[i]
-                grads["denseskips.%d.weight" % i] = \
-                    dWcat[:, c0:c0 + G[i].Cout].clone().reshape(
-                        params["denseskips.%d.weight" % i].shape)
+    if pg:
+        _out_weight_grads(plan, G, params, sink, copies, grads)
 
     Cl = plan.Clast
     if plan.rnn:
@@ -1169,13 +1461,7 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
             call("pase_colsum", plan.dYg, 3 * H, rows, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
             plan.tn("dYg", plan.dYg, 3 * H, Tq, 0, True, "xq", plan.xq, Cq, Tq + 1, False,
                     plan.dWq, 2 * Cq, 3 * H, 2 * Cq, N, Tq, 1.0, 0)
-            dWq = plan.dWq.view(3 * H, 2 * Cq)
-        if pg and sink is not None:   # [x_{t-1} | x_t] GEMM order -> the parameter's [x_t | x_{t-1}]
-            dst = sink["rnn.layers.0.linear.weight"].view(3 * H, 2 * Cq)
-            copies.append((dWq[:, Cq:], 3 * H, Cq, 2 * Cq, dst))
-            copies.append((dWq, 3 * H, Cq, 2 * Cq, dst[:, Cq:]))
-        elif pg:
-            grads["rnn.layers.0.linear.weight"] = torch.cat([dWq[:, Cq:], dWq[:, :Cq]], 1)
+            _qrnn_weight_grads(plan, sink, copies, grads)
         call("pase_transpose_pad", plan.Wq, 2 * Cq, plan.WqT, 3 * H, 3 * H, 2 * Cq)
         plan.nt("dYg", plan.dYg, 3 * H, not pg, "WqT", plan.WqT, 3 * H, True, plan.dsrc, 2 * Cq,
                 rows, 2 * Cq, 3 * H, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad")
@@ -1264,7 +1550,48 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
         else:
             _emit_sunk_grads(plan, G, sink, copies, range(0, plan.nblk), True, "all")
         return {}
+    return _autograd_grads(plan, G, grads)
 
+
+def _out_weight_grads(plan, G, params, sink, copies, grads):
+    """[W | skips] weight gradient in plan.dWcat -> sink copies or autograd gradients."""
+    emb, Kc = plan.emb, plan.Kc
+    dWcat = plan.dWcat.view(emb, Kc)
+    first = plan.H if plan.rnn else plan.Clast
+    if sink is not None:
+        copies.append((dWcat, emb, first, Kc, "W.weight"))
+        if plan.skips:
+            for i in range(plan.nblk - 1):
+                copies.append((dWcat[:, plan.col_off[i]:], emb, G[i].Cout, Kc,
+                               "denseskips.%d.weight" % i))
+    else:
+        # gradients handed to autograd must not alias plan-owned buffers (the next backward
+        # would overwrite them): copy the slices out
+        grads["W.weight"] = dWcat[:, :first].clone().reshape(params["W.weight"].shape)
+        if plan.skips:
+            for i in range(plan.nblk - 1):
+                c0 = plan.col_off[i]
+                grads["denseskips.%d.weight" % i] = \
+                    dWcat[:, c0:c0 + G[i].Cout].clone().reshape(
+                        params["denseskips.%d.weight" % i].shape)
+
+
+def _qrnn_weight_grads(plan, sink, copies, grads):
+    """QRNN gate weight gradient in plan.dWq -> sink copies or an autograd gradient."""
+    Cq, H = plan.Clast, plan.H
+    dWq = plan.dWq.view(3 * H, 2 * Cq)
+    if sink is not None:          # [x_{t-1} | x_t] GEMM order -> the parameter's [x_t | x_{t-1}]
+        dst = sink["rnn.layers.0.linear.weight"].view(3 * H, 2 * Cq)
+        copies.append((dWq[:, Cq:], 3 * H, Cq, 2 * Cq, dst))
+        copies.append((dWq, 3 * H, Cq, 2 * Cq, dst[:, Cq:]))
+    else:
+        grads["rnn.layers.0.linear.weight"] = torch.cat([dWq[:, Cq:], dWq[:, :Cq]], 1)
+
+
+def _autograd_grads(plan, G, grads):
+    """Autograd mode, after the sweep: the conv weight and small gradients added to `grads`."""
+    call = ops.call
+    sb = plan.stats_b
     # conv weight gradients: GEMM layout -> parameter layout for every block in one launch,
     # into one per-call buffer (the gradients handed to autograd are views of it)
     conv_blocks = [l for l, g in enumerate(G) if not g.sinc]

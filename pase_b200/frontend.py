@@ -159,6 +159,7 @@ class WaveFe(Model):
             self.norm_out = nn.BatchNorm1d(emb, affine=False)
         self._plans = OrderedDict()
         self._packed_plans = OrderedDict()
+        self._grad_plans = OrderedDict()       # encode_packed: apart from extract's plans
         self._long_pool = None          # (key, StreamPool) of extract_long
         # GEMM numerics (gemm.PRECISIONS): "fp32" (FFMA), "3xtf32" / "3xf16" (wgmma,
         # fp32-equivalent), "tf32" (wgmma), "bf16" (wgmma, bf16 operands and activations)
@@ -223,6 +224,19 @@ class WaveFe(Model):
                 self._packed_plans.popitem(last=False)
         else:
             self._packed_plans.move_to_end(key)
+        return plan
+
+    def _grad_plan(self, capacity, device):
+        prec = self.resolved_precision()
+        key = (capacity, prec, str(device))
+        plan = self._grad_plans.get(key)
+        if plan is None:
+            plan = _enc.PackedGradPlan(self.cfg, capacity, device, prec)
+            self._grad_plans[key] = plan
+            while len(self._grad_plans) > self.MAX_PLANS:
+                self._grad_plans.popitem(last=False)
+        else:
+            self._grad_plans.move_to_end(key)
         return plan
 
     def _sinc_consts(self, device):
@@ -299,6 +313,51 @@ class WaveFe(Model):
                 feats += _enc.encoder_forward_packed(plan, self, x, lengths[a:b], geoms[a:b],
                                                      params, mode)
         return feats
+
+    def encode_packed(self, wavs, max_samples=None):
+        """Differentiable packed encoding of utterances of any lengths (DESIGN.md section 18):
+        wavs as in extract; returns, in input order, the (1, emb, T'_i) CUDA tensors of
+        ``extract(wavs, mode=None)`` (the same launches and bits).  With grad mode on and a
+        waveform or a parameter requiring a gradient, one autograd node backpropagates to every
+        waveform (through the caller's own .to() / .view()) and to the parameters (summed over
+        the utterances; autograd or grad_sink).  One pack per call: the total must fit
+        `max_samples` (default EXTRACT_MAX_SAMPLES).  Eval mode only."""
+        device = self._eval_device("encode_packed")
+        cap = EXTRACT_MAX_SAMPLES if max_samples is None else int(max_samples)
+        if cap < 1:
+            raise ValueError("max_samples must be positive, got %r" % (max_samples,))
+        flat = []
+        for i, w in enumerate(wavs):
+            try:
+                flat.append(_recording(w))
+            except (TypeError, ValueError) as e:
+                raise type(e)("utterance %d: %s" % (i, e)) from None
+        if not flat:
+            return []
+        return self._encode_packed(flat, cap, device)
+
+    def _encode_packed(self, flat, cap, device):
+        lengths = [w.numel() for w in flat]
+        if sum(lengths) > cap:
+            raise ValueError("encode_packed: %d samples exceed max_samples=%d; one call is one "
+                             "pack, so split the list into calls that fit"
+                             % (sum(lengths), cap))
+        fold = _gemm.PRECISIONS[self.resolved_precision()].sinc_fold
+        geoms = _enc.utterance_geometry(self.cfg, lengths, fold)
+        self._sinc_consts(device)
+        plan = self._grad_plan(cap, device)
+        named = list(self.named_parameters())
+        names = tuple(n for n, _ in named)
+        tensors = [p for _, p in named]
+        xs = [w.to(device) for w in flat]
+        if torch.is_grad_enabled() and (any(w.requires_grad for w in xs) or
+                                        any(p.requires_grad for p in tensors)):
+            return list(_enc._PackedEncoderFn.apply(self, plan, lengths, geoms, names, len(xs),
+                                                    *xs, *tensors))
+        with torch.no_grad():
+            x = plan.wave[:sum(lengths)]
+            torch.cat(xs, out=x)
+            return _enc.encoder_forward_packed(plan, self, x, lengths, geoms, dict(named))
 
     def _eval_device(self, what):
         if self.training:
