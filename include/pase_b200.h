@@ -108,6 +108,22 @@ int pase_tc_gemm_nt_var(const void* Ahi, const void* Alo, long a_rows, int R,
                         const void* Bhi, const void* Blo, long ldb, void* C, long ldc,
                         int M, int N, int K, const float* bias, const int* var_tab, int nvar,
                         int fold, int mode, int c_bf16, void* stream);
+/* The two packed GEMMs above with train-mode BatchNorm column statistics (WaveFe.
+ * encode_packed_train, DESIGN.md section 19; FeBlock's conv -> BatchNorm1d,
+ * pase/models/modules.py:1014-1077): colsum[n] += sum C(m, n), colsumsq[n] += sum C(m, n)^2
+ * (DEVICE, double[N], N <= 4096) over exactly the elements the row map stores, so over the
+ * valid frames of every utterance and nothing else; in the folded sinc layer column n is
+ * virtual channel n of the fold, summed by pase_bn_finalize.  The sums are those of the uniform
+ * kernels' epilogues (fp32 per tile, fp64 across tiles); both launches of a partial last round
+ * take part. */
+int pase_gemm_nt_var_stats(const float* A, long lda, const float* B, long ldb, float* C,
+                           long ldc, int M, int N, int K, const float* bias, const int* var_tab,
+                           int nvar, int fold, double* colsum, double* colsumsq, void* stream);
+int pase_tc_gemm_nt_var_stats(const void* Ahi, const void* Alo, long a_rows, int R,
+                              const void* Bhi, const void* Blo, long ldb, void* C, long ldc,
+                              int M, int N, int K, const float* bias, const int* var_tab,
+                              int nvar, int fold, double* colsum, double* colsumsq, int mode,
+                              int c_bf16, void* stream);
 /* How pase_tc_gemm_nt / pase_tc_gemm_nt_var cover an M x N output on `sms` SMs (host only):
  * out4 = {bn, bulk_m, tail_bn, tail_pieces}.  One launch of 128 x bn tiles takes rows
  * [0, bulk_m); when the tiles leave a partial last round, a second launch takes rows
@@ -342,6 +358,24 @@ int pase_bn_prelu_bwd_apply_src_var(const void* y, int y_bf16, const int* tab, i
                                     const float* pool, long pool_row_stride, void* dst,
                                     void* dst_lo, int dst_fmt, int lead, double* dbias_acc,
                                     const float* amax, float* scale_out, void* stream);
+/* Train-mode form of pase_bn_prelu_bwd_apply_src_var (WaveFe.encode_packed_train, DESIGN.md
+ * section 19; autograd of FeBlock's BatchNorm1d + PReLU over the whole pack,
+ * pase/models/modules.py:1014-1077): dy = gamma invstd (du - S1/count - xhat S2/count), xhat =
+ * (y - mean) invstd, with S1 = sum du and S2 = sum du xhat of pase_bn_prelu_bwd_reduce_var over
+ * every utterance and count = the pack's valid frames.  Table, layout, zero frames, dbias_acc
+ * and the fp16-pair scale (bound gamma invstd (max|du| + |S1/count| + max|xhat| |S2/count|)
+ * from amax over the pack) as in pase_bn_prelu_bwd_apply_src_var. */
+int pase_bn_prelu_bwd_apply_src_var_train(const void* y, int y_bf16, const int* tab, int nseg,
+                                          int max_span, int C, const float* mean,
+                                          const float* invstd, const float* gamma,
+                                          const float* scale, const float* shift,
+                                          const float* alpha, const double* S1, const double* S2,
+                                          double count, const void* srcA, int a_bf16,
+                                          long a_row_stride, int padL, int padR,
+                                          const float* srcB, long b_row_stride, int b_shift,
+                                          const float* pool, long pool_row_stride, void* dst,
+                                          void* dst_lo, int dst_fmt, int lead, double* dbias_acc,
+                                          const float* amax, float* scale_out, void* stream);
 /* The three backward entry points above read and write y, srcA, srcB, pool, dst, dst_lo and du
  * in quads of channels: fp32 operands must be 16-byte aligned, 16-bit ones 8-byte aligned,
  * every row and sample stride a multiple of 4 elements, a/b_row_stride >= C and
@@ -401,6 +435,13 @@ int pase_out_bwd_reduce(const float* dout, const float* dout_ntc, const float* y
  * max_T >= every T. */
 int pase_out_bwd_gather_var(const float* dout, const int* tab, int nseg, int max_T, int C,
                             float* g_ntc, void* stream);
+/* pase_out_bwd_gather_var with pase_out_bwd_reduce's sums (train-mode norm_out of
+ * WaveFe.encode_packed_train, frontend.py:206-208): the same gather, and S1 += g,
+ * S2 += g*xhat (double[C]) with xhat = (y[(row0 + t)*C + c] - mean[c]) invstd[c] over every
+ * utterance's rows; pase_out_bwd_apply(use_stats = 1) then finishes dy. */
+int pase_out_bwd_reduce_var(const float* dout, const int* tab, int nseg, int max_T, int C,
+                            const float* y, const float* mean, const float* invstd, float* g_ntc,
+                            double* S1, double* S2, void* stream);
 /* in place: g = scale*(g - use_stats*(S1/M + xhat*S2/M)) */
 int pase_out_bwd_apply(float* g, const float* y, const float* mean, const float* invstd,
                        const float* scale, const double* S1, const double* S2,

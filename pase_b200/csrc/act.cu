@@ -744,21 +744,22 @@ __device__ __forceinline__ void store_grad4(void* dst_v, void* dst_lo_v, long of
   }
 }
 
-// pass 2 of pase_bn_prelu_bwd_apply_src in eval mode (S1 = S2 = 0: dy = gamma invstd du) for
-// every utterance, into frames d_off/C + f of dst, f < d_span: the utterance's T frames, zeros
-// in [T, d_span) and, for the first utterance, zeros in the `lead` frames before it.  Work item
-// j < C/4 * ceil(T/RUN) computes a run; the others write the zero frames.
-template <typename YT, typename GT, int DF>
-__global__ void __launch_bounds__(THREADS)
-bn_prelu_bwd_apply_src_var_kernel(const YT* __restrict__ y, const int* __restrict__ tab, int C,
-                                  const float* __restrict__ invstd,
-                                  const float* __restrict__ gamma,
-                                  const float* __restrict__ scale, const float* __restrict__ shift,
-                                  const float* __restrict__ alpha, const void* A, long a_rs,
-                                  int padL, int padR, const float* B, long b_rs, int b_shift,
-                                  const float* pool, long p_rs, void* dst_v, void* dst_lo_v,
-                                  int lead, double* __restrict__ dbias,
-                                  const float* __restrict__ amax, float* __restrict__ scale_out) {
+// pass 2 of pase_bn_prelu_bwd_apply_src for every utterance, into frames d_off/C + f of dst,
+// f < d_span: the utterance's T frames, zeros in [T, d_span) and, for the first utterance,
+// zeros in the `lead` frames before it.  Work item j < C/4 * ceil(T/RUN) computes a run; the
+// others write the zero frames.  TRAIN: batch statistics over the pack, dy = gamma invstd (du -
+// S1/count - xhat S2/count) with xhat = (y - mean) invstd; else eval mode (S1 = S2 = 0: dy =
+// gamma invstd du; mean, S1, S2 unused).
+template <typename YT, typename GT, int DF, bool TRAIN>
+__device__ __forceinline__ void bn_prelu_bwd_apply_src_var_body(
+    const YT* __restrict__ y, const int* __restrict__ tab, int C, const float* __restrict__ mean,
+    const float* __restrict__ invstd, const float* __restrict__ gamma,
+    const float* __restrict__ scale, const float* __restrict__ shift,
+    const float* __restrict__ alpha, const double* __restrict__ S1,
+    const double* __restrict__ S2, double inv_count, const void* A, long a_rs, int padL, int padR,
+    const float* B, long b_rs, int b_shift, const float* pool, long p_rs, void* dst_v,
+    void* dst_lo_v, int lead, double* __restrict__ dbias, const float* __restrict__ amax,
+    float* __restrict__ scale_out) {
   pdl_wait();
   extern __shared__ double red[];
   float* redm = reinterpret_cast<float*>(red + C);
@@ -766,11 +767,20 @@ bn_prelu_bwd_apply_src_var_kernel(const YT* __restrict__ y, const int* __restric
   if (threadIdx.x == 0) redm[0] = 0.f;
   __syncthreads();
   float gs_scale = 1.f;
-  if constexpr (DF == PASE_FMT_F16X2) {     // pase_bn_prelu_bwd_apply_src's bound, S1 = S2 = 0
+  if constexpr (DF == PASE_FMT_F16X2) {     // pase_bn_prelu_bwd_apply_src's bound
     const float mdu = amax[0];
     float b = 0.f;
-    for (int i = threadIdx.x; i < C; i += blockDim.x)
-      b = fmaxf(b, fabsf((gamma ? gamma[i] : 1.f) * invstd[i]) * mdu);
+    if constexpr (TRAIN) {
+      const float mxh = amax[1];
+      for (int i = threadIdx.x; i < C; i += blockDim.x) {
+        const float gi = fabsf((gamma ? gamma[i] : 1.f) * invstd[i]);
+        const float m1 = fabsf((float)(S1[i] * inv_count)), m2 = fabsf((float)(S2[i] * inv_count));
+        b = fmaxf(b, gi * (mdu + m1 + mxh * m2));
+      }
+    } else {
+      for (int i = threadIdx.x; i < C; i += blockDim.x)
+        b = fmaxf(b, fabsf((gamma ? gamma[i] : 1.f) * invstd[i]) * mdu);
+    }
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, off));
     if ((threadIdx.x & 31) == 0) atomic_max_pos(&redm[0], b);
@@ -800,13 +810,19 @@ bn_prelu_bwd_apply_src_var_kernel(const YT* __restrict__ y, const int* __restric
 #pragma unroll
     for (int i = 0; i < RUN; ++i) vs[i] = ld4t(yn + (long)((int)t0 + (i < nvalid ? i : 0)) * C + c);
     load_grad_run<GT>(s, 0, T, t0, nvalid, c, gs);
-    float gi[4], scv[4], shv[4], alv[4];
+    float gi[4], scv[4], shv[4], alv[4], m1[4], m2[4], muv[4], isv[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       gi[k] = (gamma ? gamma[c + k] : 1.f) * invstd[c + k];
       scv[k] = scale[c + k];
       shv[k] = shift[c + k];
       alv[k] = alpha[c + k];
+      if constexpr (TRAIN) {
+        m1[k] = (float)(S1[c + k] * inv_count);
+        m2[k] = (float)(S2[c + k] * inv_count);
+        muv[k] = mean[c + k];
+        isv[k] = invstd[c + k];
+      }
     }
 #pragma unroll
     for (int i = 0; i < RUN; ++i) {
@@ -818,7 +834,12 @@ bn_prelu_bwd_apply_src_var_kernel(const YT* __restrict__ y, const int* __restric
       for (int k = 0; k < 4; ++k) {
         const float u = fmaf(vv[k], scv[k], shv[k]);
         const float du = u > 0.f ? gg[k] : alv[k] * gg[k];
-        o[k] = gi[k] * du;
+        if constexpr (TRAIN) {
+          const float xh = (vv[k] - muv[k]) * isv[k];
+          o[k] = gi[k] * (du - m1[k] - xh * m2[k]);
+        } else {
+          o[k] = gi[k] * du;
+        }
         acc[k] += o[k];
       }
       store_grad4<DF>(dst_v, dst_lo_v, d_off + ((long)t0 + i) * C + c,
@@ -843,6 +864,84 @@ bn_prelu_bwd_apply_src_var_kernel(const YT* __restrict__ y, const int* __restric
     __syncthreads();
     if ((long)blockIdx.x * blockDim.x < (long)C4 * nruns)
       for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dbias + i, red[i]);
+  }
+}
+
+template <typename YT, typename GT, int DF>
+__global__ void __launch_bounds__(THREADS)
+bn_prelu_bwd_apply_src_var_kernel(const YT* __restrict__ y, const int* __restrict__ tab, int C,
+                                  const float* __restrict__ invstd,
+                                  const float* __restrict__ gamma,
+                                  const float* __restrict__ scale, const float* __restrict__ shift,
+                                  const float* __restrict__ alpha, const void* A, long a_rs,
+                                  int padL, int padR, const float* B, long b_rs, int b_shift,
+                                  const float* pool, long p_rs, void* dst_v, void* dst_lo_v,
+                                  int lead, double* __restrict__ dbias,
+                                  const float* __restrict__ amax, float* __restrict__ scale_out) {
+  bn_prelu_bwd_apply_src_var_body<YT, GT, DF, false>(
+      y, tab, C, nullptr, invstd, gamma, scale, shift, alpha, nullptr, nullptr, 0.0, A, a_rs,
+      padL, padR, B, b_rs, b_shift, pool, p_rs, dst_v, dst_lo_v, lead, dbias, amax, scale_out);
+}
+
+template <typename YT, typename GT, int DF>
+__global__ void __launch_bounds__(THREADS)
+bn_prelu_bwd_apply_src_var_train_kernel(
+    const YT* __restrict__ y, const int* __restrict__ tab, int C, const float* __restrict__ mean,
+    const float* __restrict__ invstd, const float* __restrict__ gamma,
+    const float* __restrict__ scale, const float* __restrict__ shift,
+    const float* __restrict__ alpha, const double* __restrict__ S1,
+    const double* __restrict__ S2, double inv_count, const void* A, long a_rs, int padL, int padR,
+    const float* B, long b_rs, int b_shift, const float* pool, long p_rs, void* dst_v,
+    void* dst_lo_v, int lead, double* __restrict__ dbias, const float* __restrict__ amax,
+    float* __restrict__ scale_out) {
+  bn_prelu_bwd_apply_src_var_body<YT, GT, DF, true>(
+      y, tab, C, mean, invstd, gamma, scale, shift, alpha, S1, S2, inv_count, A, a_rs, padL, padR,
+      B, b_rs, b_shift, pool, p_rs, dst_v, dst_lo_v, lead, dbias, amax, scale_out);
+}
+
+// pase_out_bwd_reduce over packed utterances: tab rows {row0, T, o_off} (blockIdx.z), tiles of
+// 32 frames x 32 channels; g_ntc[(row0 + t)*C + c] = dout[o_off + c*T + t], S1 += g,
+// S2 += g*xhat
+__global__ void out_bwd_reduce_var_kernel(const float* __restrict__ dout,
+                                          const int* __restrict__ tab,
+                                          const float* __restrict__ y,
+                                          const float* __restrict__ mean,
+                                          const float* __restrict__ invstd, int C,
+                                          float* __restrict__ g_ntc, double* __restrict__ S1,
+                                          double* __restrict__ S2) {
+  pdl_wait();
+  __shared__ float tile[32][33];
+  __shared__ double r1[32], r2[32];
+  const int* r = tab + 3 * blockIdx.z;
+  const long row0 = __ldg(r), o = __ldg(r + 2);
+  const int T = __ldg(r + 1);
+  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  if (t0 >= T) return;                       // the whole block: before any barrier
+  if (threadIdx.y == 0) { r1[threadIdx.x] = 0.0; r2[threadIdx.x] = 0.0; }
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int c = c0 + i, t = t0 + threadIdx.x;
+    tile[i][threadIdx.x] = (t < T && c < C) ? dout[o + (long)c * T + t] : 0.f;
+  }
+  __syncthreads();
+  float a1 = 0.f, a2 = 0.f;
+  const int c = c0 + threadIdx.x;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int t = t0 + i;
+    if (t < T && c < C) {
+      const long off = (row0 + t) * C + c;
+      const float g = tile[threadIdx.x][i];
+      g_ntc[off] = g;
+      const float xh = (y[off] - mean[c]) * invstd[c];
+      a1 += g;
+      a2 += g * xh;
+    }
+  }
+  atomicAdd(&r1[threadIdx.x], (double)a1);
+  atomicAdd(&r2[threadIdx.x], (double)a2);
+  __syncthreads();
+  if (threadIdx.y == 0 && c < C) {
+    atomicAdd(S1 + c, r1[threadIdx.x]);
+    atomicAdd(S2 + c, r2[threadIdx.x]);
   }
 }
 
@@ -1845,15 +1944,17 @@ int pase_bn_prelu_bwd_reduce_var(const void* y, int y_bf16, const int* tab, int 
   return PASE_OK;
 }
 
-int pase_bn_prelu_bwd_apply_src_var(const void* y, int y_bf16, const int* tab, int nseg,
-                                    int max_span, int C, const float* invstd, const float* gamma,
-                                    const float* scale, const float* shift, const float* alpha,
-                                    const void* srcA, int a_bf16, long a_row_stride, int padL,
-                                    int padR, const float* srcB, long b_row_stride, int b_shift,
-                                    const float* pool, long pool_row_stride, void* dst,
-                                    void* dst_lo, int dst_fmt, int lead, double* dbias_acc,
-                                    const float* amax, float* scale_out, void* stream) {
-  const char* fn = "pase_bn_prelu_bwd_apply_src_var";
+// pase_bn_prelu_bwd_apply_src_var (mean, S1, S2 NULL: eval mode) and its train-mode form
+static int bn_apply_src_var(const char* fn, const void* y, int y_bf16, const int* tab, int nseg,
+                            int max_span, int C, const float* mean, const float* invstd,
+                            const float* gamma, const float* scale, const float* shift,
+                            const float* alpha, const double* S1, const double* S2, double count,
+                            const void* srcA, int a_bf16, long a_row_stride, int padL, int padR,
+                            const float* srcB, long b_row_stride, int b_shift, const float* pool,
+                            long pool_row_stride, void* dst, void* dst_lo, int dst_fmt, int lead,
+                            double* dbias_acc, const float* amax, float* scale_out,
+                            void* stream) {
+  const bool train = S1 != nullptr;
   PASE_CHECK_ARG(invstd && scale && shift && alpha && dst && lead >= 0, "%s: null pointer / lead",
                  fn);
   const int rc = bn_bwd_var_check(fn, y, y_bf16, tab, nseg, max_span, C, srcA, a_bf16,
@@ -1871,10 +1972,19 @@ int pase_bn_prelu_bwd_apply_src_var(const void* y, int y_bf16, const int* tab, i
   const size_t sm = C * sizeof(double) + sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_APSV(YT, GT, DF)                                                                  \
-  PASE_LAUNCH((bn_prelu_bwd_apply_src_var_kernel<YT, GT, DF>), grid, THREADS, sm, st,          \
-              reinterpret_cast<const YT*>(y), tab, C, invstd, gamma, scale, shift, alpha, srcA, \
-              a_row_stride, padL, padR, srcB, b_row_stride, b_shift, pool, pool_row_stride,     \
-              dst, dst_lo, lead, dbias_acc, amax, scale_out)
+  do {                                                                                         \
+    if (train)                                                                                 \
+      PASE_LAUNCH((bn_prelu_bwd_apply_src_var_train_kernel<YT, GT, DF>), grid, THREADS, sm, st, \
+                  reinterpret_cast<const YT*>(y), tab, C, mean, invstd, gamma, scale, shift,    \
+                  alpha, S1, S2, 1.0 / count, srcA, a_row_stride, padL, padR, srcB,             \
+                  b_row_stride, b_shift, pool, pool_row_stride, dst, dst_lo, lead, dbias_acc,   \
+                  amax, scale_out);                                                            \
+    else                                                                                       \
+      PASE_LAUNCH((bn_prelu_bwd_apply_src_var_kernel<YT, GT, DF>), grid, THREADS, sm, st,      \
+                  reinterpret_cast<const YT*>(y), tab, C, invstd, gamma, scale, shift, alpha,   \
+                  srcA, a_row_stride, padL, padR, srcB, b_row_stride, b_shift, pool,            \
+                  pool_row_stride, dst, dst_lo, lead, dbias_acc, amax, scale_out);             \
+  } while (0)
   if (dst_fmt == PASE_FMT_BF16) {
     if (a_bf16) PASE_APSV(__nv_bfloat16, __nv_bfloat16, PASE_FMT_BF16);
     else PASE_APSV(__nv_bfloat16, float, PASE_FMT_BF16);
@@ -1885,6 +1995,51 @@ int pase_bn_prelu_bwd_apply_src_var(const void* y, int y_bf16, const int* tab, i
   }
 #undef PASE_APSV
   PASE_LAUNCH_CHECK(fn);
+  return PASE_OK;
+}
+
+int pase_bn_prelu_bwd_apply_src_var(const void* y, int y_bf16, const int* tab, int nseg,
+                                    int max_span, int C, const float* invstd, const float* gamma,
+                                    const float* scale, const float* shift, const float* alpha,
+                                    const void* srcA, int a_bf16, long a_row_stride, int padL,
+                                    int padR, const float* srcB, long b_row_stride, int b_shift,
+                                    const float* pool, long pool_row_stride, void* dst,
+                                    void* dst_lo, int dst_fmt, int lead, double* dbias_acc,
+                                    const float* amax, float* scale_out, void* stream) {
+  return bn_apply_src_var("pase_bn_prelu_bwd_apply_src_var", y, y_bf16, tab, nseg, max_span, C,
+                          nullptr, invstd, gamma, scale, shift, alpha, nullptr, nullptr, 1.0,
+                          srcA, a_bf16, a_row_stride, padL, padR, srcB, b_row_stride, b_shift,
+                          pool, pool_row_stride, dst, dst_lo, dst_fmt, lead, dbias_acc, amax,
+                          scale_out, stream);
+}
+
+int pase_bn_prelu_bwd_apply_src_var_train(
+    const void* y, int y_bf16, const int* tab, int nseg, int max_span, int C, const float* mean,
+    const float* invstd, const float* gamma, const float* scale, const float* shift,
+    const float* alpha, const double* S1, const double* S2, double count, const void* srcA,
+    int a_bf16, long a_row_stride, int padL, int padR, const float* srcB, long b_row_stride,
+    int b_shift, const float* pool, long pool_row_stride, void* dst, void* dst_lo, int dst_fmt,
+    int lead, double* dbias_acc, const float* amax, float* scale_out, void* stream) {
+  const char* fn = "pase_bn_prelu_bwd_apply_src_var_train";
+  PASE_CHECK_ARG(mean && S1 && S2 && count >= 1.0, "%s: null statistics or count %g < 1", fn,
+                 count);
+  return bn_apply_src_var(fn, y, y_bf16, tab, nseg, max_span, C, mean, invstd, gamma, scale, shift,
+                          alpha, S1, S2, count, srcA, a_bf16, a_row_stride, padL, padR, srcB,
+                          b_row_stride, b_shift, pool, pool_row_stride, dst, dst_lo, dst_fmt,
+                          lead, dbias_acc, amax, scale_out, stream);
+}
+
+int pase_out_bwd_reduce_var(const float* dout, const int* tab, int nseg, int max_T, int C,
+                            const float* y, const float* mean, const float* invstd, float* g_ntc,
+                            double* S1, double* S2, void* stream) {
+  PASE_CHECK_ARG(dout && tab && y && mean && invstd && g_ntc && S1 && S2,
+                 "pase_out_bwd_reduce_var: null pointer");
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535 && max_T > 0 && C > 0,
+                 "pase_out_bwd_reduce_var: nseg=%d max_T=%d C=%d", nseg, max_T, C);
+  dim3 grid((max_T + 31) / 32, (C + 31) / 32, nseg), block(32, 8);
+  PASE_LAUNCH((out_bwd_reduce_var_kernel), grid, block, 0, (cudaStream_t)stream, dout, tab, y,
+              mean, invstd, C, g_ntc, S1, S2);
+  PASE_LAUNCH_CHECK("pase_out_bwd_reduce_var");
   return PASE_OK;
 }
 

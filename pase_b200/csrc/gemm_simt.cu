@@ -446,21 +446,38 @@ extern "C" int pase_gemm_tn(const float* A, long lda, int pitchA, int offA, cons
   return launch_tn<128>(A, lda, B, ldb, C, ldc, I, J, rm, alpha, accumulate, st);
 }
 
-extern "C" int pase_gemm_nt_var(const float* A, long lda, const float* B, long ldb, float* C,
-                                long ldc, int M, int N, int K, const float* bias,
-                                const int* var_tab, int nvar, int fold, void* stream) {
-  PASE_CHECK_ARG(A && B && C && var_tab && nvar > 0, "pase_gemm_nt_var: null operand / table");
-  PASE_CHECK_ARG(M > 0 && N > 0 && K > 0, "pase_gemm_nt_var: bad shape M=%d N=%d K=%d", M, N, K);
+// pase_gemm_nt_var and pase_gemm_nt_var_stats (colsum / colsumsq NULL: no statistics)
+static int gemm_nt_var_impl(const char* fn, const float* A, long lda, const float* B, long ldb,
+                            float* C, long ldc, int M, int N, int K, const float* bias,
+                            const int* var_tab, int nvar, int fold, double* colsum,
+                            double* colsumsq, void* stream) {
+  PASE_CHECK_ARG(A && B && C && var_tab && nvar > 0, "%s: null operand / table", fn);
+  PASE_CHECK_ARG(M > 0 && N > 0 && K > 0, "%s: bad shape M=%d N=%d K=%d", fn, M, N, K);
   PASE_CHECK_ARG((lda % 4) == 0 && (ldb % 4) == 0 && (K % 4) == 0,
-                 "pase_gemm_nt_var: lda, ldb, K must be multiples of 4 (lda=%ld ldb=%ld K=%d)",
-                 lda, ldb, K);
-  PASE_CHECK_ARG(aligned16(A) && aligned16(B), "pase_gemm_nt_var: A/B must be 16-byte aligned");
-  PASE_CHECK_ARG(fold > 0 && (N % fold) == 0, "pase_gemm_nt_var: fold=%d N=%d", fold, N);
+                 "%s: lda, ldb, K must be multiples of 4 (lda=%ld ldb=%ld K=%d)", fn, lda, ldb, K);
+  PASE_CHECK_ARG(aligned16(A) && aligned16(B), "%s: A/B must be 16-byte aligned", fn);
+  PASE_CHECK_ARG(fold > 0 && (N % fold) == 0, "%s: fold=%d N=%d", fn, fold, N);
   RowMap rm{1, 0, 1, fold, N / fold, var_tab, nvar};
   cudaStream_t st = (cudaStream_t)stream;
   if (N <= 64)
-    return launch_nt<64, true>(A, lda, B, ldb, C, ldc, M, N, K, 1.f, bias, rm, nullptr, nullptr,
+    return launch_nt<64, true>(A, lda, B, ldb, C, ldc, M, N, K, 1.f, bias, rm, colsum, colsumsq,
                                0, st);
-  return launch_nt<128, true>(A, lda, B, ldb, C, ldc, M, N, K, 1.f, bias, rm, nullptr, nullptr, 0,
+  return launch_nt<128, true>(A, lda, B, ldb, C, ldc, M, N, K, 1.f, bias, rm, colsum, colsumsq, 0,
                               st);
+}
+
+extern "C" int pase_gemm_nt_var(const float* A, long lda, const float* B, long ldb, float* C,
+                                long ldc, int M, int N, int K, const float* bias,
+                                const int* var_tab, int nvar, int fold, void* stream) {
+  return gemm_nt_var_impl("pase_gemm_nt_var", A, lda, B, ldb, C, ldc, M, N, K, bias, var_tab,
+                          nvar, fold, nullptr, nullptr, stream);
+}
+
+extern "C" int pase_gemm_nt_var_stats(const float* A, long lda, const float* B, long ldb,
+                                      float* C, long ldc, int M, int N, int K, const float* bias,
+                                      const int* var_tab, int nvar, int fold, double* colsum,
+                                      double* colsumsq, void* stream) {
+  PASE_CHECK_ARG(colsum && colsumsq, "pase_gemm_nt_var_stats: null statistics");
+  return gemm_nt_var_impl("pase_gemm_nt_var_stats", A, lda, B, ldb, C, ldc, M, N, K, bias,
+                          var_tab, nvar, fold, colsum, colsumsq, stream);
 }

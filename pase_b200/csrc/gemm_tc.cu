@@ -1343,6 +1343,17 @@ int pase_tc_gemm_nt_var(const void* Ahi, const void* Alo, long a_rows, int R, co
                          1, 0, 1, fold, nullptr, nullptr, 0, mode, c_bf16, var_tab, nvar, stream);
 }
 
+int pase_tc_gemm_nt_var_stats(const void* Ahi, const void* Alo, long a_rows, int R,
+                              const void* Bhi, const void* Blo, long ldb, void* C, long ldc, int M,
+                              int N, int K, const float* bias, const int* var_tab, int nvar,
+                              int fold, double* colsum, double* colsumsq, int mode, int c_bf16,
+                              void* stream) {
+  PASE_CHECK_ARG(var_tab && nvar > 0, "pase_tc_gemm_nt_var_stats: empty utterance table");
+  PASE_CHECK_ARG(colsum && colsumsq, "pase_tc_gemm_nt_var_stats: null statistics");
+  return tc_gemm_nt_impl(Ahi, Alo, a_rows, R, Bhi, Blo, ldb, C, ldc, M, N, K, 1.f, nullptr, bias,
+                         1, 0, 1, fold, colsum, colsumsq, 0, mode, c_bf16, var_tab, nvar, stream);
+}
+
 // Fused output layer of a regression head (MLPMinion W + ContextualizedLoss MSE,
 // minions.py:494-524, losses.py:15-37): residual = A B^T + bias - ctx(label) is never stored
 // as fp32; the fp16 pair of s * residual (the backward GEMMs' operand), sum residual^2 and

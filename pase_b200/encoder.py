@@ -369,12 +369,13 @@ class EncoderPlan(object):
                        lambda: self.operand(an, A, afresh, akind, a_n),
                        lambda: self.operand(bn, B, bfresh, "weight"))
 
-    def nt_var(self, an, A, lda, bn, B, ldb, bfresh, C, ldc, M, N, K, bias, tab, n, fold):
+    def nt_var(self, an, A, lda, bn, B, ldb, bfresh, C, ldc, M, N, K, bias, tab, n, fold,
+               cs=None, cq=None):
         """gemm.nt_var over the packed operand `an` (written in the GEMM format by its
         producer) and the weight operand `bn`."""
         return gemm.nt_var(self.precision, A, lda, A.numel(), B, ldb, C, ldc, M, N, K, bias, tab,
                            n, fold, lambda: self.operand(an, A, False),
-                           lambda: self.operand(bn, B, bfresh, "weight"))
+                           lambda: self.operand(bn, B, bfresh, "weight"), cs, cq)
 
     def tn(self, an, A, lda, pitchA, offA, afresh, bn, B, ldb, pitchB, bfresh, C, ldc, I, J,
            groups, rpg, alpha, acc, akind="grad", a_n=None):
@@ -729,25 +730,32 @@ def packed_layout(plan, lengths, geoms, mode):
     assert table.size <= _table_size(plan.nblk, n) and table.max() < INDEX_LIMIT
     sizes = dict(rows=int(q0[n]), xq_rows=int(xr0[n]), gemm_rows=[int(r) for r in row0[n]],
                  max_T=int(max(lengths)), max_Tout=[int(t) for t in TO.max(0)],
+                 count=[int(c) for c in TO.sum(0)],
                  out=int(o0[n]), offsets=[int(o) for o in o0[:n]], Tq=[int(t) for t in Tq],
                  E=E)
     return torch.from_numpy(table.astype(np.int32)), sec, sizes
 
 
-def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None, layout=None):
-    """Eval-mode forward of utterances packed in x (fp32, sum(lengths) samples, plan.wave):
-    each one computed as a B=1 forward would.  Launches do not depend on the number of
-    utterances.  Returns the list of (1, E, T'_i) features, views of one new buffer.
-    layout: the table builder (default packed_layout; packed_grad_layout also uploads the
-    backward's sections).  Every forward bumps plan.generation: a backward saved against an
-    earlier forward of the plan raises instead of reading these activations."""
+def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None, layout=None,
+                           training=False):
+    """Forward of utterances packed in x (fp32, sum(lengths) samples, plan.wave).  Eval mode:
+    each one computed as a B=1 forward would.  training (DESIGN.md section 19): every BatchNorm
+    normalises with the statistics of the valid frames of the whole pack and updates its running
+    statistics and counter once.  Launches do not depend on the number of utterances.  Returns
+    the list of (1, E, T'_i) features, views of one new buffer.  layout: the table builder
+    (default packed_layout; packed_grad_layout also uploads the backward's sections).  Every
+    forward bumps plan.generation: a backward saved against an earlier forward of the plan
+    raises instead of reading these activations."""
     plan.generation += 1
-    sz, tab = _packed_front(plan, mod, x, lengths, geoms, params, mode, layout)
+    counters = [] if training else None
+    sz, tab = _packed_front(plan, mod, x, lengths, geoms, params, mode, layout, counters)
     n = len(lengths)
     if plan.rnn:
         ops.call("pase_qrnn_scan_fwd_var", plan.Yg, plan.cat, plan.Kc, plan.Cst, tab("scan"), n,
                  plan.H)
-    _packed_out_proj(plan, mod, params, sz["rows"])
+    _packed_out_proj(plan, mod, params, sz["rows"], counters)
+    if counters:                                 # BatchNorm step counters: one launch
+        torch._foreach_add_(counters, 1)
     bo = plan.bn_out
     out = torch.empty(sz["out"], dtype=torch.float32, device=x.device)
     ops.call("pase_out_affine_var", plan.yout, bo[2], bo[3], out, tab("out"), n, plan.emb,
@@ -756,20 +764,23 @@ def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None, layo
     return [out[o:o + E * t].view(1, E, t) for o, t in zip(sz["offsets"], sz["Tq"])]
 
 
-def _packed_front(plan, mod, x, lengths, geoms, params, mode, layout=None):
+def _packed_front(plan, mod, x, lengths, geoms, params, mode, layout=None, counters=None):
     """encoder_forward_packed up to the QRNN scan: every conv block, the pooled skips in
     plan.cat and (rnn configs) the gate pre-activations of every frame in plan.Yg.
     -> (sizes of packed_layout, section -> device table view)."""
     host, sec, sz = (layout or packed_layout)(plan, lengths, geoms, mode)
     plan.table[:host.numel()].copy_(host)                    # the one host-to-device copy
     tab = lambda name: plan.table[sec[name]:]
-    _packed_front_launch(plan, mod, x, sz, tab, params)
+    _packed_front_launch(plan, mod, x, sz, tab, params, counters)
     return sz, tab
 
 
-def _packed_front_launch(plan, mod, x, sz, tab, params):
+def _packed_front_launch(plan, mod, x, sz, tab, params, counters=None):
     """The launches of _packed_front, from a layout already on the device (tab: section ->
-    table view)."""
+    table view).  counters (a list: train mode): the blocks' BatchNorms use the statistics of
+    the pack's sz["count"] valid frames, update their running statistics, and append their
+    num_batches_tracked buffers for the caller to increment."""
+    training = counters is not None
     call = ops.call
     G, n = plan.geoms, len(sz["Tq"])
     P = lambda name: _flat(params[name])
@@ -780,6 +791,8 @@ def _packed_front_launch(plan, mod, x, sz, tab, params):
     g0 = G[0]
     call("pase_reflect_pad_wave_var", x, tab("wave"), n, sz["max_T"], plan.apad[0],
          plan.apad_lo[0], fmt, g0.padL, g0.padR)
+    if training:
+        plan.stats_f.zero_()
     if plan.skips:
         plan.cat[:rows * Kc].zero_()                         # the pools accumulate into it
     _conv_weight_operands(plan, P)
@@ -790,10 +803,21 @@ def _packed_front_launch(plan, mod, x, sz, tab, params):
             bias = None
         else:
             bias = P(pre + "conv.bias")
+        cs = cq = None
+        if training:
+            o = plan.fs_off[l]
+            cs, cq = plan.stats_f[o:o + g.Nn], plan.stats_f[o + g.Nn:o + 2 * g.Nn]
         plan.nt_var(("apad", l), plan.apad[l], g.lda, ("Wt", l), plan.Wt[l], g.K, g.sinc,
                     plan.y[l], g.Nn, sz["gemm_rows"][l], g.Nn, g.K, bias, tab(("gemm", l)), n,
-                    g.fold)
-        _bn_eval_affine(plan, P, buf, l, g)
+                    g.fold, cs, cq)
+        if training:
+            bn = plan.bn[l]
+            call("pase_bn_finalize", cs, cq, g.Cout, g.fold, float(sz["count"][l]),
+                 P(pre + "norm.weight"), P(pre + "norm.bias"), buf(pre + "norm.running_mean"),
+                 buf(pre + "norm.running_var"), BN_MOMENTUM, BN_EPS, bn[0], bn[1], bn[2], bn[3])
+            counters.append(mod.get_buffer(pre + "norm.num_batches_tracked"))
+        else:
+            _bn_eval_affine(plan, P, buf, l, g)
         C, sep = g.Cout, 0
         if l + 1 < plan.nblk:
             nx = G[l + 1]
@@ -816,17 +840,31 @@ def _packed_front_launch(plan, mod, x, sz, tab, params):
                     1)
 
 
-def _packed_out_proj(plan, mod, params, rows):
+def _packed_out_proj(plan, mod, params, rows, counters=None):
     """The output projection [W | skips] of `rows` packed frames into plan.yout (uniform over
-    the frames) and the eval-mode norm_out affine into plan.bn_out."""
+    the frames) and the norm_out affine into plan.bn_out: eval mode, or (counters given) the
+    statistics of the `rows` frames, as _packed_front_launch."""
     Kc, emb = plan.Kc, plan.emb
+    buf = lambda name: _flat(mod.get_buffer(name))
     _out_weights(plan, params)
+    cs = cq = None
+    if plan.norm_out and counters is not None:
+        o = plan.fs_out
+        cs, cq = plan.stats_f[o:o + emb], plan.stats_f[o + emb:o + 2 * emb]
     gemm.nt(plan.precision, plan.cat, Kc, rows * Kc, plan.Wcat, Kc, plan.yout, emb, rows, emb,
-            Kc, 1.0, _flat(params["W.bias"]),
+            Kc, 1.0, _flat(params["W.bias"]), cs=cs, cq=cq,
             a_op=lambda: plan.operand("cat", plan.cat, True, n=rows * Kc),
             b_op=lambda: plan.operand("Wcat", plan.Wcat, True, "weight"))
-    if plan.norm_out:
-        _out_bn_eval_affine(plan, lambda name: _flat(mod.get_buffer(name)))
+    if not plan.norm_out:
+        return
+    if cs is not None:
+        bo = plan.bn_out
+        ops.call("pase_bn_finalize", cs, cq, emb, 1, float(rows), None, None,
+                 buf("norm_out.running_mean"), buf("norm_out.running_var"), BN_MOMENTUM, BN_EPS,
+                 bo[0], bo[1], bo[2], bo[3])
+        counters.append(mod.get_buffer("norm_out.num_batches_tracked"))
+    else:
+        _out_bn_eval_affine(plan, buf)
 
 
 # -- packed variable-length backward (DESIGN.md section 18) -----------------------------------
@@ -940,13 +978,15 @@ def packed_grad_layout(plan, lengths, geoms, mode=None):
     return torch.from_numpy(table.astype(np.int32)), sec, sz
 
 
-def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_grads=True):
-    """Backward of the last packed_grad_layout forward on `plan` (eval mode), the packed mirror
-    of encoder_backward_steps.  gflat: the upstream gradients of the (1, emb, T'_i) outputs,
+def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_grads=True,
+                            training=False):
+    """Backward of the last packed_grad_layout forward on `plan`, the packed mirror of
+    encoder_backward_steps.  gflat: the upstream gradients of the (1, emb, T'_i) outputs,
     concatenated in output order.  dx (optional): the packed (sum T_i,) waveform gradient.
     param_grads / sink / the returned dict as in encoder_backward_steps; the parameter
-    gradients are summed over the utterances.  Launches do not depend on the number of
-    utterances."""
+    gradients are summed over the utterances.  training: the forward used the pack's batch
+    statistics, so every BatchNorm's sums S1 / S2 enter the data gradient (DESIGN.md section
+    19).  Launches do not depend on the number of utterances."""
     if not param_grads and dx is None:
         raise ValueError("encoder_backward_packed: nothing to compute (no parameter gradients, "
                          "no dx)")
@@ -979,9 +1019,15 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
         plan.w_batch(1, jobs)
     bo = plan.bn_out
     o = plan.bs_out
-    call("pase_out_bwd_gather_var", gflat, tab("out"), n, max(sz["Tq"]), emb, plan.g)
-    call("pase_out_bwd_apply", plan.g, plan.yout, bo[0], bo[1], bo[2], sb[o:o + emb],
-         sb[o + emb:o + 2 * emb], float(rows), 0, rows, emb)
+    S1o, S2o = sb[o:o + emb], sb[o + emb:o + 2 * emb]
+    use_stats = 1 if (plan.norm_out and training) else 0
+    if use_stats:
+        call("pase_out_bwd_reduce_var", gflat, tab("out"), n, max(sz["Tq"]), emb, plan.yout,
+             bo[0], bo[1], plan.g, S1o, S2o)
+    else:
+        call("pase_out_bwd_gather_var", gflat, tab("out"), n, max(sz["Tq"]), emb, plan.g)
+    call("pase_out_bwd_apply", plan.g, plan.yout, bo[0], bo[1], bo[2], S1o, S2o, float(rows),
+         use_stats, rows, emb)
     if pg:
         call("pase_colsum", plan.g, emb, rows, emb, sb[plan.bs_bw:plan.bs_bw + emb])
         plan.tn("g", plan.g, emb, rows, 0, True, "cat", plan.cat, Kc, rows, False, plan.dWcat,
@@ -1022,14 +1068,21 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
         amax = None if plan.amax is None else plan.amax[2 * l:2 * l + 2]
         o = plan.bs_off[l]
         t, mT = tab(("bwd", l)), sz["max_Tout"][l]
-        if pg or amax is not None:       # eval mode: the sums feed parameter gradients only
+        S1, S2 = sb[o:o + C], sb[o + C:o + 2 * C]
+        # eval mode: the sums feed parameter gradients only; train mode: the data gradient too
+        if pg or amax is not None or training:
             call("pase_bn_prelu_bwd_reduce_var", plan.y[l], ybf, t, n, mT, C, mean, invstd,
-                 scale, shift, P(pre + "act.weight"), *src, sb[o:o + C], sb[o + C:o + 2 * C],
-                 sb[o + 2 * C:o + 3 * C], amax)
-        call("pase_bn_prelu_bwd_apply_src_var", plan.y[l], ybf, t, n, sz["max_span"][l], C, invstd,
-             P(pre + "norm.weight"), scale, shift, P(pre + "act.weight"), *src, plan.dyz[l],
-             plan.dyz_lo[l], fmt, sz["lead"][l],
-             sb[o + 3 * C:o + 4 * C] if pg and not g.sinc else None, amax, plan.gscale[l])
+                 scale, shift, P(pre + "act.weight"), *src, S1, S2, sb[o + 2 * C:o + 3 * C],
+                 amax)
+        dst = (plan.dyz[l], plan.dyz_lo[l], fmt, sz["lead"][l],
+               sb[o + 3 * C:o + 4 * C] if pg and not g.sinc else None, amax, plan.gscale[l])
+        if training:
+            call("pase_bn_prelu_bwd_apply_src_var_train", plan.y[l], ybf, t, n,
+                 sz["max_span"][l], C, mean, invstd, P(pre + "norm.weight"), scale, shift,
+                 P(pre + "act.weight"), S1, S2, float(sz["count"][l]), *src, *dst)
+        else:
+            call("pase_bn_prelu_bwd_apply_src_var", plan.y[l], ybf, t, n, sz["max_span"][l], C,
+                 invstd, P(pre + "norm.weight"), scale, shift, P(pre + "act.weight"), *src, *dst)
         if g.sinc:
             if pg:
                 plan.tn(("dyz", l), plan.dyz[l], g.Nn, M, g.dg_rows - 1, False, ("apad", l),
@@ -1074,20 +1127,20 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
 
 
 class _PackedEncoderFn(torch.autograd.Function):
-    """Autograd node of WaveFe.encode_packed: one packed eval-mode forward of n utterances
-    (tensors = the n flat CUDA waveforms, then the parameters) and one packed backward sweep.
-    The outputs are views of one buffer."""
+    """Autograd node of WaveFe.encode_packed (eval mode) and WaveFe.encode_packed_train
+    (training): one packed forward of n utterances (tensors = the n flat CUDA waveforms, then
+    the parameters) and one packed backward sweep.  The outputs are views of one buffer."""
 
     @staticmethod
-    def forward(ctx, mod, plan, lengths, geoms, names, n, *tensors):
+    def forward(ctx, mod, plan, lengths, geoms, names, training, n, *tensors):
         params = dict(zip(names, tensors[n:]))
         plan.ensure_backward()
         x = plan.wave[:sum(lengths)]
         torch.cat(tensors[:n], out=x)
         feats = encoder_forward_packed(plan, mod, x, lengths, geoms, params, None,
-                                       packed_grad_layout)
+                                       packed_grad_layout, training)
         ctx.set_materialize_grads(False)
-        ctx.mod, ctx.plan, ctx.names, ctx.n = mod, plan, names, n
+        ctx.mod, ctx.plan, ctx.names, ctx.n, ctx.training = mod, plan, names, n, training
         ctx.generation = plan.generation
         ctx.save_for_backward(*tensors[n:])
         return tuple(feats)
@@ -1101,9 +1154,9 @@ class _PackedEncoderFn(torch.autograd.Function):
                 "encode_packed forward on the same plan before this backward ran; run backward "
                 "before the next forward.")
         params = dict(zip(ctx.names, ctx.saved_tensors))
-        need_x = ctx.needs_input_grad[6:6 + n]
-        param_grads = any(ctx.needs_input_grad[6 + n:])        # all or nothing, as _EncoderFn
-        none = (None,) * 6
+        need_x = ctx.needs_input_grad[7:7 + n]
+        param_grads = any(ctx.needs_input_grad[7 + n:])        # all or nothing, as _EncoderFn
+        none = (None,) * 7
         if not param_grads and not any(need_x):
             return none + (None,) * (n + len(ctx.names))
         sink = getattr(ctx.mod, "grad_sink", None)
@@ -1118,7 +1171,8 @@ class _PackedEncoderFn(torch.autograd.Function):
         dx = None
         if any(need_x):
             dx = torch.empty(sz["total"], dtype=torch.float32, device=plan.device)
-        grads = encoder_backward_packed(plan, ctx.mod, params, gflat, sink, dx, param_grads)
+        grads = encoder_backward_packed(plan, ctx.mod, params, gflat, sink, dx, param_grads,
+                                        ctx.training)
         dxs, o = [], 0
         for T, need in zip(sz["lengths"], need_x):
             dxs.append(dx[o:o + T] if need else None)

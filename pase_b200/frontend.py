@@ -323,25 +323,59 @@ class WaveFe(Model):
         the utterances; autograd or grad_sink).  One pack per call: the total must fit
         `max_samples` (default EXTRACT_MAX_SAMPLES).  Eval mode only."""
         device = self._eval_device("encode_packed")
+        cap = self._packed_cap(max_samples)
+        flat = self._packed_inputs(wavs)
+        if not flat:
+            return []
+        return self._encode_packed(flat, cap, device)
+
+    def encode_packed_train(self, wavs, max_samples=None):
+        """Train-mode packed encoding (DESIGN.md section 19): wavs and the returned (1, emb,
+        T'_i) CUDA views of one buffer as in encode_packed.  Every BatchNorm (each block's and
+        norm_out) normalises with the mean and biased variance over the valid frames of all
+        utterances, i.e. as nn.BatchNorm1d on their time-concatenation (1, C, sum T_i), and
+        updates its running statistics and num_batches_tracked once per call (also under
+        no_grad).  No padding enters the statistics, so with equal lengths this is the train
+        forward of the stacked (N, 1, T) batch.  With grad mode on and a waveform or a parameter
+        requiring a gradient, one autograd node backpropagates through the batch statistics to
+        every waveform and to the parameters (autograd or grad_sink, all or nothing as in
+        encode).  One pack per call: the total must fit `max_samples` (default
+        EXTRACT_MAX_SAMPLES).  Train mode only; everything is checked before any launch."""
+        if not self.training:
+            raise RuntimeError("WaveFe.encode_packed_train runs the encoder in train mode; in "
+                               "eval mode use encode_packed")
+        device = self.W.weight.device
+        if device.type != "cuda":
+            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; the module lives "
+                               "on %s. There is no CPU path." % device)
+        flat = self._packed_inputs(wavs)
+        if not flat:
+            return []
+        return self._encode_packed(flat, self._packed_cap(max_samples), device, True)
+
+    def _packed_cap(self, max_samples):
         cap = EXTRACT_MAX_SAMPLES if max_samples is None else int(max_samples)
         if cap < 1:
             raise ValueError("max_samples must be positive, got %r" % (max_samples,))
+        return cap
+
+    @staticmethod
+    def _packed_inputs(wavs):
         flat = []
         for i, w in enumerate(wavs):
             try:
                 flat.append(_recording(w))
             except (TypeError, ValueError) as e:
                 raise type(e)("utterance %d: %s" % (i, e)) from None
-        if not flat:
-            return []
-        return self._encode_packed(flat, cap, device)
+        return flat
 
-    def _encode_packed(self, flat, cap, device):
+    def _encode_packed(self, flat, cap, device, training=False):
         lengths = [w.numel() for w in flat]
+        what = "encode_packed_train" if training else "encode_packed"
         if sum(lengths) > cap:
-            raise ValueError("encode_packed: %d samples exceed max_samples=%d; one call is one "
+            raise ValueError("%s: %d samples exceed max_samples=%d; one call is one "
                              "pack, so split the list into calls that fit"
-                             % (sum(lengths), cap))
+                             % (what, sum(lengths), cap))
         fold = _gemm.PRECISIONS[self.resolved_precision()].sinc_fold
         geoms = _enc.utterance_geometry(self.cfg, lengths, fold)
         self._sinc_consts(device)
@@ -352,12 +386,13 @@ class WaveFe(Model):
         xs = [w.to(device) for w in flat]
         if torch.is_grad_enabled() and (any(w.requires_grad for w in xs) or
                                         any(p.requires_grad for p in tensors)):
-            return list(_enc._PackedEncoderFn.apply(self, plan, lengths, geoms, names, len(xs),
-                                                    *xs, *tensors))
+            return list(_enc._PackedEncoderFn.apply(self, plan, lengths, geoms, names, training,
+                                                    len(xs), *xs, *tensors))
         with torch.no_grad():
             x = plan.wave[:sum(lengths)]
             torch.cat(xs, out=x)
-            return _enc.encoder_forward_packed(plan, self, x, lengths, geoms, dict(named))
+            return _enc.encoder_forward_packed(plan, self, x, lengths, geoms, dict(named),
+                                               training=training)
 
     def _eval_device(self, what):
         if self.training:

@@ -130,16 +130,22 @@ def nt(p, A, lda, a_n, B, ldb, C, ldc, M, N, K, alpha=1.0, bias=None, rows_in=No
                     p.mode, 1 if C.dtype == torch.bfloat16 else 0)
 
 
-def nt_var(p, A, lda, a_n, B, ldb, C, ldc, M, N, K, bias, tab, n, fold, a_op=None, b_op=None):
-    """nt over a packed variable-length batch (inference): the row map is the device table `tab`
-    of n utterances (pase_gemm_nt_var); operands as for nt."""
+def nt_var(p, A, lda, a_n, B, ldb, C, ldc, M, N, K, bias, tab, n, fold, a_op=None, b_op=None,
+           cs=None, cq=None):
+    """nt over a packed variable-length batch: the row map is the device table `tab` of n
+    utterances (pase_gemm_nt_var); operands as for nt.  cs / cq (train mode): the BatchNorm
+    column statistics of the stored elements (pase_gemm_nt_var_stats)."""
+    stats = () if cs is None else (cs, cq)
+    suffix = "" if cs is None else "_stats"
     if not nt_ok(p, lda, K, ldb):
         _ffma_operands(p, "GEMM shape (lda=%d K=%d)" % (lda, K), A, B)
-        return ops.call("pase_gemm_nt_var", A, lda, B, ldb, C, ldc, M, N, K, bias, tab, n, fold)
+        return ops.call("pase_gemm_nt_var" + suffix, A, lda, B, ldb, C, ldc, M, N, K, bias, tab,
+                        n, fold, *stats)
     a = _tc_operand(a_op, p, A, a_n, "act")
     b = _tc_operand(b_op, p, B, None if B is None else B.numel(), "weight")
-    return ops.call("pase_tc_gemm_nt_var", a.hi, a.lo, a_n // lda, lda, b.hi, b.lo, ldb, C, ldc,
-                    M, N, K, bias, tab, n, fold, p.mode, 1 if C.dtype == torch.bfloat16 else 0)
+    return ops.call("pase_tc_gemm_nt_var" + suffix, a.hi, a.lo, a_n // lda, lda, b.hi, b.lo, ldb,
+                    C, ldc, M, N, K, bias, tab, n, fold, *stats, p.mode,
+                    1 if C.dtype == torch.bfloat16 else 0)
 
 
 def tn(p, A, lda, a_n, B, ldb, b_n, C, ldc, I, J, rows, groups=1, pitchA=None, offA=0,
