@@ -258,6 +258,13 @@ int pase_reflect_fold_wave(const float* dpad, long pitch, float* dx, int N, int 
  * (pase_reflect_pad_wave_var's table): dx[x_off + t] from dpad[dst_off ..]; max_T >= every T. */
 int pase_reflect_fold_wave_var(const float* dpad, const int* tab, int nseg, int max_T, float* dx,
                                int padL, int padR, void* stream);
+/* One window of a recording's backward (WaveFe.encode_long): dx[x0 + t] += the fold of the
+ * window's padded gradient dpad (T + padL + padR floats) at t, for t < T.  The mirrored pad
+ * gradient is added on the left only when fold_l != 0 and on the right only when fold_r != 0 (the
+ * sides where the window's reflect pad is the recording's own); x0 is a 64-bit offset.  Windows
+ * overlap, so dx accumulates: run them one after the other, never concurrently. */
+int pase_reflect_fold_wave_acc(const float* dpad, float* dx, long x0, int T, int padL, int padR,
+                               int fold_l, int fold_r, void* stream);
 /* batch statistics -> per-channel affine; updates running stats (training) */
 int pase_bn_finalize(const double* colsum, const double* colsumsq, int C, int fold,
                      double count, const float* gamma, const float* beta,
@@ -435,6 +442,11 @@ int pase_out_bwd_reduce(const float* dout, const float* dout_ntc, const float* y
  * max_T >= every T. */
 int pase_out_bwd_gather_var(const float* dout, const int* tab, int nseg, int max_T, int C,
                             float* g_ntc, void* stream);
+/* One window of a recording's backward (WaveFe.encode_long): g_ntc[t*C + c] = dout[c*ld + col0
+ * + t - c0] for the crop frames c0 <= t < c0+cn of the window's T frames, 0 for its other frames;
+ * dout is the recording's (C, ld) output gradient and col0 (64-bit) its column of frame c0. */
+int pase_out_bwd_gather_crop(const float* dout, long ld, long col0, int T, int c0, int cn, int C,
+                             float* g_ntc, void* stream);
 /* pase_out_bwd_gather_var with pase_out_bwd_reduce's sums (train-mode norm_out of
  * WaveFe.encode_packed_train, frontend.py:206-208): the same gather, and S1 += g,
  * S2 += g*xhat (double[C]) with xhat = (y[(row0 + t)*C + c] - mean[c]) invstd[c] over every
@@ -478,6 +490,17 @@ int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long l
  * Two launches. */
 int pase_qrnn_scan_bwd_var(const float* Y, const float* Cst, const float* dh, long lddh, float* dY,
                            const int* tab, int nseg, int H, void* stream);
+/* Backward of pase_qrnn_scan_fwd_carry_var over windows of recordings (WaveFe.encode_long):
+ * tab (DEVICE, nseg rows of 6 ints) {row0, T, drow0, c0, cn, slot}: rows row0 .. row0+T-1 of
+ * Y / Cst / dh are one window, whose frames c0 .. c0+cn-1 were scanned from row `slot` of state
+ * (nslots, H).  Their gate gradients go to rows drow0+c0 .. drow0+c0+cn-1 of dY; rows drow0 ..
+ * drow0+T of dY outside them are written zero.  The scan starts from the cell-state gradient in
+ * row `slot` of dstate and writes there the gradient of that row of state.  The per-step
+ * arithmetic is pase_qrnn_scan_bwd's sequential kernel's.  A slot appears at most once per
+ * call. */
+int pase_qrnn_scan_bwd_carry_var(const float* Y, const float* Cst, const float* dh, long lddh,
+                                 float* dY, const float* state, float* dstate, const int* tab,
+                                 int nseg, int H, void* stream);
 /* Which kernels the two scans run for T time steps (host only, launches nothing): out1 =
  * segments per block of the time-segmented kernels (16, 24 or 32; T <= 512), or 0 for the
  * sequential kernels (T > 512). */

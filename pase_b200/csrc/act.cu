@@ -962,6 +962,20 @@ out_bwd_gather_var_kernel(const float* __restrict__ dout, const int* __restrict_
   }
 }
 
+// One window of a recording (WaveFe.encode_long): g[t*C + c] = dout[c*ld + col0 + t - c0] for
+// the crop frames c0 <= t < c0+cn, 0 for the window's other frames t < T
+__global__ void __launch_bounds__(256)
+out_bwd_gather_crop_kernel(const float* __restrict__ dout, long ld, long col0, int T, int c0,
+                           int cn, int C, float* __restrict__ g) {
+  pdl_wait();
+  const long total = (long)T * C;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i / T), t = (int)(i - (long)c * T);
+    g[(long)t * C + c] = (t >= c0 && t < c0 + cn) ? dout[c * ld + col0 + (t - c0)] : 0.f;
+  }
+}
+
 // ---- plain PReLU on (rows, C) ----
 __global__ void prelu_fwd_kernel(const float* __restrict__ u, float* __restrict__ h,
                                  const float* __restrict__ alpha, long rows, int C, long ldu,
@@ -2053,6 +2067,21 @@ int pase_out_bwd_gather_var(const float* dout, const int* tab, int nseg, int max
   PASE_LAUNCH((out_bwd_gather_var_kernel), dim3((unsigned)bx, nseg), 256, 0, (cudaStream_t)stream,
               dout, tab, C, g_ntc);
   PASE_LAUNCH_CHECK("pase_out_bwd_gather_var");
+  return PASE_OK;
+}
+
+int pase_out_bwd_gather_crop(const float* dout, long ld, long col0, int T, int c0, int cn, int C,
+                             float* g_ntc, void* stream) {
+  PASE_CHECK_ARG(dout && g_ntc && T > 0 && C > 0 && c0 >= 0 && cn > 0 && c0 + cn <= T &&
+                     col0 >= 0 && col0 + cn <= ld,
+                 "pase_out_bwd_gather_crop: bad args (T=%d crop %d+%d, col0=%ld ld=%ld)", T, c0,
+                 cn, col0, ld);
+  const long total = (long)T * C;
+  long bx = (total + 255) / 256;
+  if (bx > 1024) bx = 1024;
+  PASE_LAUNCH((out_bwd_gather_crop_kernel), dim3((unsigned)bx), 256, 0, (cudaStream_t)stream, dout,
+              ld, col0, T, c0, cn, C, g_ntc);
+  PASE_LAUNCH_CHECK("pase_out_bwd_gather_crop");
   return PASE_OK;
 }
 

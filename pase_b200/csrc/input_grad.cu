@@ -87,6 +87,22 @@ reflect_fold_wave_var_kernel(const float* __restrict__ dpad, const int* __restri
   }
 }
 
+// One window of a recording (WaveFe.encode_long): dx[x0 + t] += the window's padded-waveform
+// gradient at t, with the mirrored pad gradient added only on the sides where the window's pad is
+// the recording's own (fold_l / fold_r)
+__global__ void __launch_bounds__(THREADS)
+reflect_fold_wave_acc_kernel(const float* __restrict__ d, float* __restrict__ dx, long x0, int T,
+                             int padL, int padR, int fold_l, int fold_r) {
+  pdl_wait();
+  float* o = dx + x0;
+  for (int t = blockIdx.x * THREADS + threadIdx.x; t < T; t += gridDim.x * THREADS) {
+    float v = d[t + padL];
+    if (fold_l && t >= 1 && t <= padL) v += d[padL - t];                           // left mirror
+    if (fold_r && t >= T - 1 - padR && t <= T - 2) v += d[padL + 2 * (T - 1) - t]; // right mirror
+    o[t] += v;
+  }
+}
+
 inline unsigned grid_for(long total) {
   long b = (total + THREADS - 1) / THREADS;
   const long cap = (long)pase_num_sms() * 16;
@@ -161,5 +177,16 @@ int pase_reflect_fold_wave_var(const float* dpad, const int* tab, int nseg, int 
   PASE_LAUNCH((reflect_fold_wave_var_kernel), grid, THREADS, 0, (cudaStream_t)stream, dpad, tab,
               dx, padL, padR);
   PASE_LAUNCH_CHECK("pase_reflect_fold_wave_var");
+  return PASE_OK;
+}
+
+int pase_reflect_fold_wave_acc(const float* dpad, float* dx, long x0, int T, int padL, int padR,
+                               int fold_l, int fold_r, void* stream) {
+  PASE_CHECK_ARG(dpad && dx && x0 >= 0 && T > 0 && padL >= 0 && padR >= 0 && padL < T &&
+                     padR < T, "pase_reflect_fold_wave_acc: bad args (x0=%ld T=%d pad %d,%d)", x0,
+                 T, padL, padR);
+  PASE_LAUNCH((reflect_fold_wave_acc_kernel), dim3((unsigned)((T + THREADS - 1) / THREADS)),
+              THREADS, 0, (cudaStream_t)stream, dpad, dx, x0, T, padL, padR, fold_l, fold_r);
+  PASE_LAUNCH_CHECK("pase_reflect_fold_wave_acc");
   return PASE_OK;
 }

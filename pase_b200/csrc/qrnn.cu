@@ -77,6 +77,60 @@ qrnn_scan_fwd_carry_var_kernel(const float* __restrict__ Y, float* __restrict__ 
                      c0);
 }
 
+// One sample's sequential backward scan of hidden unit c over its T steps, last to first: y /
+// cp / dhp / dy point at its first step, cm0 is the cell state before it and carry the cell-state
+// gradient entering from after its last step.  Returns the gradient of cm0.  The per-step
+// arithmetic is that of qrnn_scan_bwd_kernel and qrnn_scan_bwd_seq_var_kernel below (whose cm0
+// and carry are 0), in an unrolled group or in the remainder alike, so a backward cut into
+// windows that carry the gradient reproduces the whole scan's bits (pase_qrnn_scan_bwd_carry_var).
+// Those two kernels keep their own copies of the loop: routing them through this function
+// changes their SASS.
+__device__ __forceinline__ float qrnn_bwd_seq(const float* __restrict__ y,
+                                              const float* __restrict__ cp,
+                                              const float* __restrict__ dhp, long lddh,
+                                              float* __restrict__ dy, int T, int H, float cm0,
+                                              float carry) {
+  int t = T - 1;
+  // the loads do not depend on the recurrence: issue UNROLL time steps of them up front
+  for (; t - (UNROLL - 1) >= 0; t -= UNROLL) {
+    float z[UNROLL], f[UNROLL], o[UNROLL], c[UNROLL], cm[UNROLL], g[UNROLL];
+#pragma unroll
+    for (int i = 0; i < UNROLL; ++i) {
+      const int tt = t - i;
+      const float* yr = y + (long)tt * 3 * H;
+      z[i] = yr[0]; f[i] = yr[H]; o[i] = yr[2 * H];
+      c[i] = cp[(long)tt * H];
+      cm[i] = tt > 0 ? cp[(long)(tt - 1) * H] : cm0;
+      g[i] = dhp[(long)tt * lddh];
+    }
+#pragma unroll
+    for (int i = 0; i < UNROLL; ++i) {
+      const int tt = t - i;
+      const float zz = tanhf(z[i]), ff = sigmoidf_(f[i]), oo = sigmoidf_(o[i]);
+      const float dc = g[i] * oo + carry;
+      carry = dc * (1.f - ff);
+      float* dr = dy + (long)tt * 3 * H;
+      dr[0] = dc * ff * (1.f - zz * zz);
+      dr[H] = dc * (zz - cm[i]) * ff * (1.f - ff);
+      dr[2 * H] = g[i] * c[i] * oo * (1.f - oo);
+    }
+  }
+  for (; t >= 0; --t) {
+    const float* yr = y + (long)t * 3 * H;
+    const float zz = tanhf(yr[0]), ff = sigmoidf_(yr[H]), oo = sigmoidf_(yr[2 * H]);
+    const float ct = cp[(long)t * H];
+    const float cm1 = t > 0 ? cp[(long)(t - 1) * H] : cm0;
+    const float g = dhp[(long)t * lddh];
+    const float dc = g * oo + carry;
+    carry = dc * (1.f - ff);
+    float* dr = dy + (long)t * 3 * H;
+    dr[0] = dc * ff * (1.f - zz * zz);
+    dr[H] = dc * (zz - cm1) * ff * (1.f - ff);
+    dr[2 * H] = g * ct * oo * (1.f - oo);
+  }
+  return carry;
+}
+
 __global__ void __launch_bounds__(128)
 qrnn_scan_bwd_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
                      const float* __restrict__ dh, long lddh, float* __restrict__ dY, int T,
@@ -425,6 +479,35 @@ qrnn_scan_bwd_seq_var_kernel(const float* __restrict__ Y, const float* __restric
   }
 }
 
+// Backward of one window's carried scan (WaveFe.encode_long): tab row {row0, T, drow0, c0, cn,
+// slot} per window (blockIdx.y).  Rows row0 .. row0+T-1 of Y / Cst / dh are the window's frames,
+// of which c0 .. c0+cn-1 (its crop) were scanned from state[slot]; the gate gradients of the crop
+// go to rows drow0+c0 .. of dY, every other row of drow0 .. drow0+T (the separator included) is
+// written zero.  The scan starts from the cell-state gradient dstate[slot] (the next window's
+// gradient of this window's last state) and leaves there the gradient of state[slot].
+__global__ void __launch_bounds__(128)
+qrnn_scan_bwd_carry_var_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
+                               const float* __restrict__ dh, long lddh, float* __restrict__ dY,
+                               const float* __restrict__ state, float* __restrict__ dstate,
+                               const int* __restrict__ tab, int H) {
+  pdl_wait();
+  const int* r = tab + 6 * blockIdx.y;
+  const long row0 = __ldg(r), drow0 = __ldg(r + 2), slot = __ldg(r + 5);
+  const int T = __ldg(r + 1), c0 = __ldg(r + 3), cn = __ldg(r + 4);
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= H) return;
+  float* dy = dY + drow0 * 3 * H + c;
+  for (int t = 0; t <= T; ++t) {
+    if (t >= c0 && t < c0 + cn) continue;
+    float* dr = dy + (long)t * 3 * H;
+    dr[0] = 0.f; dr[H] = 0.f; dr[2 * H] = 0.f;
+  }
+  float* ds = dstate + slot * H + c;
+  *ds = qrnn_bwd_seq(Y + (row0 + c0) * 3 * H + c, Cst + (row0 + c0) * H + c,
+                     dh + (row0 + c0) * lddh + c, lddh, dy + (long)c0 * 3 * H, cn, H,
+                     state[slot * H + c], *ds);
+}
+
 }  // namespace
 
 extern "C" {
@@ -517,6 +600,19 @@ int pase_qrnn_scan_bwd_var(const float* Y, const float* Cst, const float* dh, lo
   PASE_LAUNCH((qrnn_scan_bwd_seq_var_kernel), dim3((H + 127) / 128, nseg), 128, 0, st, Y, Cst, dh,
               lddh, dY, tab, H);
   PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd_var");
+  return PASE_OK;
+}
+
+int pase_qrnn_scan_bwd_carry_var(const float* Y, const float* Cst, const float* dh, long lddh,
+                                 float* dY, const float* state, float* dstate, const int* tab,
+                                 int nseg, int H, void* stream) {
+  PASE_CHECK_ARG(Y && Cst && dh && dY && state && dstate && tab,
+                 "pase_qrnn_scan_bwd_carry_var: null pointer");
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535 && H > 0 && lddh >= H,
+                 "pase_qrnn_scan_bwd_carry_var: nseg=%d H=%d lddh=%ld", nseg, H, lddh);
+  PASE_LAUNCH((qrnn_scan_bwd_carry_var_kernel), dim3((H + 127) / 128, nseg), 128, 0,
+              (cudaStream_t)stream, Y, Cst, dh, lddh, dY, state, dstate, tab, H);
+  PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd_carry_var");
   return PASE_OK;
 }
 

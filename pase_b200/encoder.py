@@ -979,14 +979,20 @@ def packed_grad_layout(plan, lengths, geoms, mode=None):
 
 
 def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_grads=True,
-                            training=False):
+                            training=False, window=None):
     """Backward of the last packed_grad_layout forward on `plan`, the packed mirror of
     encoder_backward_steps.  gflat: the upstream gradients of the (1, emb, T'_i) outputs,
     concatenated in output order.  dx (optional): the packed (sum T_i,) waveform gradient.
     param_grads / sink / the returned dict as in encoder_backward_steps; the parameter
     gradients are summed over the utterances.  training: the forward used the pack's batch
     statistics, so every BatchNorm's sums S1 / S2 enter the data gradient (DESIGN.md section
-    19).  Launches do not depend on the number of utterances."""
+    19).  Launches do not depend on the number of utterances.
+
+    window (WaveFe.encode_long, DESIGN.md section 20): the pack is one window of a recording
+    recomputed by _window_forward, a dict of _window_backward's.  Then three launches differ:
+    the cotangent is the crop's columns of the recording's gradient (gflat unused), the QRNN
+    scan carries the cell-state gradient across windows, and dx is the recording's gradient,
+    into which the window's waveform gradient is added at its offset."""
     if not param_grads and dx is None:
         raise ValueError("encoder_backward_packed: nothing to compute (no parameter gradients, "
                          "no dx)")
@@ -1021,7 +1027,10 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
     o = plan.bs_out
     S1o, S2o = sb[o:o + emb], sb[o + emb:o + 2 * emb]
     use_stats = 1 if (plan.norm_out and training) else 0
-    if use_stats:
+    if window is not None:
+        call("pase_out_bwd_gather_crop", window["gout"], window["ld"], window["col0"], rows,
+             window["crop_f0"], window["crop_n"], emb, plan.g)
+    elif use_stats:
         call("pase_out_bwd_reduce_var", gflat, tab("out"), n, max(sz["Tq"]), emb, plan.yout,
              bo[0], bo[1], plan.g, S1o, S2o)
     else:
@@ -1039,8 +1048,12 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
 
     if plan.rnn:
         Cq, H, R = plan.Clast, plan.H, sz["xq_rows"]
-        call("pase_qrnn_scan_bwd_var", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg, tab("qbwd"),
-             n, H)
+        if window is not None:
+            call("pase_qrnn_scan_bwd_carry_var", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg,
+                 window["state"], window["dstate"], tab("qcarry"), 1, H)
+        else:
+            call("pase_qrnn_scan_bwd_var", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg,
+                 tab("qbwd"), n, H)
         if pg:
             call("pase_colsum", plan.dYg, 3 * H, R, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
             plan.tn("dYg", plan.dYg, 3 * H, R, 0, True, "xq", plan.xq, Cq, R, False, plan.dWq,
@@ -1107,8 +1120,13 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
                 plan.nt(("dyz", l), plan.dyz[l], g.Nn, False, "Wdg", plan.Wdg, g.dg_K, True,
                         plan.dxpad[0], f, M, f, g.dg_K, 1.0, None, M, M, M, 1, None, None, 0,
                         akind="grad")
-                call("pase_reflect_fold_wave_var", plan.dxpad[0], tab("wave"), n,
-                     sz["max_T"], dx, g.padL, g.padR)
+                if window is not None:
+                    call("pase_reflect_fold_wave_acc", plan.dxpad[0], dx, window["seg_start"],
+                         sz["total"], g.padL, g.padR, int(window["fold_l"]),
+                         int(window["fold_r"]))
+                else:
+                    call("pase_reflect_fold_wave_var", plan.dxpad[0], tab("wave"), n,
+                         sz["max_T"], dx, g.padL, g.padR)
         else:
             if pg:
                 plan.tn(("dyz", l), plan.dyz[l], C, M, g.taps - 1, False, ("apad", l),
@@ -1417,6 +1435,135 @@ def plan_windows(cfg, L, window):
         if seg is not None:
             segs.append(seg)
     return segs
+
+
+# -- gradients through one long recording (DESIGN.md section 20) ----------------------------
+def _window_layout(seg):
+    """packed_grad_layout of one window (segment `seg`) as a one-utterance pack, plus two
+    sections: "carry" {crop_f0, crop_n, 0, 0}, the recomputed scan over the crop from a one-row
+    state, and "qcarry" {0, T', 0, crop_f0, crop_n, 0}, its backward."""
+    def layout(plan, lengths, geoms, mode=None):
+        host, sec, sz = packed_grad_layout(plan, lengths, geoms, mode)
+        c0, cn = seg["crop_f0"], seg["crop_n"]
+        extra = torch.tensor([c0, cn, 0, 0, 0, sz["Tq"][0], 0, c0, cn, 0], dtype=torch.int32)
+        sec["carry"], sec["qcarry"] = host.numel(), host.numel() + 4
+        host = torch.cat([host, extra])
+        assert host.numel() <= plan.table.numel()
+        return host, sec, sz
+    return layout
+
+
+def _window_forward(plan, mod, wav, seg, k, geom, params, log, state):
+    """Recompute window k of a recording on `plan` as a one-utterance pack (its samples copied
+    into plan.wave): the packed front end, the crop's QRNN scan continued from row k of the
+    state log (the sequential body, as the windowed forward ran it) and the output projection.
+    Bumps plan.generation, as every forward through a packed plan does."""
+    s, n = seg["seg_start"], seg["seg_len"]
+    plan.generation += 1
+    x = plan.wave[:n]
+    x.copy_(wav[s:s + n])
+    sz, tab = _packed_front(plan, mod, x, [n], [geom], params, None, _window_layout(seg))
+    if plan.rnn:
+        if not plan.skips:        # frames outside the crop: no scan writes their QRNN columns
+            plan.cat[:sz["rows"] * plan.Kc].zero_()
+        state.copy_(log[k])
+        ops.call("pase_qrnn_scan_fwd_carry_var", plan.Yg, plan.cat, plan.Kc, plan.Cst, state,
+                 tab("carry"), 1, plan.H)
+    _packed_out_proj(plan, mod, params, sz["rows"])
+
+
+def _window_backward(plan, mod, params, wav, segs, log, gout, dx, param_grads, sink):
+    """Backward of a recording windowed into `segs` (plan_windows) whose forward logged the
+    QRNN state entering each window in `log` (nseg, H): the windows in reverse order, each
+    recomputed (_window_forward) and differentiated by encoder_backward_packed with a cotangent
+    that is zero outside its crop.  The cell-state gradient is carried from each window to the
+    one before it; dx (the recording's, zeroed) accumulates every window's waveform gradient.
+    param_grads: the gradients of every parameter are summed over the windows in fp32, in a
+    fixed order (last window first), into one flat buffer; then they go to `sink` (a dict of destinations, written
+    once) or are returned as a dict of views of that buffer."""
+    cfg, H, emb = plan.cfg, plan.H, plan.emb
+    hop, L = hop_size(cfg), wav.numel()
+    geoms = utterance_geometry(cfg, [sg["seg_len"] for sg in segs], plan.precision.sinc_fold)
+    T = gout.shape[-1]
+    gout = gout.reshape(emb, T).contiguous()
+    f32 = dict(dtype=torch.float32, device=plan.device)
+    state = torch.empty(max(H, 1), **f32)
+    dstate = torch.zeros(max(H, 1), **f32)
+    acc = part = None
+    if param_grads:
+        names = list(params)
+        sizes = [params[nm].numel() for nm in names]
+        acc, part = torch.empty(sum(sizes), **f32), torch.empty(sum(sizes), **f32)
+        views = lambda flat: dict(zip(names, [v.view(params[nm].shape) for nm, v in
+                                              zip(names, flat.split(sizes))]))
+        acc_sink, part_sink = views(acc), views(part)
+    for k in range(len(segs) - 1, -1, -1):
+        seg = segs[k]
+        _window_forward(plan, mod, wav, seg, k, geoms[k], params, log, state)
+        s, n = seg["seg_start"], seg["seg_len"]
+        win = dict(gout=gout, ld=T, col0=s // hop + seg["crop_f0"], crop_f0=seg["crop_f0"],
+                   crop_n=seg["crop_n"], state=log[k], dstate=dstate, seg_start=s, fold_l=s == 0,
+                   fold_r=s + n == L)
+        first = k == len(segs) - 1
+        encoder_backward_packed(plan, mod, params, None,
+                                (acc_sink if first else part_sink) if param_grads else None,
+                                dx, param_grads, window=win)
+        if param_grads and not first:
+            ops.call("pase_axpy", part, acc, acc.numel(), 1.0)
+    if not param_grads:
+        return {}
+    if sink is None:
+        return acc_sink
+    rows = [[acc_sink[nm].data_ptr(), sink[nm].data_ptr(), 1, acc_sink[nm].numel(),
+             acc_sink[nm].numel(), acc_sink[nm].numel()] for nm in acc_sink]
+    table = torch.tensor(rows, dtype=torch.int64).reshape(-1).to(plan.device)
+    ops.call("pase_scatter_copy", table, len(rows), acc.numel())
+    return {}
+
+
+class _LongEncoderFn(torch.autograd.Function):
+    """Autograd node of WaveFe.encode_long: the windowed forward of one recording (a one-stream
+    StreamPool push, as WaveFe.extract_long runs it) with the QRNN state entering each window
+    logged, and a backward that recomputes the windows one at a time (_window_backward).
+    Saves the waveform, the parameters, the state log and the host window list; no
+    activation."""
+
+    @staticmethod
+    def forward(ctx, mod, pool, window, segs, names, x, *tensors):
+        L, H, emb = x.numel(), pool.plan.H, mod.emb_dim
+        T = frame_counts(mod.cfg, L)[-1]
+        out = torch.empty(emb, T, dtype=torch.float32, device=x.device)
+        log = torch.zeros(len(segs), max(H, 1), dtype=torch.float32, device=x.device)
+        sid = pool.open()
+        try:
+            pool._push({sid: x}, [sid], out, iter(log))
+        finally:
+            pool._release(sid)
+        ctx.set_materialize_grads(False)
+        ctx.mod, ctx.window, ctx.segs, ctx.names, ctx.log = mod, window, segs, names, log
+        ctx.save_for_backward(x, *tensors)
+        return out.view(1, emb, T)
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, *tensors = ctx.saved_tensors        # raises if any was modified in place since
+        need_x = ctx.needs_input_grad[5]
+        param_grads = any(ctx.needs_input_grad[6:])          # all or nothing, as _EncoderFn
+        none = (None,) * 5
+        if gout is None or not (need_x or param_grads):
+            return none + (None,) * (1 + len(tensors))
+        mod = ctx.mod
+        sink = getattr(mod, "grad_sink", None) if param_grads else None
+        if sink is not None and any(nm not in sink for nm in ctx.names):
+            raise RuntimeError("pase_b200: WaveFe.grad_sink must name every parameter "
+                               "(missing %s)" % [nm for nm in ctx.names if nm not in sink][:3])
+        plan = mod._grad_plan(window_capacity(mod.cfg, ctx.window), x.device)
+        mod._sinc_consts(x.device)
+        dx = torch.zeros(x.numel(), dtype=torch.float32, device=x.device) if need_x else None
+        params = dict(zip(ctx.names, tensors))
+        grads = _window_backward(plan, mod, params, x, ctx.segs, ctx.log, gout, dx, param_grads,
+                                 sink)
+        return none + (dx,) + tuple(grads.get(nm) for nm in ctx.names)
 
 
 def encoder_backward(plan, mod, params, gout, gntc, training, sink=None, dx=None,

@@ -431,13 +431,7 @@ class WaveFe(Model):
             x = x.to(device)
         T, emb = _enc.frame_counts(cfg, L)[-1], self.emb_dim
         E = emb * (2 if mode in ("avg_concat", "avg_norm_concat") else 1)
-        # one cached one-stream pool (its ring and staging) per (window, device, precision)
-        key = (win, str(device), self.resolved_precision())
-        if self._long_pool is None or self._long_pool[0] != key:
-            self._long_pool = None
-            self._long_pool = (key, StreamPool(self, device, 1, win,
-                                               _enc.window_capacity(cfg, win)))
-        pool = self._long_pool[1]
+        pool = self._long_stream_pool(win, device)
         out = torch.empty(E, T, dtype=torch.float32, device=device)
         sid = pool.open()
         try:                        # the whole recording as one push: plan_windows' segments
@@ -447,6 +441,66 @@ class WaveFe(Model):
         if mode is not None:
             _ops.call("pase_out_select", out, T, emb, _enc.OUT_MODES[mode])
         return out.view(1, E, T)
+
+    def _long_stream_pool(self, win, device):
+        """The cached one-stream pool (its ring and staging) of extract_long and encode_long,
+        one per (window, device, precision)."""
+        key = (win, str(device), self.resolved_precision())
+        if self._long_pool is None or self._long_pool[0] != key:
+            self._long_pool = None
+            self._long_pool = (key, StreamPool(self, device, 1, win,
+                                               _enc.window_capacity(self.cfg, win)))
+        return self._long_pool[1]
+
+    def encode_long(self, wav, window=None):
+        """Differentiable encoding of one recording of any length in bounded memory (DESIGN.md
+        section 20).  wav: fp32 (T,), (1,T) or (1,1,T) on the module's CUDA device.  Returns the
+        (1, emb, T') features of ``extract_long(wav, mode=None, window=window)``: the same
+        segments and bits.  With grad mode on and the waveform or a parameter requiring a
+        gradient, one autograd node backpropagates to the waveform and to the parameters
+        (summed over the recording; autograd or grad_sink, all or nothing as in encode; a frozen
+        encoder runs the data-gradient sweep only).  Its backward recomputes one window at a
+        time on the PackedGradPlan of encoder.window_capacity(window) samples, which it may
+        share with encode_packed: running it bumps that plan's generation, so a pending
+        encode_packed backward on the same plan raises.  Memory is bounded by that plan, the
+        forward's plan and O(T) tensors.  A recording of at most `window` samples is
+        ``encode_packed([wav], max_samples=window)[0]``.  Eval mode only; select_output modes are
+        torch ops on the result.  Everything is checked before any launch."""
+        return self._encode_long(wav, window, self._eval_device("encode_long"))
+
+    def _encode_long(self, wav, window, device):
+        x = _recording(wav)
+        if x.device != device:
+            raise RuntimeError("WaveFe.encode_long: the recording lives on %s, the module on "
+                               "%s; move it to the module's device (its gradient is returned "
+                               "there)" % (x.device, device))
+        win = EXTRACT_LONG_WINDOW if window is None else int(window)
+        cfg, L = self.cfg, x.numel()
+        if win < _enc.min_window(cfg):
+            raise ValueError("window must be at least %d samples, got %d"
+                             % (_enc.min_window(cfg), win))
+        if L < _enc.min_length(cfg):
+            raise ValueError("a recording of %d samples is shorter than the encoder's minimum "
+                             "of %d" % (L, _enc.min_length(cfg)))
+        if L <= win:
+            return self._encode_packed([x], win, device)[0]
+        _enc.check_windowable(cfg, L)
+        segs = _enc.plan_windows(cfg, L, win)
+        named = list(self.named_parameters())
+        names = tuple(n for n, _ in named)
+        tensors = [p for _, p in named]
+        pool = self._long_stream_pool(win, device)
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in tensors)):
+            return _enc._LongEncoderFn.apply(self, pool, win, segs, names, x, *tensors)
+        T = _enc.frame_counts(cfg, L)[-1]
+        out = torch.empty(self.emb_dim, T, dtype=torch.float32, device=device)
+        sid = pool.open()
+        try:
+            with torch.no_grad():
+                pool._push({sid: x}, [sid], out)
+        finally:
+            pool._release(sid)
+        return out.view(1, self.emb_dim, T)
 
     def stream(self, mode=None, window=None):
         """A FeatureStream over this encoder: push() samples as they arrive, get back the
@@ -606,9 +660,12 @@ class StreamPool(object):
         planned, before the first launch: a call that raises changes no stream."""
         return self._push(blocks, finish, None)
 
-    def _push(self, blocks, finish, out):
+    def _push(self, blocks, finish, out, state_log=None):
         """push(), writing the frames into `out` (None: a new buffer) as consecutive (emb, n)
-        blocks, one per id in the order of blocks then finish."""
+        blocks, one per id in the order of blocks then finish.  state_log (WaveFe.encode_long):
+        an iterator over zeroed (H,) device rows; the QRNN state entering each segment, in the
+        order the segments run, is copied into the next one (a stream's first segment starts
+        from zero and leaves its row as it is)."""
         m, emb = self.model, self.model.emb_dim
         if m.training:
             raise RuntimeError("WaveFe.streams runs the encoder in eval mode; call .eval() first")
@@ -654,7 +711,7 @@ class StreamPool(object):
         with torch.no_grad():
             for r in range(max((len(s) for s in steps.values()), default=0)):
                 entries = [(i, steps[i][r]) for i in ids if r < len(steps[i])]
-                self._round(entries, out, ocol, new, params)
+                self._round(entries, out, ocol, new, params, state_log)
         for i in ids:                                  # commit
             self._streams[i].n, self._streams[i].done, self._streams[i].keep = new[i]
         for i in fin:
@@ -693,7 +750,7 @@ class StreamPool(object):
             steps[i], new[i] = out, (n, done, keep)
         return steps, new
 
-    def _round(self, entries, out, ocol, new, params):
+    def _round(self, entries, out, ocol, new, params, state_log=None):
         """One round: stage the new samples, upload one table for every pack, then per pack the
         gather, the packed front end, the carried scan, the output projection and the place."""
         cfg, plan, emb = self.cfg, self.plan, self.model.emb_dim
@@ -739,7 +796,8 @@ class StreamPool(object):
                                    stage_off[i], 0, 0, 0, 0])
             if not g_rows:
                 continue
-            job = dict(segs=len(pk), gather=(off, len(g_rows)))
+            job = dict(segs=len(pk), gather=(off, len(g_rows)),
+                       entering=[(self._streams[i].slot, e[2]) for i, e in pk])
             parts.append(np.asarray(g_rows, dtype=np.int64).reshape(-1))
             off += parts[-1].size
             job["max_len"] = max(max(r[2], r[6]) for r in g_rows)
@@ -775,6 +833,12 @@ class StreamPool(object):
             _enc._packed_front_launch(plan, self.model, plan.wave, sz,
                                       lambda name, sec=sec: tab[sec[name]:], params)
             if plan.rnn:
+                if state_log is not None:
+                    H = plan.H
+                    for slot, d0 in job["entering"]:
+                        row = next(state_log)
+                        if d0 > 0:
+                            row.copy_(self.state[slot * H:(slot + 1) * H])
                 call("pase_qrnn_scan_fwd_carry_var", plan.Yg, plan.cat, plan.Kc, plan.Cst,
                      self.state, tab[job["carry"]:], job["segs"], plan.H)
             _enc._packed_out_proj(plan, self.model, params, sz["rows"])
