@@ -10,6 +10,9 @@
  * as /root/reference/<file>:<line>.
  *
  * Conventions
+ *   - the packed and windowed entry points (*_var, pase_stream_gather) give each table row
+ *     (utterance, segment or stream) one grid row: nseg / nrow must be in 1..65535, anything
+ *     else is refused (PASE_ERR_ARG) before a launch;
  *   - all pointers are DEVICE pointers into buffers owned by the caller
  *     (PyTorch caching allocator); the library allocates nothing persistent;
  *   - activations are channel-last: (sample, time, channel), fp32;
@@ -231,7 +234,7 @@ int pase_sinc_grad(const float* dWp, const float* low_hz, const float* band_hz,
 int pase_reflect_pad_wave(const float* x, void* dst, void* dst_lo, int dst_fmt, int N, int T,
                           int padL, int padR, long pitch, void* stream);
 /* Packed variable-length form: tab (DEVICE, nseg rows of 3 ints) {x_off, T, dst_off}: utterance
- * x[x_off, +T) reflect-padded into dst[dst_off, +T+padL+padR); max_T >= every T. */
+ * x[x_off, +T) reflect-padded into dst[dst_off, +T+padL+padR); max_T >= every T; nseg <= 65535. */
 int pase_reflect_pad_wave_var(const float* x, const int* tab, int nseg, int max_T, void* dst,
                               void* dst_lo, int dst_fmt, int padL, int padR, void* stream);
 
@@ -289,7 +292,8 @@ int pase_bn_prelu_pad_fwd(const void* y, int y_bf16, long y_sample_stride, int N
  * and its own dense-skip pool (pool_d, pool_T; pool_T * pool_d <= T) into
  * pool[pool_off + j*pool_row_stride + c] (pool zeroed by the caller; NULL: no pool).  sep != 0
  * also writes zeros to the row ahead of each utterance (dst_off - dst_row_stride, C elements):
- * the x_{t-1} of the QRNN's first step.  max_T >= every T.  One launch for all utterances. */
+ * the x_{t-1} of the QRNN's first step.  max_T >= every T, nseg <= 65535.  One launch for all
+ * utterances. */
 int pase_bn_prelu_pad_fwd_var(const void* y, int y_bf16, const int* tab, int nseg, int max_T,
                               int C, const float* scale, const float* shift, const float* alpha,
                               void* dst, void* dst_lo, int dst_fmt, long dst_row_stride,
@@ -419,7 +423,7 @@ int pase_out_affine_nct(const float* y, const float* scale, const float* shift,
  * tab (DEVICE, nseg rows of 3 ints) {y_row, T, out_off}; h = y[y_row + t, :]*scale+shift;
  * mode 0: out[out_off..] (C,T) = h; 1 (avg_norm): h - mean_t h; 2 (avg_concat): (2C,T) =
  * [h ; mean_t h]; 3 (avg_norm_concat): [h - mean_t h ; mean_t h].  The time mean is a double
- * sum in a fixed order. */
+ * sum in a fixed order.  nseg <= 65535. */
 int pase_out_affine_var(const float* y, const float* scale, const float* shift, float* out,
                         const int* tab, int nseg, int C, int mode, void* stream);
 /* Windowed output of many streams' crops at once (StreamPool, so FeatureStream and
@@ -470,7 +474,7 @@ int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst,
                        int N, int T, int H, void* stream);
 /* Packed variable-length forward: tab (DEVICE, nseg rows of 2 ints) {row0, T}: rows row0 ..
  * row0+T-1 of Y / h / Cst are one utterance.  Each utterance runs the kernel its own T selects
- * (pase_qrnn_scan_plan), so its result is that of a B=1 scan.  Two launches. */
+ * (pase_qrnn_scan_plan), so its result is that of a B=1 scan.  nseg <= 65535.  Two launches. */
 int pase_qrnn_scan_fwd_var(const float* Y, float* h, long ldh, float* Cst, const int* tab,
                            int nseg, int H, void* stream);
 /* Sequential scans continued over windows of many streams at once (StreamPool, so FeatureStream

@@ -1431,7 +1431,8 @@ int pase_reflect_pad_wave(const float* x, void* dst, void* dst_lo, int dst_fmt, 
 
 int pase_reflect_pad_wave_var(const float* x, const int* tab, int nseg, int max_T, void* dst,
                               void* dst_lo, int dst_fmt, int padL, int padR, void* stream) {
-  PASE_CHECK_ARG(x && tab && dst && nseg > 0 && max_T > 0, "pase_reflect_pad_wave_var: bad args");
+  PASE_CHECK_ARG(x && tab && dst && nseg > 0 && nseg <= 65535 && max_T > 0,
+                 "pase_reflect_pad_wave_var: bad args (nseg=%d max_T=%d)", nseg, max_T);
   PASE_CHECK_ARG(padL < max_T && padR < max_T && padL >= 0 && padR >= 0,
                  "pase_reflect_pad_wave_var: reflect pad (%d,%d)", padL, padR);
   PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2 && (dst_fmt != PASE_FMT_F16X2 || dst_lo),
@@ -1533,7 +1534,7 @@ int pase_bn_prelu_pad_fwd_var(const void* y, int y_bf16, const int* tab, int nse
                               void* stream) {
   const char* fn = "pase_bn_prelu_pad_fwd_var";
   PASE_CHECK_ARG(y && tab && dst && scale && shift && alpha, "%s: null pointer", fn);
-  PASE_CHECK_ARG(nseg > 0 && max_T > 0 && C > 0 && (C % 4) == 0,
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535 && max_T > 0 && C > 0 && (C % 4) == 0,
                  "%s: nseg=%d max_T=%d C=%d (C a positive multiple of 4)", fn, nseg, max_T, C);
   PASE_CHECK_ARG(padL >= 0 && padR >= 0, "%s: reflect pad (%d,%d)", fn, padL, padR);
   PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2 && (dst_fmt != PASE_FMT_F16X2 || dst_lo),
@@ -1811,8 +1812,8 @@ int pase_out_affine_nct(const float* y, const float* scale, const float* shift, 
 
 int pase_out_affine_var(const float* y, const float* scale, const float* shift, float* out,
                         const int* tab, int nseg, int C, int mode, void* stream) {
-  PASE_CHECK_ARG(y && scale && shift && out && tab && nseg > 0 && C > 0,
-                 "pase_out_affine_var: bad args");
+  PASE_CHECK_ARG(y && scale && shift && out && tab && C > 0, "pase_out_affine_var: bad args");
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535, "pase_out_affine_var: nseg=%d", nseg);
   PASE_CHECK_ARG(mode >= 0 && mode <= 3, "pase_out_affine_var: mode %d", mode);
   PASE_LAUNCH((out_affine_var_kernel), dim3((C + 31) / 32, nseg), dim3(32, 8), 0,
               (cudaStream_t)stream, y, scale, shift, out, tab, C, mode);

@@ -515,8 +515,8 @@ extern "C" {
 int pase_qrnn_scan_fwd_var(const float* Y, float* h, long ldh, float* Cst, const int* tab,
                            int nseg, int H, void* stream) {
   PASE_CHECK_ARG(Y && h && Cst && tab, "pase_qrnn_scan_fwd_var: null pointer");
-  PASE_CHECK_ARG(nseg > 0 && H > 0 && ldh >= H, "pase_qrnn_scan_fwd_var: nseg=%d H=%d ldh=%ld",
-                 nseg, H, ldh);
+  PASE_CHECK_ARG(nseg > 0 && nseg <= 65535 && H > 0 && ldh >= H,
+                 "pase_qrnn_scan_fwd_var: nseg=%d H=%d ldh=%ld", nseg, H, ldh);
   cudaStream_t st = (cudaStream_t)stream;
   PASE_LAUNCH((qrnn_scan_fwd_seg_var_kernel), dim3((H + 31) / 32, nseg), dim3(32, MAX_SEGS), 0,
               st, Y, h, ldh, Cst, tab, H);

@@ -583,6 +583,7 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
 
 # -- packed variable-length inference (DESIGN.md section 11) ----------------------------------
 INDEX_LIMIT = 2 ** 31          # the packed kernels' tables and row counts are 32-bit ints
+MAX_UTTS = 65535               # utterances per pack: the packed kernels give each a grid row
 OUT_MODES = {None: 0, "avg_norm": 1, "avg_concat": 2, "avg_norm_concat": 3}
 
 
@@ -621,12 +622,15 @@ def utterance_geometry(cfg, lengths, sinc_fold):
     return out
 
 
-def split_packs(lengths, max_samples):
-    """Greedy, in order: consecutive utterances while their sum fits max_samples; an utterance
-    longer than max_samples is a pack of its own.  -> list of (start, stop)."""
+def split_packs(lengths, max_samples, max_count=MAX_UTTS):
+    """Greedy, in order: consecutive utterances while their sum fits max_samples and their
+    count max_count (at most MAX_UTTS, the packed kernels' grid-row limit); an utterance longer
+    than max_samples is a pack of its own.  -> list of (start, stop)."""
+    if not 1 <= max_count <= MAX_UTTS:
+        raise ValueError("max_count must be in 1..%d, got %r" % (MAX_UTTS, max_count))
     packs, start, total = [], 0, 0
     for i, T in enumerate(lengths):
-        if i > start and total + T > max_samples:
+        if i > start and (total + T > max_samples or i - start >= max_count):
             packs.append((start, i))
             start, total = i, 0
         total += T
@@ -663,7 +667,7 @@ class PackedPlan(EncoderPlan):
         self.min_len = min_length(cfg)
         self._setup(cfg, device, prec, lambda fold: build_geometry(cfg, self.min_len, fold))
         G = self.geoms
-        self.max_utts = max(self.capacity // self.min_len, 1)
+        self.max_utts = min(max(self.capacity // self.min_len, 1), MAX_UTTS)
         n_apad, n_y, rows = packed_bounds(G, self.capacity, self.max_utts)
         sizes = [("waveform", self.capacity)]
         sizes += [("block %d operand" % g.idx, na + g.K + 64) for g, na in zip(G, n_apad)]

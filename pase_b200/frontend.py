@@ -376,6 +376,9 @@ class WaveFe(Model):
             raise ValueError("%s: %d samples exceed max_samples=%d; one call is one "
                              "pack, so split the list into calls that fit"
                              % (what, sum(lengths), cap))
+        if len(lengths) > _enc.MAX_UTTS:
+            raise ValueError("%s: %d utterances exceed the %d of one pack; split the list into "
+                             "calls that fit" % (what, len(lengths), _enc.MAX_UTTS))
         fold = _gemm.PRECISIONS[self.resolved_precision()].sinc_fold
         geoms = _enc.utterance_geometry(self.cfg, lengths, fold)
         self._sinc_consts(device)
