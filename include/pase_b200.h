@@ -554,23 +554,26 @@ int pase_stream_gather(const float* staging, float* ring, long ring_cap, float* 
 int pase_axpy(const float* x, float* y, long n, float a, void* stream);
 int pase_scale_dev(float* x, long n, const float* dev_scalar, float host_coef, void* stream);
 
-/* ---- optimizer (SURVEY 8f N4): the reference steps 13 torch.optim.Adam instances
+/* ---- optimizer (SURVEY 8f N4): the reference steps 13 torch.optim.Adam or RAdam instances
  * (trainer.py:86-143, worker_scheduler.py:66-73); here ONE launch updates every
  * parameter of the flat fp32 buffers.  seg_table: device array of nseg rows of 6 x 8
  * bytes {long start, long end, float lr, float beta1, float beta2, float eps,
- * float weight_decay, float pad, long step_index}; segments are sorted, disjoint and
+ * float weight_decay, float algorithm, long step_index}; segments are sorted, disjoint and
  * start at multiples of 4 elements; steps: device float vector of step counts (already
  * incremented for this update).  grad_scale multiplies the gradient (1/world of a
- * summed all-reduce, or 1).  Semantics = torch.optim.Adam (amsgrad / maximize off). */
+ * summed all-reduce, or 1).  algorithm 0: torch.optim.Adam (amsgrad / maximize off, L2
+ * weight decay); 1: the reference's RAdam (WorkerScheduler/radam.py: rho and the step size
+ * in fp64 from the step count, momentum-SGD step while rho < 5, decoupled weight decay). */
 int pase_adam_flat(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long n,
                    const long* seg_table, int nseg, const float* steps, float grad_scale,
                    void* stream);
-/* Data parallelism fused into the update (the reference is single-GPU: its per-worker Adam
- * instances, trainer.py:86-143 / worker_scheduler.py:66-73, have no exchange step; this
+/* Data parallelism fused into the update (the reference is single-GPU: its per-worker
+ * optimizer instances, trainer.py:86-143 / worker_scheduler.py:66-73, have no exchange step; this
  * replaces ncclAllReduce + the update above, see SURVEY.md 8e): every rank's flat gradient / parameter / flag buffers are peer-mapped
  * (param_peers / grad_peers / flag_peers: DEVICE arrays of `world` pointers; flags: int[2*world]
  * per rank, zero-initialised).  One launch per rank and step: cross-GPU barrier, mean of the
- * peers' gradients over this rank's 1/world shard read through NVLink, Adam on the local
+ * peers' gradients over this rank's 1/world shard read through NVLink, each segment's update
+ * (the same arithmetic as pase_adam_flat) on the local
  * (exp_avg, exp_avg_sq) shard, new parameters stored into every rank's buffer, barrier.
  * epoch / done: zero-initialised device scalars owned by the optimizer.  n % 4 == 0. */
 int pase_adam_flat_dp(void* const* param_peers, void* const* grad_peers,

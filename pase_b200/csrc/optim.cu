@@ -1,9 +1,11 @@
-// Flat-buffer Adam: ONE launch updates every parameter of the model (encoder + all worker
-// heads) with per-segment hyper-parameters.  Replaces the 13 torch.optim.Adam instances the
-// reference steps one after the other (pase/models/WorkerScheduler/trainer.py:86-143,
-// worker_scheduler.py:66-73), and folds the 1/world gradient scale of the data-parallel
-// all-reduce into the same pass.  Semantics = torch.optim.Adam (amsgrad off, maximize off,
-// L2 weight decay added to the gradient).
+// Flat-buffer Adam / RAdam: ONE launch updates every parameter of the model (encoder + all
+// worker heads) with per-segment hyper-parameters and algorithm.  Replaces the 13 optimizer
+// instances the reference steps one after the other (pase/models/WorkerScheduler/trainer.py:
+// 86-143, worker_scheduler.py:66-73), and folds the 1/world gradient scale of the
+// data-parallel all-reduce into the same pass.  Per segment:
+//   Adam   torch.optim.Adam (amsgrad off, maximize off, L2 weight decay added to the gradient)
+//   RAdam  the reference's RAdam (WorkerScheduler/radam.py): rectified step once rho >= 5,
+//          un-normalised momentum step before, decoupled weight decay p += -(wd*lr)*p
 #include "common.cuh"
 #include <cstring>
 
@@ -11,11 +13,80 @@ namespace {
 
 constexpr int SEG_MAX = 64;
 
-struct AdamSeg {           // one row of the device segment table (8 x 8 bytes)
+struct AdamSeg {           // one row of the device segment table (6 x 8 bytes)
   long start, end;         // element range [start, end) of the flat buffers
-  float lr, beta1, beta2, eps, weight_decay, pad;
+  float lr, beta1, beta2, eps, weight_decay;
+  float algorithm;         // 0: Adam, 1: RAdam
   long step_index;         // index into the device step-count vector
 };
+
+enum : int { UPD_ADAM = 0, UPD_RADAM_RECT = 1, UPD_RADAM_SGD = 2 };
+
+struct SegConst {          // per-segment constants of one step, computed once per block
+  float step_size;         // Adam: lr / (1 - beta1^t); RAdam: the fp64 step size, rounded
+  float inv_sqrt_b2;       // Adam: 1 / sqrt(1 - beta2^t)
+  float decay;             // RAdam: -(weight_decay * lr)
+  int mode;                // UPD_*
+};
+
+// t = the segment's step count, already incremented for this update.  RAdam's rho is the
+// difference of two numbers near 2/(1-beta2) (~2000 for beta2 = 0.999) that lands within
+// 0.004 of the threshold 5 at steps 5 and 6: it and the step size are computed in fp64, as the
+// reference computes them in Python floats.  The branch is chosen here, from the device step
+// count, so a captured graph crosses rho = 5 by itself.
+__device__ __forceinline__ SegConst seg_constants(const AdamSeg& sg, float t) {
+  SegConst c;
+  if (sg.algorithm == 0.f) {
+    const float b1 = 1.f - powf(sg.beta1, t), b2 = 1.f - powf(sg.beta2, t);
+    c.step_size = sg.lr / b1;
+    c.inv_sqrt_b2 = rsqrtf(b2);
+    c.decay = 0.f;
+    c.mode = UPD_ADAM;
+    return c;
+  }
+  const double td = (double)t, lr = (double)sg.lr, beta2 = (double)sg.beta2;
+  const double b2t = pow(beta2, td);
+  const double bias1 = 1.0 - pow((double)sg.beta1, td);
+  const double rho_inf = 2.0 / (1.0 - beta2) - 1.0;
+  const double rho = rho_inf - 2.0 * td * b2t / (1.0 - b2t);
+  double step_size;
+  if (rho >= 5.0) {
+    step_size = lr * sqrt((1.0 - b2t) * (rho - 4.0) / (rho_inf - 4.0) * (rho - 2.0) / rho *
+                          rho_inf / (rho_inf - 2.0)) / bias1;
+    c.mode = UPD_RADAM_RECT;
+  } else {
+    step_size = lr / bias1;
+    c.mode = UPD_RADAM_SGD;
+  }
+  c.step_size = (float)step_size;
+  c.inv_sqrt_b2 = 0.f;
+  c.decay = (float)(-((double)sg.weight_decay * lr));
+  return c;
+}
+
+// One element of one segment: the arithmetic both kernels share.  g is the raw gradient,
+// gscale its factor (grad_scale, or 1/world of the peers' sum).
+__device__ __forceinline__ void seg_update(float& p, float& m, float& v, float g, float gscale,
+                                           const AdamSeg& sg, const SegConst& c) {
+  const float beta1 = sg.beta1, beta2 = sg.beta2, eps = sg.eps;
+  if (c.mode == UPD_ADAM) {
+    const float gg = g * gscale + sg.weight_decay * p;
+    m = beta1 * m + (1.f - beta1) * gg;
+    v = beta2 * v + (1.f - beta2) * gg * gg;
+    const float denom = sqrtf(v) * c.inv_sqrt_b2 + eps;
+    p -= c.step_size * m / denom;
+    return;
+  }
+  // RAdam, in the order of the reference's tensor ops; decay is 0 when weight_decay is
+  const float gg = g * gscale;
+  m = beta1 * m + (1.f - beta1) * gg;
+  v = beta2 * v + (1.f - beta2) * gg * gg;
+  p = p + c.decay * p;
+  if (c.mode == UPD_RADAM_RECT)
+    p = p + (-c.step_size) * (m / (sqrtf(v) + eps));
+  else
+    p = p + (-c.step_size) * m;
+}
 
 __global__ void __launch_bounds__(256)
 adam_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
@@ -23,13 +94,10 @@ adam_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
                  const float* __restrict__ steps, float grad_scale) {
   pdl_wait();
   __shared__ AdamSeg ss[SEG_MAX];
-  __shared__ float c1[SEG_MAX], c2[SEG_MAX];       // lr / bias1, 1 / sqrt(bias2)
+  __shared__ SegConst cs[SEG_MAX];
   for (int i = threadIdx.x; i < nseg; i += blockDim.x) {
     ss[i] = segs[i];
-    const float t = steps[ss[i].step_index];
-    const float b1 = 1.f - powf(ss[i].beta1, t), b2 = 1.f - powf(ss[i].beta2, t);
-    c1[i] = ss[i].lr / b1;
-    c2[i] = rsqrtf(b2);
+    cs[i] = seg_constants(ss[i], steps[ss[i].step_index]);
   }
   __syncthreads();
   const long stride = (long)gridDim.x * blockDim.x * 4;
@@ -39,8 +107,7 @@ adam_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
     // a float4 never straddles two segments when every segment starts at a multiple of 4
     // (the host pads); the scalar tail handles a ragged end
     const AdamSeg& sg = ss[s];
-    const float beta1 = sg.beta1, beta2 = sg.beta2, eps = sg.eps, wd = sg.weight_decay;
-    const float step_size = c1[s], inv_sqrt_b2 = c2[s];
+    const SegConst c = cs[s];
     const int cnt = (i + 3 < n) ? 4 : (int)(n - i);
     float pv[4], gv[4], mv[4], vv[4];
     if (cnt == 4) {
@@ -59,11 +126,7 @@ adam_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
     for (int k = 0; k < 4; ++k) {
       if (k >= cnt) break;
       if (i + k >= sg.end) continue;                 // padding between segments: untouched
-      const float gg = gv[k] * grad_scale + wd * pv[k];
-      mv[k] = beta1 * mv[k] + (1.f - beta1) * gg;
-      vv[k] = beta2 * vv[k] + (1.f - beta2) * gg * gg;
-      const float denom = sqrtf(vv[k]) * inv_sqrt_b2 + eps;
-      pv[k] -= step_size * mv[k] / denom;
+      seg_update(pv[k], mv[k], vv[k], gv[k], grad_scale, sg, c);
     }
     if (cnt == 4) {
       *reinterpret_cast<float4*>(p + i) = make_float4(pv[0], pv[1], pv[2], pv[3]);
@@ -80,14 +143,14 @@ adam_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
 // space (CUDA IPC over NVLink / NVSwitch peer access).  Rank r owns the shard
 // [lo_r, hi_r) of the flat index space.  ONE kernel per rank and step:
 //   barrier A   my gradients are complete -> flag in every peer; wait for theirs
-//   shard       g = mean_p grad_p[i] read straight from the peers' buffers (ld.cv), Adam on
-//               the local (m, v, p) shard, the new parameter value stored into EVERY rank's
+//   shard       g = mean_p grad_p[i] read straight from the peers' buffers (ld.cv), the
+//               segment's update (seg_update) on the local (m, v, p) shard, the new parameter value stored into EVERY rank's
 //               parameter buffer
 //   barrier B   all my remote stores are performed -> flag in every peer; the LAST block
 //               of the grid waits for the peers' flags before the kernel may complete (the
 //               next forward reads parameters the peers wrote, and the next backward
 //               overwrites gradients the peers read)
-// No collective library call, no separate Adam launch, nothing for the host to order: the
+// No collective library call, no separate optimizer launch, nothing for the host to order: the
 // step stays one CUDA graph.  NVLink traffic per rank and step: (W-1)/W of the gradient bytes
 // in, the same out -- the reduce-scatter + all-gather volume of a ring, without its W-1 hops.
 struct DpArgs {
@@ -126,16 +189,13 @@ __device__ __forceinline__ void wait_flags(const int* flags, int world, int want
 __global__ void __launch_bounds__(256)
 adam_flat_dp_kernel(const DpArgs a) {
   __shared__ AdamSeg ss[SEG_MAX];
-  __shared__ float c1[SEG_MAX], c2[SEG_MAX];
+  __shared__ SegConst cs[SEG_MAX];
   __shared__ int s_last;
   const int W = a.world, R = a.rank;
   const int want = *reinterpret_cast<volatile int*>(a.epoch) + 1;
   for (int i = threadIdx.x; i < a.nseg; i += blockDim.x) {
     ss[i] = a.segs[i];
-    const float t = a.steps[ss[i].step_index];
-    const float b1 = 1.f - powf(ss[i].beta1, t), b2 = 1.f - powf(ss[i].beta2, t);
-    c1[i] = ss[i].lr / b1;
-    c2[i] = rsqrtf(b2);
+    cs[i] = seg_constants(ss[i], a.steps[ss[i].step_index]);
   }
   // ---- barrier A: the kernel is stream-ordered after backward, so my gradients are final
   if (blockIdx.x == 0 && threadIdx.x < W) {
@@ -156,8 +216,7 @@ adam_flat_dp_kernel(const DpArgs a) {
   for (long i = lo + ((long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < hi; i += stride) {
     while (s + 1 < a.nseg && i >= ss[s].end) ++s;
     const AdamSeg& sg = ss[s];
-    const float beta1 = sg.beta1, beta2 = sg.beta2, eps = sg.eps, wd = sg.weight_decay;
-    const float step_size = c1[s], inv_sqrt_b2 = c2[s];
+    const SegConst c = cs[s];
     // the flat buffers are padded to a multiple of 4 elements: whole float4 accesses
     float4 G = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int q = 0; q < W; ++q) {
@@ -172,11 +231,7 @@ adam_flat_dp_kernel(const DpArgs a) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (i + k >= sg.end) continue;                 // padding between segments: untouched
-      const float gg = gv[k] * inv_w + wd * pv[k];
-      mv[k] = beta1 * mv[k] + (1.f - beta1) * gg;
-      vv[k] = beta2 * vv[k] + (1.f - beta2) * gg * gg;
-      const float denom = sqrtf(vv[k]) * inv_sqrt_b2 + eps;
-      pv[k] -= step_size * mv[k] / denom;
+      seg_update(pv[k], mv[k], vv[k], gv[k], inv_w, sg, c);
     }
     const float4 Pn = make_float4(pv[0], pv[1], pv[2], pv[3]);
     *reinterpret_cast<float4*>(a.m + i) = make_float4(mv[0], mv[1], mv[2], mv[3]);

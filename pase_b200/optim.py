@@ -1,18 +1,21 @@
-"""Flat-buffer Adam (SURVEY.md 8f N4).
+"""Flat-buffer Adam / RAdam (SURVEY.md 8f N4).
 
-The reference trains with one ``torch.optim.Adam`` per worker plus one for the frontend
+The reference trains with one optimizer per worker plus one for the frontend
 (pase/models/WorkerScheduler/trainer.py:86-143) and steps them one after the other
-(worker_scheduler.py:66-73): 13 x (zero_grad + multi-tensor step).  ``FlatAdam`` keeps every
-parameter, gradient and moment of ALL those groups in four flat fp32 buffers and updates them
-with ONE kernel launch (``pase_adam_flat``), with per-group learning rates / betas / eps /
-weight decay.  The gradient buffer is the same flat buffer the data-parallel all-reduce
-works on (``pase_b200.dp.FlatGradAllReducer``), so a step is: backward -> one NCCL
-all-reduce -> one Adam launch.
+(worker_scheduler.py:66-73): 13 x (zero_grad + multi-tensor step).  The optimizers are
+``torch.optim.Adam``, or the reference's own ``RAdam`` for ``--fe_opt radam`` /
+``--min_opt radam``.  ``FlatAdam`` keeps every parameter, gradient and moment of ALL those
+groups in four flat fp32 buffers and updates them with ONE kernel launch (``pase_adam_flat``),
+with per-group learning rates / betas / eps / weight decay and algorithm (``"adam"`` or
+``"radam"``, mixed freely).  The gradient buffer is the same flat buffer the data-parallel
+all-reduce works on (``pase_b200.dp.FlatGradAllReducer``), so a step is: backward -> one NCCL
+all-reduce -> one optimizer launch.
 
 Drop-in surface: ``param_groups`` (LR schedulers mutate ``group['lr']``), ``step()``,
-``zero_grad()``, ``state_dict()`` / ``load_state_dict()`` in torch.optim.Adam's own format
-(so ``Saver`` checkpoints interchange with the reference's), and ``views()``: one
-per-group facade with ``step()`` / ``zero_grad()`` / ``state_dict()`` for callers that hold a
+``zero_grad()``, ``state_dict()`` / ``load_state_dict()`` in torch.optim.Adam's own format,
+or the reference RAdam's for RAdam groups (so ``Saver`` checkpoints interchange with the
+reference's), and ``views()``: one per-group facade with ``step()`` / ``zero_grad()`` /
+``state_dict()`` / ``load_state_dict()`` for callers that hold a
 dict of optimizers like the reference's ``backprop_scheduler`` -- the facades' steps are
 deferred and the single launch happens when the last group has stepped.
 """
@@ -25,18 +28,40 @@ def _ru4(n):
     return (n + 3) // 4 * 4
 
 
+# the segment table's algorithm code of each supported update
+ALGORITHMS = {"adam": 0, "radam": 1}
+
+
+def _algorithm(name):
+    if name not in ALGORITHMS:
+        raise ValueError("FlatAdam: algorithm=%r; supported: %s"
+                         % (name, ", ".join(repr(a) for a in ALGORITHMS)))
+    return name
+
+
 class FlatAdam(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
-                 grad_buffer=None, grad_scale=1.0, peer_dp=False, group=None):
-        """peer_dp=True (torch.distributed initialised, one process per GPU of ONE node): the
+                 grad_buffer=None, grad_scale=1.0, peer_dp=False, group=None, algorithm="adam"):
+        """algorithm (default of every group; a group may set its own ``"algorithm"`` key):
+        ``"adam"`` is torch.optim.Adam (L2 weight decay added to the gradient); ``"radam"`` is
+        the reference's RAdam (pase/models/WorkerScheduler/radam.py: rectified steps from the
+        step where rho >= 5, momentum-SGD steps before it, decoupled weight decay).  Each RAdam
+        group computes its own step size; the reference's RAdam caches one per step for all
+        groups of an instance, which differs only for an instance with several groups of
+        different lr, a layout the reference trainer never builds.
+
+        peer_dp=True (torch.distributed initialised, one process per GPU of ONE node): the
         flat parameter / gradient buffers are CUDA-IPC peer-mapped across the ranks and
         ``step()`` becomes ``pase_adam_flat_dp`` -- gradient averaging (reduce-scatter),
         the Adam update of this rank's 1/world shard and the parameter all-gather in ONE
         kernel over NVLink, no collective call (``reduce_grads()`` turns into a no-op).  The
         Adam moments are then sharded: ``consolidate_state()`` (collective) before
         ``state_dict()``."""
-        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
+                        algorithm=_algorithm(algorithm))
         super().__init__(params, defaults)
+        for g in self.param_groups:
+            _algorithm(g["algorithm"])
         plist = [p for g in self.param_groups for p in g["params"]]
         if not plist:
             raise ValueError("FlatAdam: no parameters")
@@ -163,17 +188,17 @@ class FlatAdam(torch.optim.Optimizer):
 
     # ---- the update ------------------------------------------------------------------
     def _segments(self):
-        """The device table of per-group hyper-parameters.  It is allocated once and keeps its
+        """The device table of per-group hyper-parameters and algorithm.  It is allocated once and keeps its
         address: a captured ``pase_adam_flat`` launch reads whatever the table holds at replay
         time, so a changed lr / betas / eps / weight decay is written into the same tensor, by
         a copy ordered on the current stream after every earlier update that read it."""
-        key = tuple((g["lr"], g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"])
-                    for g in self.param_groups)
+        key = tuple((g["lr"], g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"],
+                     ALGORITHMS[_algorithm(g["algorithm"])]) for g in self.param_groups)
         if key != self._table_key:
             import struct
             raw = b"".join(
                 struct.pack("<qqffffffq", a, b, float(k[0]), float(k[1]), float(k[2]), float(k[3]),
-                            float(k[4]), 0.0, i)
+                            float(k[4]), float(k[5]), i)
                 for i, ((a, b), k) in enumerate(zip(self._ranges, key)))
             src = torch.frombuffer(bytearray(raw), dtype=torch.int64)
             dev = self.flat_param.device
@@ -227,42 +252,56 @@ class FlatAdam(torch.optim.Optimizer):
             dist.all_gather_into_tensor(pad, pad[lo:lo + per].clone(), group=self._group)
             buf.copy_(pad[:self.n])
 
-    # ---- torch.optim.Adam-compatible persistence ----------------------------------------
+    # ---- torch.optim.Adam / reference RAdam-compatible persistence ----------------------
     def state_dict(self):
+        """torch.optim.Adam's format for Adam groups; for RAdam groups the reference RAdam's:
+        an int ``step`` and only lr / betas / eps / weight_decay in the group."""
         state, groups, idx = {}, [], 0
         steps = self.steps.detach().cpu()
         for gi, g in enumerate(self.param_groups):
+            radam = g["algorithm"] == "radam"
             ids = []
             for p in g["params"]:
                 o = self._offsets[idx]
-                state[idx] = {"step": steps[gi].clone(),
+                state[idx] = {"step": int(steps[gi]) if radam else steps[gi].clone(),
                               "exp_avg": self.exp_avg[o:o + p.numel()].view_as(p).clone(),
                               "exp_avg_sq": self.exp_avg_sq[o:o + p.numel()].view_as(p).clone()}
                 ids.append(idx)
                 idx += 1
-            gd = {k: v for k, v in g.items() if k != "params"}
-            gd.update(params=ids, amsgrad=False, maximize=False, foreach=None, capturable=False,
-                      differentiable=False, fused=None)
+            if radam:
+                gd = {k: g[k] for k in ("lr", "betas", "eps", "weight_decay")}
+                gd.update(params=ids)
+            else:
+                gd = {k: v for k, v in g.items() if k not in ("params", "algorithm")}
+                gd.update(params=ids, amsgrad=False, maximize=False, foreach=None,
+                          capturable=False, differentiable=False, fused=None)
             groups.append(gd)
         return {"state": state, "param_groups": groups}
 
     def load_state_dict(self, sd):
-        idx = 0
-        for gi, (g, sg) in enumerate(zip(self.param_groups, sd["param_groups"])):
-            for k in ("lr", "betas", "eps", "weight_decay"):
-                if k in sg:
-                    g[k] = tuple(sg[k]) if k == "betas" else sg[k]
-            step = None
-            for p in g["params"]:
-                st = sd["state"].get(idx, sd["state"].get(str(idx)))
-                if st is not None:
-                    o = self._offsets[idx]
-                    self.exp_avg[o:o + p.numel()].view_as(p).copy_(st["exp_avg"])
-                    self.exp_avg_sq[o:o + p.numel()].view_as(p).copy_(st["exp_avg_sq"])
-                    step = float(st["step"])
-                idx += 1
-            if step is not None:
-                self.steps[gi] = step
+        """Either format; the groups keep their algorithm, which neither format records."""
+        first = 0
+        for gi, sg in enumerate(sd["param_groups"][:len(self.param_groups)]):
+            self._load_group(gi, sg, sd["state"], first)
+            first += len(self.param_groups[gi]["params"])
+
+    def _load_group(self, gi, sg, state, first):
+        """Group gi from a saved group ``sg`` whose parameters are ``state[first + j]``."""
+        g = self.param_groups[gi]
+        for k in ("lr", "betas", "eps", "weight_decay"):
+            if k in sg:
+                g[k] = tuple(sg[k]) if k == "betas" else sg[k]
+        base = sum(len(h["params"]) for h in self.param_groups[:gi])
+        step = None
+        for j, p in enumerate(g["params"]):
+            st = state.get(first + j, state.get(str(first + j)))
+            if st is not None:
+                o = self._offsets[base + j]
+                self.exp_avg[o:o + p.numel()].view_as(p).copy_(st["exp_avg"])
+                self.exp_avg_sq[o:o + p.numel()].view_as(p).copy_(st["exp_avg_sq"])
+                step = float(st["step"])
+        if step is not None:
+            self.steps[gi] = step
         self._table_key = None
 
     # ---- per-group facades for callers that hold a dict of optimizers -------------------
@@ -280,7 +319,7 @@ class FlatAdam(torch.optim.Optimizer):
 class _GroupView(object):
     """What ``backprop_scheduler`` needs from an optimizer (worker_scheduler.py:43-75):
     ``zero_grad()`` and ``step()``; plus ``param_groups`` for the LR schedulers and
-    ``state_dict`` for the per-worker ``Saver``.  ``step()`` is deferred: the one kernel launch
+    ``state_dict`` / ``load_state_dict`` for the per-worker ``Saver``.  ``step()`` is deferred: the one kernel launch
     happens when the last group of the engine has stepped."""
 
     def __init__(self, engine, gi):
@@ -305,3 +344,6 @@ class _GroupView(object):
         g = dict(full["param_groups"][self.gi])
         g["params"] = list(range(len(ids)))
         return {"state": {remap[i]: full["state"][i] for i in ids}, "param_groups": [g]}
+
+    def load_state_dict(self, sd):
+        self.engine._load_group(self.gi, sd["param_groups"][0], sd["state"], 0)
