@@ -10,6 +10,14 @@ constexpr int THREADS = 256;
 // 3.42 ms/step against 4 steps per thread with 2-3 resident blocks per SM: loads in flight per
 // thread matter more than occupancy here)
 constexpr int RUN = 8;
+// threads per block of the forward kernels, and blocks per SM their register budget must allow:
+// 7 x 128 threads (72 registers) keep block 0's grid of 32 x 200 windows x 16 channel quads
+// (800 blocks) resident in one wave on 132 SMs, where 3 x 256 threads (80 registers) left 4 of
+// its 400 blocks to start only as the first ones finished.  The fp32 operand writer (with its
+// optional tf32 residual) needs more than 72 and keeps 6 x 128, as does the packed form.
+constexpr int FWD_THREADS = 128;
+template <int DF>
+constexpr int fwd_min_blocks() { return DF == PASE_FMT_F32 ? 6 : 7; }
 
 // DF: operand format of the padded waveform (block 0's GEMM operand)
 template <int DF>
@@ -116,11 +124,115 @@ __device__ __forceinline__ float prelu1(float u, float a) { return u > 0.f ? u :
 //   YT  storage type of y (float / bf16);  DF  operand format of dst:
 //   PASE_FMT_F32 (+ optional tf32-residual twin dst_lo), PASE_FMT_BF16, PASE_FMT_F16X2
 //   (dst = hi, dst_lo = lo').  The dense-skip pool accumulates the value the next layer
-//   reads (i.e. after rounding to bf16 in the bf16 format); the thread that writes the first
-//   time step of a pooling window sums the whole window in time order, so each window mean
-//   has one writer and comes out the same on every run.
+//   reads (i.e. after rounding to bf16 in the bf16 format).
+
+// One activation of the channel quad at c, written at dst offset o; returns the value the next
+// layer reads (the bf16-rounded one in the bf16 format), which is what the pool sums.
+template <int DF>
+__device__ __forceinline__ float4 bn_prelu_store(float4 v, float4 sc, float4 sh, float4 al,
+                                                 void* __restrict__ dst_v,
+                                                 void* __restrict__ dst_lo_v, long o) {
+  float4 a;
+  a.x = prelu1(fmaf(v.x, sc.x, sh.x), al.x);
+  a.y = prelu1(fmaf(v.y, sc.y, sh.y), al.y);
+  a.z = prelu1(fmaf(v.z, sc.z, sh.z), al.z);
+  a.w = prelu1(fmaf(v.w, sc.w, sh.w), al.w);
+  if constexpr (DF == PASE_FMT_F32) {
+    st4(reinterpret_cast<float*>(dst_v) + o, a);
+    if (dst_lo_v != nullptr)      // 3xTF32 residual of the operand just written
+      st4(reinterpret_cast<float*>(dst_lo_v) + o,
+          make_float4(tf32_residual(a.x), tf32_residual(a.y), tf32_residual(a.z),
+                      tf32_residual(a.w)));
+  } else if constexpr (DF == PASE_FMT_BF16) {
+    __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst_v) + o;
+    st4t(d, a);
+    a = rt4t(d, a);
+  } else {
+    st4_f16x2(reinterpret_cast<__half*>(dst_v) + o, reinterpret_cast<__half*>(dst_lo_v) + o, a);
+  }
+  return a;
+}
+
+// Runs of one sample's forward pass.  Without a pool (pool_d <= 0 or pool_T == 0) the padded
+// output [0, Tp) is cut into runs of RUN time steps.  With one, the time steps are cut into
+//   [0, padL)                        the left reflect halo, runs of RUN steps;
+//   [padL, padL + pool_T * pool_d)   the pooled frames, runs of L = pool_d * ceil(RUN / pool_d)
+//                                    steps: whole pooling windows only;
+//   [padL + pool_T * pool_d, Tp)     the unpooled tail and the right halo, runs of RUN steps.
+// Every window then lies inside one thread's run, and that thread sums it as it produces it.
+struct FwdRuns {
+  int nA, nB;             // runs of the left halo, of the pooled frames
+  int wpr;                // pooling windows per pooled run
+  int tail0;              // first time step of the runs after the pooled ones
+  long total;             // all runs
+};
+
+__host__ __device__ __forceinline__ FwdRuns fwd_runs(int Tp, int padL, int pool_d, int pool_T) {
+  FwdRuns r;
+  if (pool_d > 0 && pool_T > 0) {
+    r.nA = (padL + RUN - 1) / RUN;
+    r.wpr = (RUN + pool_d - 1) / pool_d;
+    r.nB = (pool_T + r.wpr - 1) / r.wpr;
+    r.tail0 = padL + pool_T * pool_d;
+  } else {
+    r.nA = r.nB = r.wpr = r.tail0 = 0;
+  }
+  r.total = (long)r.nA + r.nB + (Tp - r.tail0 + RUN - 1) / RUN;
+  return r;
+}
+
+// A pooled run: len time steps of the channel quad whose raw conv output starts at y, whole
+// pooling windows of pd steps, streamed in chunks of RUN (RUN loads in flight, then compute and
+// store).  Each activation is added to its window's sum in time order as it is produced; the
+// window's mean goes to pp, the next window's to pp + p_rs.
+template <typename YT, int DF>
+__device__ __forceinline__ void bn_prelu_pooled_run(const YT* __restrict__ y, int C, int len,
+                                                    int pd, float4 sc, float4 sh, float4 al,
+                                                    void* __restrict__ dst_v,
+                                                    void* __restrict__ dst_lo_v, long o, long d_rs,
+                                                    float* __restrict__ pp, long p_rs) {
+  float4 ps = make_float4(0.f, 0.f, 0.f, 0.f);
+  int k = 0;                    // time steps of the current window summed so far
+  for (int t0 = 0; t0 < len; t0 += RUN) {
+    const int nvalid = min(RUN, len - t0);
+    // straight-line loads (a step past the run re-reads the chunk's first row): no predicate, so
+    // the chunk's registers never merge with the previous chunk's
+    float4 vals[RUN];
+#pragma unroll
+    for (int i = 0; i < RUN; ++i) vals[i] = ld4t(y + (long)(t0 + (i < nvalid ? i : 0)) * C);
+#pragma unroll
+    for (int i = 0; i < RUN; ++i) {
+      if (i >= nvalid) break;
+      const float4 a = bn_prelu_store<DF>(vals[i], sc, sh, al, dst_v, dst_lo_v, o);
+      o += d_rs;
+      // round-to-nearest adds: the sum is never contracted into the PReLU multiply
+      ps.x = __fadd_rn(ps.x, a.x); ps.y = __fadd_rn(ps.y, a.y);
+      ps.z = __fadd_rn(ps.z, a.z); ps.w = __fadd_rn(ps.w, a.w);
+      if (++k == pd) {
+        const float inv_d = __frcp_rn((float)pd);     // = 1.f / pd, correctly rounded
+        const float4 m = make_float4(ps.x * inv_d, ps.y * inv_d, ps.z * inv_d, ps.w * inv_d);
+        // one 16-byte reduction per window where the quad is aligned (always in the uniform
+        // launch; a packed table's pool_off need not be a multiple of 4)
+        if ((reinterpret_cast<uintptr_t>(pp) & 15u) == 0) {
+          atomicAdd(reinterpret_cast<float4*>(pp), m);
+        } else {
+          atomicAdd(pp + 0, m.x);
+          atomicAdd(pp + 1, m.y);
+          atomicAdd(pp + 2, m.z);
+          atomicAdd(pp + 3, m.w);
+        }
+        pp += p_rs;
+        ps = make_float4(0.f, 0.f, 0.f, 0.f);
+        k = 0;
+      }
+    }
+  }
+}
+
 // One sample: yn its raw conv output, dst / pool offsets d_base / p_base; thread idx owns the
-// channel quad idx % (C/4) over RUN time steps of the padded output.
+// channel quad idx % (C/4) over run idx / (C/4) of fwd_runs.  A pooled run sums each of its
+// windows in time order as it produces it (bn_prelu_pooled_run), so each window mean has one
+// writer and comes out the same on every run.
 template <typename YT, int DF>
 __device__ __forceinline__ void bn_prelu_pad_fwd_sample(
     const YT* __restrict__ yn, long idx, int T, int C, const float* __restrict__ scale,
@@ -130,65 +242,37 @@ __device__ __forceinline__ void bn_prelu_pad_fwd_sample(
   const int C4 = C >> 2;
   const int q = (int)(idx % C4);
   const long run = idx / C4;
-  const long tau0 = run * RUN;
-  if (tau0 >= Tp) return;
+  const FwdRuns R = fwd_runs(Tp, padL, pool_d, pool_T);
+  if (run >= R.total) return;
   const int c = q * 4;
   const float4 sc = ld4(scale + c), sh = ld4(shift + c), al = ld4(alpha + c);
-  const int pool_len = pool_d > 0 ? pool_T * pool_d : 0;
-  const float inv_d = pool_d > 0 ? 1.f / (float)pool_d : 0.f;
-  const int nvalid = (Tp - tau0) < RUN ? (int)(Tp - tau0) : RUN;
+  if (run >= R.nA && run < R.nA + R.nB) {
+    const int w0 = (int)(run - R.nA) * R.wpr;      // first window, first frame w0 * pool_d
+    const int tr0 = w0 * pool_d;
+    bn_prelu_pooled_run<YT, DF>(yn + (long)tr0 * C + c, C,
+                                min(R.wpr, pool_T - w0) * pool_d, pool_d, sc, sh, al, dst_v,
+                                dst_lo_v, d_base + (long)(padL + tr0) * d_rs + c, d_rs,
+                                pool + p_base + (long)w0 * p_rs + c, p_rs);
+    return;
+  }
+  // RUN padded time steps from tau0 (fewer at the end of their range): the left halo, the
+  // unpooled tail and right halo, or any run of a launch without a pool
+  const int tau0 = run < R.nA ? (int)run * RUN : R.tail0 + (int)(run - R.nA - R.nB) * RUN;
+  const int tend = run < R.nA ? padL : Tp;
+  const int nvalid = min(RUN, tend - tau0);
   float4 vals[RUN];
 #pragma unroll
   for (int i = 0; i < RUN; ++i)
-    if (i < nvalid) vals[i] = ld4t(yn + (long)reflect_idx((int)tau0 + i - padL, T) * C + c);
+    if (i < nvalid) vals[i] = ld4t(yn + (long)reflect_idx(tau0 + i - padL, T) * C + c);
 #pragma unroll
   for (int i = 0; i < RUN; ++i) {
     if (i >= nvalid) break;
-    const long tau = tau0 + i;
-    const int tr = (int)tau - padL;
-    const float4 v = vals[i];
-    float4 a;
-    a.x = prelu1(fmaf(v.x, sc.x, sh.x), al.x);
-    a.y = prelu1(fmaf(v.y, sc.y, sh.y), al.y);
-    a.z = prelu1(fmaf(v.z, sc.z, sh.z), al.z);
-    a.w = prelu1(fmaf(v.w, sc.w, sh.w), al.w);
-    const long o = d_base + tau * d_rs + c;
-    if constexpr (DF == PASE_FMT_F32) {
-      st4(reinterpret_cast<float*>(dst_v) + o, a);
-      if (dst_lo_v != nullptr)      // 3xTF32 residual of the operand just written
-        st4(reinterpret_cast<float*>(dst_lo_v) + o,
-            make_float4(tf32_residual(a.x), tf32_residual(a.y), tf32_residual(a.z),
-                        tf32_residual(a.w)));
-    } else if constexpr (DF == PASE_FMT_BF16) {
-      __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst_v) + o;
-      st4t(d, a);
-      a = rt4t(d, a);
-    } else {
-      st4_f16x2(reinterpret_cast<__half*>(dst_v) + o, reinterpret_cast<__half*>(dst_lo_v) + o, a);
-    }
-    if (tr >= 0 && tr < pool_len && tr % pool_d == 0) {
-      float4 ps = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int k = 0; k < pool_d; ++k) {
-        const float4 w = ld4t(yn + (long)(tr + k) * C + c);
-        float4 b;
-        b.x = prelu1(fmaf(w.x, sc.x, sh.x), al.x);
-        b.y = prelu1(fmaf(w.y, sc.y, sh.y), al.y);
-        b.z = prelu1(fmaf(w.z, sc.z, sh.z), al.z);
-        b.w = prelu1(fmaf(w.w, sc.w, sh.w), al.w);
-        if constexpr (DF == PASE_FMT_BF16) b = rt4t(static_cast<const __nv_bfloat16*>(nullptr), b);
-        ps.x += b.x; ps.y += b.y; ps.z += b.z; ps.w += b.w;
-      }
-      float* pp = pool + p_base + (long)(tr / pool_d) * p_rs + c;
-      atomicAdd(pp + 0, ps.x * inv_d);
-      atomicAdd(pp + 1, ps.y * inv_d);
-      atomicAdd(pp + 2, ps.z * inv_d);
-      atomicAdd(pp + 3, ps.w * inv_d);
-    }
+    bn_prelu_store<DF>(vals[i], sc, sh, al, dst_v, dst_lo_v, d_base + (long)(tau0 + i) * d_rs + c);
   }
 }
 
 template <typename YT, int DF>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(FWD_THREADS, fwd_min_blocks<DF>())
 bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
                         const float* __restrict__ scale, const float* __restrict__ shift,
                         const float* __restrict__ alpha, void* __restrict__ dst_v, long d_ss,
@@ -206,7 +290,7 @@ bn_prelu_pad_fwd_kernel(const YT* __restrict__ y, long y_ss, int T, int C,
 // pool_d, pool_T} (elements).  sep != 0: the row ahead of each utterance's output (dst_off -
 // d_rs, C elements) is written zero (the QRNN input's x_{-1} row).
 template <typename YT, int DF>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(FWD_THREADS, 6)   // the sep row and the table: 80 registers
 bn_prelu_pad_fwd_var_kernel(const YT* __restrict__ y, const int* __restrict__ tab, int C,
                             const float* __restrict__ scale, const float* __restrict__ shift,
                             const float* __restrict__ alpha, void* __restrict__ dst_v, long d_rs,
@@ -1505,11 +1589,11 @@ int pase_bn_prelu_pad_fwd(const void* y, int y_bf16, long y_sample_stride, int N
   }
   if (pool == nullptr) pool_d = 0;
   const int Tp = T + padL + padR;
-  const long threads = (long)(C / 4) * ((Tp + RUN - 1) / RUN);
-  dim3 grid((unsigned)((threads + THREADS - 1) / THREADS), N);
+  const long threads = (long)(C / 4) * fwd_runs(Tp, padL, pool_d, pool_T).total;
+  dim3 grid((unsigned)((threads + FWD_THREADS - 1) / FWD_THREADS), N);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_FWD(YT, DF)                                                                       \
-  PASE_LAUNCH((bn_prelu_pad_fwd_kernel<YT, DF>), grid, THREADS, 0, st,                         \
+  PASE_LAUNCH((bn_prelu_pad_fwd_kernel<YT, DF>), grid, FWD_THREADS, 0, st,                     \
       reinterpret_cast<const YT*>(y), y_sample_stride, T, C, scale, shift, alpha, dst,         \
       dst_sample_stride, dst_row_stride, padL, Tp, pool, pool_sample_stride, pool_row_stride,  \
       pool_d, pool_T, dst_lo)
@@ -1550,11 +1634,14 @@ int pase_bn_prelu_pad_fwd_var(const void* y, int y_bf16, const int* tab, int nse
       PASE_CHECK_STRIDE(fn, pool_row_stride, "pool_row_stride");
     }
   }
-  const long threads = (long)(C / 4) * (((long)max_T + padL + padR + RUN - 1) / RUN);
-  dim3 grid((unsigned)((threads + THREADS - 1) / THREADS), nseg);
+  // each utterance's pool_d / pool_T live in the device table: size for the most runs any
+  // T <= max_T can need (cutting [0, Tp) into three ranges adds at most two partial runs, and
+  // a pooled run is never shorter than RUN)
+  const long threads = (long)(C / 4) * (((long)max_T + padL + padR + RUN - 1) / RUN + 2);
+  dim3 grid((unsigned)((threads + FWD_THREADS - 1) / FWD_THREADS), nseg);
   cudaStream_t st = (cudaStream_t)stream;
 #define PASE_FWD(YT, DF)                                                                       \
-  PASE_LAUNCH((bn_prelu_pad_fwd_var_kernel<YT, DF>), grid, THREADS, 0, st,                     \
+  PASE_LAUNCH((bn_prelu_pad_fwd_var_kernel<YT, DF>), grid, FWD_THREADS, 0, st,                 \
       reinterpret_cast<const YT*>(y), tab, C, scale, shift, alpha, dst, dst_row_stride, padL,  \
       padR, pool, pool_row_stride, sep, dst_lo)
   if (y_bf16) {
