@@ -438,11 +438,52 @@ def _conv_weight_operands(plan, P):
         plan.w_batch(0, jobs)
 
 
-def _sinc_weights(plan, mod, P, l, g):
+def _dgrad_weight_operands(plan, P):
+    """Data-gradient GEMM operands (in the plan's operand format) of every conv block with an
+    input gradient: one launch."""
+    jobs = []
+    for l, g in enumerate(plan.geoms):
+        if not g.sinc and l > 0:
+            hi, lo = plan.w_operand(("Wd", l), plan.Wd[l])
+            dst = plan.Wd[l] if plan.precision.fmt == gemm.FMT_F32 else None
+            jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
+                         g.s, g.taps, g.s * g.Cin * g.taps * g.Cout))
+    if jobs:
+        plan.w_batch(1, jobs)
+
+
+def _sinc_weights(plan, mod, P, l, g, filt=None):
+    """The sinc layer's polyphase GEMM operand in plan.Wt[l] (and its band-pass bank in `filt`)
+    from low_hz_ / band_hz_."""
     pre = "blocks.%d." % l
     ops.call("pase_sinc_make", P(pre + "conv.low_hz_"), P(pre + "conv.band_hz_"),
-             mod._sinc_n, mod._sinc_win, None, plan.Wt[l], g.Cout, g.k, g.fold, g.K,
+             mod._sinc_n, mod._sinc_win, filt, plan.Wt[l], g.Cout, g.k, g.fold, g.K,
              50.0, 50.0, float(plan.cfg["sr"]))
+
+
+def _sinc_dgrad_weights(plan, mod, P, g):
+    """The sinc layer's banded dgrad operand plan.Wdg (DESIGN.md section 17), from the band-pass
+    bank regenerated into plan.filt."""
+    _sinc_weights(plan, mod, P, g.idx, g, plan.filt)
+    ops.call("pase_sinc_dgrad_weight", plan.filt, plan.Wdg, g.Cout, g.k, g.fold, g.dg_rows)
+
+
+def _sinc_weight_grads(plan, mod, params, g, sink, grads):
+    """low_hz_ / band_hz_ gradients from the sinc layer's weight gradient in plan.dWt: written
+    into the sink, or new tensors added to `grads`."""
+    pre = "blocks.%d." % g.idx
+    P = lambda name: _flat(params[name])
+    if sink is not None:
+        dlow, dband = sink[pre + "conv.low_hz_"], sink[pre + "conv.band_hz_"]
+    else:
+        dlow = torch.empty_like(params[pre + "conv.low_hz_"])
+        dband = torch.empty_like(params[pre + "conv.band_hz_"])
+    ops.call("pase_sinc_grad", plan.dWt[g.idx], P(pre + "conv.low_hz_"),
+             P(pre + "conv.band_hz_"), mod._sinc_n, mod._sinc_win, dlow.reshape(-1),
+             dband.reshape(-1), g.Cout, g.k, g.fold, g.K, 50.0, 50.0, float(plan.cfg["sr"]))
+    if sink is None:
+        grads[pre + "conv.low_hz_"] = dlow
+        grads[pre + "conv.band_hz_"] = dband
 
 
 def _bn_eval_affine(plan, P, buf, l, g):
@@ -476,6 +517,34 @@ def _out_bn_eval_affine(plan, buf):
              None, None, plan.emb, BN_EPS, bo[0], bo[1], bo[2], bo[3])
 
 
+def _out_proj(plan, mod, params, rows, counters=None):
+    """The output projection [W | skips] of the first `rows` frames of plan.cat into plan.yout
+    (uniform over the frames) and the norm_out affine into plan.bn_out: eval mode, or (counters
+    given: train mode) the statistics of the `rows` frames, whose num_batches_tracked buffer is
+    appended to counters for the caller to increment."""
+    Kc, emb = plan.Kc, plan.emb
+    buf = lambda name: _flat(mod.get_buffer(name))
+    _out_weights(plan, params)
+    cs = cq = None
+    if plan.norm_out and counters is not None:
+        o = plan.fs_out
+        cs, cq = plan.stats_f[o:o + emb], plan.stats_f[o + emb:o + 2 * emb]
+    gemm.nt(plan.precision, plan.cat, Kc, rows * Kc, plan.Wcat, Kc, plan.yout, emb, rows, emb,
+            Kc, 1.0, _flat(params["W.bias"]), cs=cs, cq=cq,
+            a_op=lambda: plan.operand("cat", plan.cat, True, n=rows * Kc),
+            b_op=lambda: plan.operand("Wcat", plan.Wcat, True, "weight"))
+    if not plan.norm_out:
+        return
+    if cs is not None:
+        bo = plan.bn_out
+        ops.call("pase_bn_finalize", cs, cq, emb, 1, float(rows), None, None,
+                 buf("norm_out.running_mean"), buf("norm_out.running_var"), BN_MOMENTUM, BN_EPS,
+                 bo[0], bo[1], bo[2], bo[3])
+        counters.append(mod.get_buffer("norm_out.num_batches_tracked"))
+    else:
+        _out_bn_eval_affine(plan, buf)
+
+
 def encoder_forward(plan, mod, x, params, training, save_for_backward):
     """x: (N,1,T) fp32 CUDA tensor.  params: dict name -> tensor.  Returns
     (out (N,emb,Tq), out_ntc (N*Tq, emb))."""
@@ -496,7 +565,7 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
         plan.cat.zero_()
 
     _conv_weight_operands(plan, P)
-    counters = []
+    counters = [] if training else None
 
     for l, g in enumerate(G):
         pre = "blocks.%d." % l
@@ -553,26 +622,10 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
                 Tq + 1, Tq, Tq, 1, None, None, 0)
         call("pase_qrnn_scan_fwd", plan.Yg, plan.cat, Kc, plan.Cst, N, Tq, H)
 
-    _out_weights(plan, params)
-    use_stats = plan.norm_out and training
-    if use_stats:
-        o = plan.fs_out
-        cs, cq = plan.stats_f[o:o + emb], plan.stats_f[o + emb:o + 2 * emb]
-    else:
-        cs = cq = None
-    plan.nt("cat", plan.cat, Kc, True, "Wcat", plan.Wcat, Kc, True, plan.yout, emb,
-            rows, emb, Kc, 1.0, P("W.bias"), rows, rows, rows, 1, cs, cq, 0)
-    bo = plan.bn_out
-    if plan.norm_out:
-        if training:
-            call("pase_bn_finalize", cs, cq, emb, 1, float(rows), None, None,
-                 buf("norm_out.running_mean"), buf("norm_out.running_var"),
-                 BN_MOMENTUM, BN_EPS, bo[0], bo[1], bo[2], bo[3])
-            counters.append(mod.get_buffer("norm_out.num_batches_tracked"))
-        else:
-            _out_bn_eval_affine(plan, buf)
+    _out_proj(plan, mod, params, rows, counters)
     if counters:                                 # BatchNorm step counters: one launch
         torch._foreach_add_(counters, 1)
+    bo = plan.bn_out
     out = torch.empty(N, emb, Tq, dtype=torch.float32, device=x.device)
     out_ntc = torch.empty(rows, emb, dtype=torch.float32, device=x.device)
     call("pase_out_affine_nct", plan.yout, bo[2], bo[3], out.reshape(-1), out_ntc.reshape(-1),
@@ -677,12 +730,7 @@ class PackedPlan(EncoderPlan):
         if self.rnn:
             sizes += [("QRNN input", (rows + self.max_utts) * self.Clast + 2 * self.Clast + 64),
                       ("QRNN gates", rows * 3 * self.H)]
-        for what, n in sizes:
-            if n >= INDEX_LIMIT:
-                raise ValueError(
-                    "a pack of %d samples needs %d elements for the %s, beyond the 32-bit indices "
-                    "of the packed kernels: split it into shorter utterances"
-                    % (self.capacity, n, what))
+        _check_indices(self.capacity, sizes)
         self.rows_cap = rows
         self._alloc(n_apad, n_y, rows, rows + self.max_utts)
         self.wave = torch.zeros(self.capacity, dtype=torch.float32, device=device)
@@ -690,9 +738,37 @@ class PackedPlan(EncoderPlan):
                                  device=device)
 
 
+def _check_indices(capacity, sizes):
+    """ValueError unless every (what, elements) of a plan for packs of `capacity` samples is
+    addressable by the packed kernels' 32-bit indices."""
+    for what, n in sizes:
+        if n >= INDEX_LIMIT:
+            raise ValueError(
+                "a pack of %d samples needs %d elements for the %s, beyond the 32-bit indices "
+                "of the packed kernels: split it into shorter utterances" % (capacity, n, what))
+
+
 def _table_size(nblk, n):
     # wave, per block (GEMM map + BN/PReLU rows), QRNN GEMM map, scan, output
     return 3 * n + nblk * (3 * n + 1 + 6 * n) + (3 * n + 1) + 2 * n + 3 * n
+
+
+def _cum0(a):
+    """Exclusive prefix sums over the first axis, with the total as the last row."""
+    return np.concatenate([np.zeros((1,) + a.shape[1:], np.int64), np.cumsum(a, 0)])
+
+
+def _packed_offsets(plan, geoms):
+    """Per utterance and block of a pack: rows per sample P and output frames T_out, (n, nblk);
+    the first row of every utterance in each block's padded operand (row0) and raw output
+    (orow0); its output frames Tq, first output frame q0 and first QRNN input row xr0 (one
+    separator row per utterance).  The offsets have n + 1 rows, the last the total."""
+    n = len(geoms)
+    P = np.array([[g.P for g in gi] for gi in geoms], dtype=np.int64).reshape(n, plan.nblk)
+    RO = np.array([[g.rows_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
+    TO = np.array([[g.T_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
+    Tq = TO[:, -1]
+    return P, TO, _cum0(P), _cum0(RO), Tq, _cum0(Tq), _cum0(Tq + 1)
 
 
 def packed_layout(plan, lengths, geoms, mode):
@@ -700,16 +776,10 @@ def packed_layout(plan, lengths, geoms, mode):
     -> (host table, {section: offset}, dict of sizes).  Utterance i's rows are contiguous at
     every layer; each padded operand starts on a folded-row boundary of its GEMM."""
     G, n = plan.geoms, len(lengths)
-    P = np.array([[g.P for g in gi] for gi in geoms], dtype=np.int64).reshape(n, plan.nblk)
-    RO = np.array([[g.rows_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
-    TO = np.array([[g.T_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
-    cum = lambda a: np.concatenate([np.zeros((1,) + a.shape[1:], np.int64), np.cumsum(a, 0)])
-    row0, orow0 = cum(P), cum(RO)
-    Tq = TO[:, -1]
-    q0, xr0 = cum(Tq), cum(Tq + 1)
+    _, TO, row0, orow0, Tq, q0, xr0 = _packed_offsets(plan, geoms)
     E = plan.emb * (2 if mode in ("avg_concat", "avg_norm_concat") else 1)
-    o0 = cum(E * Tq)
-    x0 = cum(np.asarray(lengths, dtype=np.int64))
+    o0 = _cum0(E * Tq)
+    x0 = _cum0(np.asarray(lengths, dtype=np.int64))
     Kc, sec, parts = plan.Kc, {}, []
 
     def put(name, *cols, rows=None):
@@ -757,7 +827,7 @@ def encoder_forward_packed(plan, mod, x, lengths, geoms, params, mode=None, layo
     if plan.rnn:
         ops.call("pase_qrnn_scan_fwd_var", plan.Yg, plan.cat, plan.Kc, plan.Cst, tab("scan"), n,
                  plan.H)
-    _packed_out_proj(plan, mod, params, sz["rows"], counters)
+    _out_proj(plan, mod, params, sz["rows"], counters)
     if counters:                                 # BatchNorm step counters: one launch
         torch._foreach_add_(counters, 1)
     bo = plan.bn_out
@@ -844,33 +914,6 @@ def _packed_front_launch(plan, mod, x, sz, tab, params, counters=None):
                     1)
 
 
-def _packed_out_proj(plan, mod, params, rows, counters=None):
-    """The output projection [W | skips] of `rows` packed frames into plan.yout (uniform over
-    the frames) and the norm_out affine into plan.bn_out: eval mode, or (counters given) the
-    statistics of the `rows` frames, as _packed_front_launch."""
-    Kc, emb = plan.Kc, plan.emb
-    buf = lambda name: _flat(mod.get_buffer(name))
-    _out_weights(plan, params)
-    cs = cq = None
-    if plan.norm_out and counters is not None:
-        o = plan.fs_out
-        cs, cq = plan.stats_f[o:o + emb], plan.stats_f[o + emb:o + 2 * emb]
-    gemm.nt(plan.precision, plan.cat, Kc, rows * Kc, plan.Wcat, Kc, plan.yout, emb, rows, emb,
-            Kc, 1.0, _flat(params["W.bias"]), cs=cs, cq=cq,
-            a_op=lambda: plan.operand("cat", plan.cat, True, n=rows * Kc),
-            b_op=lambda: plan.operand("Wcat", plan.Wcat, True, "weight"))
-    if not plan.norm_out:
-        return
-    if cs is not None:
-        bo = plan.bn_out
-        ops.call("pase_bn_finalize", cs, cq, emb, 1, float(rows), None, None,
-                 buf("norm_out.running_mean"), buf("norm_out.running_var"), BN_MOMENTUM, BN_EPS,
-                 bo[0], bo[1], bo[2], bo[3])
-        counters.append(mod.get_buffer("norm_out.num_batches_tracked"))
-    else:
-        _out_bn_eval_affine(plan, buf)
-
-
 # -- packed variable-length backward (DESIGN.md section 18) -----------------------------------
 _BWD_ROW = 9            # {T, y_off, a_off, b_off, pool_off, pool_d, pool_T, d_off, d_span}
 
@@ -904,12 +947,7 @@ class PackedGradPlan(PackedPlan):
         sizes = [("block %d output gradient" % g.idx, nd) for g, nd in zip(G, self.n_dyz)]
         if self.rnn:
             sizes.append(("QRNN gate gradient", self.yg_rows * 3 * self.H + 64))
-        for what, n in sizes:
-            if n >= INDEX_LIMIT:
-                raise ValueError(
-                    "a pack of %d samples needs %d elements for the %s, beyond the 32-bit indices "
-                    "of the packed kernels: split it into shorter utterances"
-                    % (self.capacity, n, what))
+        _check_indices(self.capacity, sizes)
         self.table = torch.zeros(_table_size(self.nblk, self.max_utts)
                                  + _grad_table_size(self.nblk, self.max_utts),
                                  dtype=torch.int32, device=device)
@@ -941,13 +979,7 @@ def packed_grad_layout(plan, lengths, geoms, mode=None):
     forward's sections in one copy; the plan keeps (sections, sizes) for the backward."""
     host, sec, sz = packed_layout(plan, lengths, geoms, mode)
     G, n = plan.geoms, len(lengths)
-    P = np.array([[g.P for g in gi] for gi in geoms], dtype=np.int64).reshape(n, plan.nblk)
-    RO = np.array([[g.rows_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
-    TO = np.array([[g.T_out for g in gi] for gi in geoms], dtype=np.int64).reshape(n, -1)
-    cum = lambda a: np.concatenate([np.zeros((1,) + a.shape[1:], np.int64), np.cumsum(a, 0)])
-    row0, orow0 = cum(P), cum(RO)
-    Tq = TO[:, -1]
-    q0, xr0 = cum(Tq), cum(Tq + 1)
+    P, TO, row0, orow0, Tq, q0, xr0 = _packed_offsets(plan, geoms)
     Kc, parts, base = plan.Kc, [host.numpy().astype(np.int64)], host.numel()
     zero = np.zeros(n, np.int64)
 
@@ -1009,7 +1041,7 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
     call = ops.call
     sec, sz = plan.layout
     tab = lambda name: plan.table[sec[name]:]
-    cfg, G, n = plan.cfg, plan.geoms, len(sz["Tq"])
+    G, n = plan.geoms, len(sz["Tq"])
     rows, Kc, emb = sz["rows"], plan.Kc, plan.emb
     P = lambda name: _flat(params[name])
     grads, copies = {}, []
@@ -1018,15 +1050,7 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
     if plan.amax is not None:
         plan.amax.zero_()
     fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
-    jobs = []
-    for l, g in enumerate(G):
-        if not g.sinc and l > 0:
-            hi, lo = plan.w_operand(("Wd", l), plan.Wd[l])
-            dst = plan.Wd[l] if fmt == gemm.FMT_F32 else None
-            jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
-                         g.s, g.taps, g.s * g.Cin * g.taps * g.Cout))
-    if jobs:
-        plan.w_batch(1, jobs)
+    _dgrad_weight_operands(plan, P)
     bo = plan.bn_out
     o = plan.bs_out
     S1o, S2o = sb[o:o + emb], sb[o + emb:o + 2 * emb]
@@ -1104,23 +1128,10 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
             if pg:
                 plan.tn(("dyz", l), plan.dyz[l], g.Nn, M, g.dg_rows - 1, False, ("apad", l),
                         plan.apad[l], g.lda, M, False, plan.dWt[l], g.K, g.Nn, g.K, 1, M, 1.0, 0)
-                if sink is not None:
-                    dlow, dband = sink[pre + "conv.low_hz_"], sink[pre + "conv.band_hz_"]
-                else:
-                    dlow = torch.empty_like(params[pre + "conv.low_hz_"])
-                    dband = torch.empty_like(params[pre + "conv.band_hz_"])
-                call("pase_sinc_grad", plan.dWt[l], P(pre + "conv.low_hz_"),
-                     P(pre + "conv.band_hz_"), mod._sinc_n, mod._sinc_win, dlow.reshape(-1),
-                     dband.reshape(-1), g.Cout, g.k, g.fold, g.K, 50.0, 50.0, float(cfg["sr"]))
-                if sink is None:
-                    grads[pre + "conv.low_hz_"] = dlow
-                    grads[pre + "conv.band_hz_"] = dband
+                _sinc_weight_grads(plan, mod, params, g, sink, grads)
             if dx is not None:
                 f = g.fold
-                call("pase_sinc_make", P(pre + "conv.low_hz_"), P(pre + "conv.band_hz_"),
-                     mod._sinc_n, mod._sinc_win, plan.filt, plan.Wt[0], g.Cout, g.k, f, g.K,
-                     50.0, 50.0, float(cfg["sr"]))
-                call("pase_sinc_dgrad_weight", plan.filt, plan.Wdg, g.Cout, g.k, f, g.dg_rows)
+                _sinc_dgrad_weights(plan, mod, P, g)
                 plan.nt(("dyz", l), plan.dyz[l], g.Nn, False, "Wdg", plan.Wdg, g.dg_K, True,
                         plan.dxpad[0], f, M, f, g.dg_K, 1.0, None, M, M, M, 1, None, None, 0,
                         akind="grad")
@@ -1148,6 +1159,23 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
     return _autograd_grads(plan, G, grads)
 
 
+def _grad_sink(mod, names):
+    """mod.grad_sink (None when unset), refused unless it names every parameter in `names`."""
+    sink = getattr(mod, "grad_sink", None)
+    if sink is not None and any(nm not in sink for nm in names):
+        raise RuntimeError("pase_b200: WaveFe.grad_sink must name every parameter "
+                           "(missing %s)" % [nm for nm in names if nm not in sink][:3])
+    return sink
+
+
+def _check_generation(ctx, buffers, later, hint=""):
+    """Refuse a backward whose forward's activations in ctx.plan were replaced: every forward
+    through a plan bumps its generation, and the forward saved the one it left in ctx."""
+    if ctx.plan.generation != ctx.generation:
+        raise RuntimeError("pase_b200: %s were overwritten by a later %s before this backward "
+                           "ran; run backward before the next forward%s." % (buffers, later, hint))
+
+
 class _PackedEncoderFn(torch.autograd.Function):
     """Autograd node of WaveFe.encode_packed (eval mode) and WaveFe.encode_packed_train
     (training): one packed forward of n utterances (tensors = the n flat CUDA waveforms, then
@@ -1170,21 +1198,15 @@ class _PackedEncoderFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *gouts):
         plan, n = ctx.plan, ctx.n
-        if plan.generation != ctx.generation:
-            raise RuntimeError(
-                "pase_b200: the activation buffers of encode_packed were overwritten by a later "
-                "encode_packed forward on the same plan before this backward ran; run backward "
-                "before the next forward.")
+        _check_generation(ctx, "the activation buffers of encode_packed",
+                          "encode_packed forward on the same plan")
         params = dict(zip(ctx.names, ctx.saved_tensors))
         need_x = ctx.needs_input_grad[7:7 + n]
         param_grads = any(ctx.needs_input_grad[7 + n:])        # all or nothing, as _EncoderFn
         none = (None,) * 7
         if not param_grads and not any(need_x):
             return none + (None,) * (n + len(ctx.names))
-        sink = getattr(ctx.mod, "grad_sink", None)
-        if sink is not None and any(nm not in sink for nm in ctx.names):
-            raise RuntimeError("pase_b200: WaveFe.grad_sink must name every parameter "
-                               "(missing %s)" % [nm for nm in ctx.names if nm not in sink][:3])
+        sink = _grad_sink(ctx.mod, ctx.names)
         sec, sz = plan.layout
         emb = plan.emb
         gflat = plan.gflat[:sz["out"]]
@@ -1473,7 +1495,7 @@ def _window_forward(plan, mod, wav, seg, k, geom, params, log, state):
         state.copy_(log[k])
         ops.call("pase_qrnn_scan_fwd_carry_var", plan.Yg, plan.cat, plan.Kc, plan.Cst, state,
                  tab("carry"), 1, plan.H)
-    _packed_out_proj(plan, mod, params, sz["rows"])
+    _out_proj(plan, mod, params, sz["rows"])
 
 
 def _window_backward(plan, mod, params, wav, segs, log, gout, dx, param_grads, sink):
@@ -1557,10 +1579,7 @@ class _LongEncoderFn(torch.autograd.Function):
         if gout is None or not (need_x or param_grads):
             return none + (None,) * (1 + len(tensors))
         mod = ctx.mod
-        sink = getattr(mod, "grad_sink", None) if param_grads else None
-        if sink is not None and any(nm not in sink for nm in ctx.names):
-            raise RuntimeError("pase_b200: WaveFe.grad_sink must name every parameter "
-                               "(missing %s)" % [nm for nm in ctx.names if nm not in sink][:3])
+        sink = _grad_sink(mod, ctx.names) if param_grads else None
         plan = mod._grad_plan(window_capacity(mod.cfg, ctx.window), x.device)
         mod._sinc_consts(x.device)
         dx = torch.zeros(x.numel(), dtype=torch.float32, device=x.device) if need_x else None
@@ -1617,7 +1636,7 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
         sink = None
     pg = param_grads
     call = ops.call
-    cfg, G, N = plan.cfg, plan.geoms, plan.N
+    G, N = plan.geoms, plan.N
     Tq, Kc, rows, emb = plan.Tq, plan.Kc, plan.rows, plan.emb
     P = lambda name: _flat(params[name])
     grads = {}
@@ -1626,16 +1645,7 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     if plan.amax is not None:
         plan.amax.zero_()
     fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
-    # dgrad operands (operand format) of every conv block with an input gradient: one launch
-    jobs = []
-    for l, g in enumerate(G):
-        if not g.sinc and l > 0:
-            hi, lo = plan.w_operand(("Wd", l), plan.Wd[l])
-            dst = plan.Wd[l] if plan.precision.fmt == gemm.FMT_F32 else None
-            jobs.append((P("blocks.%d.conv.weight" % l), dst, hi, lo, g.Cout, g.Cin, g.k,
-                         g.s, g.taps, g.s * g.Cin * g.taps * g.Cout))
-    if jobs:
-        plan.w_batch(1, jobs)
+    _dgrad_weight_operands(plan, P)
     zeros = plan.zeros64
     bo = plan.bn_out
     o = plan.bs_out
@@ -1724,17 +1734,7 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
         if g.sinc and pg:
             plan.tn(("dyz", l), plan.dyz[l], g.Nn, g.rows_out, 0, False, ("apad", l), plan.apad[l],
                     g.lda, g.P, False, plan.dWt[l], g.K, g.Nn, g.K, N, g.rows_out, 1.0, 0)
-            if sink is not None:
-                dlow, dband = sink[pre + "conv.low_hz_"], sink[pre + "conv.band_hz_"]
-            else:
-                dlow = torch.empty_like(params[pre + "conv.low_hz_"])
-                dband = torch.empty_like(params[pre + "conv.band_hz_"])
-            call("pase_sinc_grad", plan.dWt[l], P(pre + "conv.low_hz_"),
-                 P(pre + "conv.band_hz_"), mod._sinc_n, mod._sinc_win, dlow.reshape(-1),
-                 dband.reshape(-1), g.Cout, g.k, g.fold, g.K, 50.0, 50.0, float(cfg["sr"]))
-            if sink is None:
-                grads[pre + "conv.low_hz_"] = dlow
-                grads[pre + "conv.band_hz_"] = dband
+            _sinc_weight_grads(plan, mod, params, g, sink, grads)
         elif not g.sinc:
             if pg:
                 plan.tn(("dyz", l), plan.dyz[l], C, g.Pd, g.taps - 1, False, ("apad", l),
@@ -1825,10 +1825,7 @@ def _sinc_input_grad(plan, mod, P, g, dx):
     its banded dgrad operand, a copy of dy with a zero halo around every sample, one polyphase
     GEMM into the padded-waveform gradient and the reflect fold-back."""
     call, N, f, p = ops.call, plan.N, g.fold, plan.precision
-    call("pase_sinc_make", P("blocks.0.conv.low_hz_"), P("blocks.0.conv.band_hz_"), mod._sinc_n,
-         mod._sinc_win, plan.filt, plan.Wt[0], g.Cout, g.k, f, g.K, 50.0, 50.0,
-         float(plan.cfg["sr"]))
-    call("pase_sinc_dgrad_weight", plan.filt, plan.Wdg, g.Cout, g.k, f, g.dg_rows)
+    _sinc_dgrad_weights(plan, mod, P, g)
     call("pase_sinc_dgrad_pack", plan.dyz[0], plan.dyz_lo[0], plan.dyh, plan.dyh_lo, p.esz, N,
          g.Cout, g.T_out, g.Ty, g.dg_halo, g.dg_P * f)
     plan.nt(("dyh", 0), plan.dyh, g.Nn, False, "Wdg", plan.Wdg, g.dg_K, True, plan.dxpad[0], f,
@@ -1909,20 +1906,14 @@ class _EncoderFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout, gntc):
         plan = ctx.plan
-        if plan.generation != ctx.generation:
-            raise RuntimeError(
-                "pase_b200: the encoder's activation buffers were overwritten by a later "
-                "forward of the same (N,T) shape before this backward ran; run backward "
-                "before the next forward (or build a second WaveFe instance).")
+        _check_generation(ctx, "the encoder's activation buffers",
+                          "forward of the same (N,T) shape", " (or build a second WaveFe instance)")
         params = dict(zip(ctx.names, ctx.saved_tensors))
         if gout is not None:
             gout = gout.contiguous()
         if gntc is not None:
             gntc = gntc.contiguous()
-        sink = getattr(ctx.mod, "grad_sink", None)
-        if sink is not None and any(n not in sink for n in ctx.names):
-            raise RuntimeError("pase_b200: WaveFe.grad_sink must name every parameter "
-                               "(missing %s)" % [n for n in ctx.names if n not in sink][:3])
+        sink = _grad_sink(ctx.mod, ctx.names)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(plan.N, 1, plan.T, dtype=torch.float32, device=plan.device)

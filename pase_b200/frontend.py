@@ -200,44 +200,32 @@ class WaveFe(Model):
         wide = all(f % 64 == 0 for f in self.cfg["fmaps"])
         return "3xf16" if wide else "3xtf32"
 
+    def _cached_plan(self, cache, key, build):
+        """cache[key], built by build() on a miss; the cache keeps the MAX_PLANS most recently
+        used plans."""
+        plan = cache.get(key)
+        if plan is None:
+            plan = cache[key] = build()
+            while len(cache) > self.MAX_PLANS:
+                cache.popitem(last=False)
+        else:
+            cache.move_to_end(key)
+        return plan
+
     def _plan(self, N, T, device):
         prec = self.resolved_precision()
-        key = (N, T, str(device), prec)
-        plan = self._plans.get(key)
-        if plan is None:
-            plan = _enc.EncoderPlan(self.cfg, N, T, device, prec)
-            self._plans[key] = plan
-            while len(self._plans) > self.MAX_PLANS:
-                self._plans.popitem(last=False)
-        else:
-            self._plans.move_to_end(key)
-        return plan
+        return self._cached_plan(self._plans, (N, T, str(device), prec),
+                                 lambda: _enc.EncoderPlan(self.cfg, N, T, device, prec))
 
     def _packed_plan(self, capacity, device):
         prec = self.resolved_precision()
-        key = (capacity, str(device), prec)
-        plan = self._packed_plans.get(key)
-        if plan is None:
-            plan = _enc.PackedPlan(self.cfg, capacity, device, prec)
-            self._packed_plans[key] = plan
-            while len(self._packed_plans) > self.MAX_PLANS:
-                self._packed_plans.popitem(last=False)
-        else:
-            self._packed_plans.move_to_end(key)
-        return plan
+        return self._cached_plan(self._packed_plans, (capacity, str(device), prec),
+                                 lambda: _enc.PackedPlan(self.cfg, capacity, device, prec))
 
     def _grad_plan(self, capacity, device):
         prec = self.resolved_precision()
-        key = (capacity, prec, str(device))
-        plan = self._grad_plans.get(key)
-        if plan is None:
-            plan = _enc.PackedGradPlan(self.cfg, capacity, device, prec)
-            self._grad_plans[key] = plan
-            while len(self._grad_plans) > self.MAX_PLANS:
-                self._grad_plans.popitem(last=False)
-        else:
-            self._grad_plans.move_to_end(key)
-        return plan
+        return self._cached_plan(self._grad_plans, (capacity, prec, str(device)),
+                                 lambda: _enc.PackedGradPlan(self.cfg, capacity, device, prec))
 
     def _sinc_consts(self, device):
         if self._sinc_n is None or self._sinc_n.device != device:
@@ -284,15 +272,8 @@ class WaveFe(Model):
     def _extract(self, wavs, mode, max_samples, device):
         if mode not in _enc.OUT_MODES:
             raise ValueError("mode must be one of %s, got %r" % (list(_enc.OUT_MODES), mode))
-        cap = EXTRACT_MAX_SAMPLES if max_samples is None else int(max_samples)
-        if cap < 1:
-            raise ValueError("max_samples must be positive, got %r" % (max_samples,))
-        flat = []
-        for i, w in enumerate(wavs):
-            try:
-                flat.append(_recording(w))
-            except (TypeError, ValueError) as e:
-                raise type(e)("utterance %d: %s" % (i, e)) from None
+        cap = self._packed_cap(max_samples)
+        flat = self._packed_inputs(wavs)
         if not flat:
             return []
         lengths = [w.numel() for w in flat]
@@ -344,10 +325,7 @@ class WaveFe(Model):
         if not self.training:
             raise RuntimeError("WaveFe.encode_packed_train runs the encoder in train mode; in "
                                "eval mode use encode_packed")
-        device = self.W.weight.device
-        if device.type != "cuda":
-            raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; the module lives "
-                               "on %s. There is no CPU path." % device)
+        device = self._device()
         flat = self._packed_inputs(wavs)
         if not flat:
             return []
@@ -401,6 +379,10 @@ class WaveFe(Model):
         if self.training:
             raise RuntimeError("WaveFe.%s runs the encoder in eval mode; call .eval() first"
                                % what)
+        return self._device()
+
+    def _device(self):
+        """The module's device, which must be a CUDA one."""
         device = self.W.weight.device
         if device.type != "cuda":
             raise RuntimeError("pase_b200.WaveFe runs on CUDA (sm_90a) only; the module lives "
@@ -423,11 +405,8 @@ class WaveFe(Model):
         if mode not in _enc.OUT_MODES:
             raise ValueError("mode must be one of %s, got %r" % (list(_enc.OUT_MODES), mode))
         x = _recording(wav)
-        win = EXTRACT_LONG_WINDOW if window is None else int(window)
         cfg, L = self.cfg, x.numel()
-        if win < _enc.min_window(cfg):
-            raise ValueError("window must be at least %d samples, got %d"
-                             % (_enc.min_window(cfg), win))
+        win = _check_window(cfg, EXTRACT_LONG_WINDOW if window is None else window)
         if L <= win:
             return self._extract([x], mode, win, device)[0]
         if x.is_cuda and x.device != device:
@@ -477,11 +456,8 @@ class WaveFe(Model):
             raise RuntimeError("WaveFe.encode_long: the recording lives on %s, the module on "
                                "%s; move it to the module's device (its gradient is returned "
                                "there)" % (x.device, device))
-        win = EXTRACT_LONG_WINDOW if window is None else int(window)
         cfg, L = self.cfg, x.numel()
-        if win < _enc.min_window(cfg):
-            raise ValueError("window must be at least %d samples, got %d"
-                             % (_enc.min_window(cfg), win))
+        win = _check_window(cfg, EXTRACT_LONG_WINDOW if window is None else window)
         if L < _enc.min_length(cfg):
             raise ValueError("a recording of %d samples is shorter than the encoder's minimum "
                              "of %d" % (L, _enc.min_length(cfg)))
@@ -552,6 +528,15 @@ def _recording(w):
     return w.reshape(-1).contiguous()
 
 
+def _check_window(cfg, window):
+    """A window of `window` samples (int), refused below encoder.min_window."""
+    win = int(window)
+    if win < _enc.min_window(cfg):
+        raise ValueError("window must be at least %d samples, got %d"
+                         % (_enc.min_window(cfg), win))
+    return win
+
+
 class FeatureStream(object):
     """Online feature extraction of one recording (WaveFe.stream()).  push(samples) returns the
     (1, emb, n) frames that became final (n may be 0): frame j is final once sample
@@ -609,10 +594,7 @@ class StreamPool(object):
 
     def __init__(self, model, device, max_streams, window=None, max_samples=None):
         cfg = model.cfg
-        win = _enc.min_window(cfg) if window is None else int(window)
-        if win < _enc.min_window(cfg):
-            raise ValueError("window must be at least %d samples, got %d"
-                             % (_enc.min_window(cfg), win))
+        win = _check_window(cfg, _enc.min_window(cfg) if window is None else window)
         if not 1 <= int(max_streams) <= 65535:           # one grid row per stream
             raise ValueError("max_streams must be in 1..65535, got %r" % (max_streams,))
         cap = STREAM_POOL_MAX_SAMPLES if max_samples is None else int(max_samples)
@@ -844,7 +826,7 @@ class StreamPool(object):
                             row.copy_(self.state[slot * H:(slot + 1) * H])
                 call("pase_qrnn_scan_fwd_carry_var", plan.Yg, plan.cat, plan.Kc, plan.Cst,
                      self.state, tab[job["carry"]:], job["segs"], plan.H)
-            _enc._packed_out_proj(plan, self.model, params, sz["rows"])
+            _enc._out_proj(plan, self.model, params, sz["rows"])
             call("pase_out_place_var", plan.yout, bo[2], bo[3], out, tab[job["place"]:],
                  job["segs"], job["max_T"], emb)
 
