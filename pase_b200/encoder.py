@@ -486,12 +486,57 @@ def _sinc_weight_grads(plan, mod, params, g, sink, grads):
         grads[pre + "conv.band_hz_"] = dband
 
 
-def _bn_eval_affine(plan, P, buf, l, g):
+def _block_conv_inputs(plan, mod, P, l, g, training):
+    """Block l's conv bias (the sinc layer: None, and its band-pass operand regenerated into
+    plan.Wt[l]) and, in train mode, its BatchNorm sums in plan.stats_f (else None, None)."""
+    if g.sinc:
+        _sinc_weights(plan, mod, P, l, g)
+        bias = None
+    else:
+        bias = P("blocks.%d.conv.bias" % l)
+    if not training:
+        return bias, None, None
+    o = plan.fs_off[l]
+    return bias, plan.stats_f[o:o + g.Nn], plan.stats_f[o + g.Nn:o + 2 * g.Nn]
+
+
+def _block_bn(plan, mod, P, l, g, cs, cq, count, counters):
+    """Block l's BatchNorm affine into plan.bn[l]: eval mode, from the running statistics, or
+    (counters given: train mode) from the sums cs / cq over `count` frames, which also update the
+    running statistics; the num_batches_tracked buffer is appended to counters for the caller to
+    increment."""
     pre = "blocks.%d." % l
+    buf = lambda name: _flat(mod.get_buffer(name))
     mean, invstd, scale, shift = plan.bn[l][0], plan.bn[l][1], plan.bn[l][2], plan.bn[l][3]
-    ops.call("pase_bn_eval_affine", buf(pre + "norm.running_mean"),
-             buf(pre + "norm.running_var"), P(pre + "norm.weight"), P(pre + "norm.bias"),
-             g.Cout, BN_EPS, mean, invstd, scale, shift)
+    if counters is None:
+        ops.call("pase_bn_eval_affine", buf(pre + "norm.running_mean"),
+                 buf(pre + "norm.running_var"), P(pre + "norm.weight"), P(pre + "norm.bias"),
+                 g.Cout, BN_EPS, mean, invstd, scale, shift)
+        return
+    ops.call("pase_bn_finalize", cs, cq, g.Cout, g.fold, float(count), P(pre + "norm.weight"),
+             P(pre + "norm.bias"), buf(pre + "norm.running_mean"), buf(pre + "norm.running_var"),
+             BN_MOMENTUM, BN_EPS, mean, invstd, scale, shift)
+    counters.append(mod.get_buffer(pre + "norm.num_batches_tracked"))
+
+
+def _act_dst(plan, l, xq_row):
+    """Where block l's BatchNorm/PReLU pass writes, in the format of the GEMM that reads it:
+    (dst, dst_lo, format, row stride, left pad, right pad) of the next block's padded operand, of
+    the QRNN input from row xq_row on, or of the output projection's fp32 operand plan.cat."""
+    C, fmt = plan.geoms[l].Cout, plan.precision.fmt
+    if l + 1 < plan.nblk:
+        nx = plan.geoms[l + 1]
+        return plan.apad[l + 1], plan.apad_lo[l + 1], fmt, C, nx.padL, nx.padR
+    if plan.rnn:
+        o = xq_row * C
+        return plan.xq[o:], None if plan.xq_lo is None else plan.xq_lo[o:], fmt, C, 0, 0
+    return plan.cat, None, gemm.FMT_F32, plan.Kc, 0, 0
+
+
+def _skip_pool(plan, l, buf):
+    """Block l's dense-skip columns of `buf` (the output projection's operand plan.cat or its
+    gradient plan.dcat); None for the last block or without dense skips."""
+    return buf[plan.col_off[l]:] if plan.skips and l + 1 < plan.nblk else None
 
 
 def _qrnn_weights(plan, params):
@@ -553,7 +598,6 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
     Tq, Kc, rows, emb = plan.Tq, plan.Kc, plan.rows, plan.emb
     plan.generation += 1
     P = lambda name: _flat(params[name])
-    buf = lambda name: _flat(mod.get_buffer(name))
     fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
 
     g0 = G[0]
@@ -568,51 +612,23 @@ def encoder_forward(plan, mod, x, params, training, save_for_backward):
     counters = [] if training else None
 
     for l, g in enumerate(G):
-        pre = "blocks.%d." % l
-        if g.sinc:
-            _sinc_weights(plan, mod, P, l, g)
-            bias = None
-        else:
-            bias = P(pre + "conv.bias")
-        if training:
-            o = plan.fs_off[l]
-            cs, cq = plan.stats_f[o:o + g.Nn], plan.stats_f[o + g.Nn:o + 2 * g.Nn]
-        else:
-            cs = cq = None
+        bias, cs, cq = _block_conv_inputs(plan, mod, P, l, g, training)
         # sinc: the band-pass operand is regenerated (and converted) every step; conv blocks:
         # pase_conv_w_batch already wrote the operand format
         plan.nt(("apad", l), plan.apad[l], g.lda, False, ("Wt", l), plan.Wt[l], g.K, g.sinc,
                 plan.y[l], g.Nn, N * g.P, g.Nn, g.K, 1.0, bias, g.P, g.T_out, g.rows_out,
                 g.fold, cs, cq, 0)
-        mean, invstd, scale, shift = plan.bn[l][0], plan.bn[l][1], plan.bn[l][2], plan.bn[l][3]
-        if training:
-            call("pase_bn_finalize", cs, cq, g.Cout, g.fold, float(N * g.T_out),
-                 P(pre + "norm.weight"), P(pre + "norm.bias"),
-                 buf(pre + "norm.running_mean"), buf(pre + "norm.running_var"),
-                 BN_MOMENTUM, BN_EPS, mean, invstd, scale, shift)
-            counters.append(mod.get_buffer(pre + "norm.num_batches_tracked"))
-        else:
-            _bn_eval_affine(plan, P, buf, l, g)
-        C = g.Cout
+        _block_bn(plan, mod, P, l, g, cs, cq, N * g.T_out, counters)
         # the producer writes the next GEMM's operand in its own format (3xTF32: + the tf32
-        # residual twin; 3xF16: the fp16 pair)
-        if l + 1 < plan.nblk:
-            nx = G[l + 1]
-            dst, dst_lo, dfmt = plan.apad[l + 1], plan.apad_lo[l + 1], fmt
-            d_ss, d_rs, pl, pr = nx.apad_floats, C, nx.padL, nx.padR
-        elif plan.rnn:
-            dst, dfmt = plan.xq[C:], fmt
-            dst_lo = None if plan.xq_lo is None else plan.xq_lo[C:]
-            d_ss, d_rs, pl, pr = (Tq + 1) * C, C, 0, 0
-        else:
-            dst, dst_lo, dfmt, d_ss, d_rs, pl, pr = plan.cat, None, gemm.FMT_F32, Tq * Kc, Kc, 0, 0
-        if plan.skips and l + 1 < plan.nblk:
-            pool, pd = plan.cat[plan.col_off[l]:], plan.pool_d[l]
-        else:
-            pool, pd = None, 0
-        call("pase_bn_prelu_pad_fwd", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, scale, shift,
-             P(pre + "act.weight"), dst, dst_lo, dfmt, d_ss, d_rs, pl, pr, pool, Tq * Kc, Kc, pd,
-             Tq)
+        # residual twin; 3xF16: the fp16 pair); each sample's QRNN input starts at its row 1,
+        # row 0 staying zero (its x_{-1})
+        C = g.Cout
+        dst, dst_lo, dfmt, d_rs, pl, pr = _act_dst(plan, l, 1)
+        d_ss = G[l + 1].apad_floats if l + 1 < plan.nblk else (Tq + 1 if plan.rnn else Tq) * d_rs
+        pool = _skip_pool(plan, l, plan.cat)
+        call("pase_bn_prelu_pad_fwd", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, plan.bn[l][2],
+             plan.bn[l][3], P("blocks.%d.act.weight" % l), dst, dst_lo, dfmt, d_ss, d_rs, pl, pr,
+             pool, Tq * Kc, Kc, 0 if pool is None else plan.pool_d[l], Tq)
 
     if plan.rnn:
         Cq, H = plan.Clast, plan.H
@@ -858,9 +874,8 @@ def _packed_front_launch(plan, mod, x, sz, tab, params, counters=None):
     call = ops.call
     G, n = plan.geoms, len(sz["Tq"])
     P = lambda name: _flat(params[name])
-    buf = lambda name: _flat(mod.get_buffer(name))
     fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
-    rows, Kc, emb = sz["rows"], plan.Kc, plan.emb
+    rows, Kc = sz["rows"], plan.Kc
 
     g0 = G[0]
     call("pase_reflect_pad_wave_var", x, tab("wave"), n, sz["max_T"], plan.apad[0],
@@ -871,40 +886,18 @@ def _packed_front_launch(plan, mod, x, sz, tab, params, counters=None):
         plan.cat[:rows * Kc].zero_()                         # the pools accumulate into it
     _conv_weight_operands(plan, P)
     for l, g in enumerate(G):
-        pre = "blocks.%d." % l
-        if g.sinc:
-            _sinc_weights(plan, mod, P, l, g)
-            bias = None
-        else:
-            bias = P(pre + "conv.bias")
-        cs = cq = None
-        if training:
-            o = plan.fs_off[l]
-            cs, cq = plan.stats_f[o:o + g.Nn], plan.stats_f[o + g.Nn:o + 2 * g.Nn]
+        bias, cs, cq = _block_conv_inputs(plan, mod, P, l, g, training)
         plan.nt_var(("apad", l), plan.apad[l], g.lda, ("Wt", l), plan.Wt[l], g.K, g.sinc,
                     plan.y[l], g.Nn, sz["gemm_rows"][l], g.Nn, g.K, bias, tab(("gemm", l)), n,
                     g.fold, cs, cq)
-        if training:
-            bn = plan.bn[l]
-            call("pase_bn_finalize", cs, cq, g.Cout, g.fold, float(sz["count"][l]),
-                 P(pre + "norm.weight"), P(pre + "norm.bias"), buf(pre + "norm.running_mean"),
-                 buf(pre + "norm.running_var"), BN_MOMENTUM, BN_EPS, bn[0], bn[1], bn[2], bn[3])
-            counters.append(mod.get_buffer(pre + "norm.num_batches_tracked"))
-        else:
-            _bn_eval_affine(plan, P, buf, l, g)
-        C, sep = g.Cout, 0
-        if l + 1 < plan.nblk:
-            nx = G[l + 1]
-            dst, dst_lo, dfmt, d_rs, pl, pr = plan.apad[l + 1], plan.apad_lo[l + 1], fmt, C, \
-                nx.padL, nx.padR
-        elif plan.rnn:
-            dst, dst_lo, dfmt, d_rs, pl, pr, sep = plan.xq, plan.xq_lo, fmt, C, 0, 0, 1
-        else:
-            dst, dst_lo, dfmt, d_rs, pl, pr = plan.cat, None, gemm.FMT_F32, Kc, 0, 0
-        pool = plan.cat[plan.col_off[l]:] if plan.skips and l + 1 < plan.nblk else None
+        _block_bn(plan, mod, P, l, g, cs, cq, sz["count"][l], counters)
+        # the QRNN input: the table's offsets leave a row ahead of each utterance, which the
+        # kernel zeroes (its x_{-1} row)
+        dst, dst_lo, dfmt, d_rs, pl, pr = _act_dst(plan, l, 0)
+        sep = 1 if plan.rnn and l + 1 == plan.nblk else 0
         call("pase_bn_prelu_pad_fwd_var", plan.y[l], ybf, tab(("bn", l)), n, sz["max_Tout"][l],
-             C, plan.bn[l][2], plan.bn[l][3], P(pre + "act.weight"), dst, dst_lo, dfmt, d_rs,
-             pl, pr, pool, Kc, sep)
+             g.Cout, plan.bn[l][2], plan.bn[l][3], P("blocks.%d.act.weight" % l), dst, dst_lo,
+             dfmt, d_rs, pl, pr, _skip_pool(plan, l, plan.cat), Kc, sep)
 
     if plan.rnn:
         Cq, H = plan.Clast, plan.H
@@ -1029,14 +1022,7 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
     the cotangent is the crop's columns of the recording's gradient (gflat unused), the QRNN
     scan carries the cell-state gradient across windows, and dx is the recording's gradient,
     into which the window's waveform gradient is added at its offset."""
-    if not param_grads and dx is None:
-        raise ValueError("encoder_backward_packed: nothing to compute (no parameter gradients, "
-                         "no dx)")
-    plan.ensure_backward()
-    if dx is not None:
-        plan.ensure_input_grad()
-    if not param_grads:
-        sink = None
+    sink, S1o, S2o = _bwd_begin(plan, params, sink, dx, param_grads, "encoder_backward_packed")
     pg = param_grads
     call = ops.call
     sec, sz = plan.layout
@@ -1045,15 +1031,8 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
     rows, Kc, emb = sz["rows"], plan.Kc, plan.emb
     P = lambda name: _flat(params[name])
     grads, copies = {}, []
-    sb = plan.stats_b
-    sb.zero_()
-    if plan.amax is not None:
-        plan.amax.zero_()
     fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
-    _dgrad_weight_operands(plan, P)
     bo = plan.bn_out
-    o = plan.bs_out
-    S1o, S2o = sb[o:o + emb], sb[o + emb:o + 2 * emb]
     use_stats = 1 if (plan.norm_out and training) else 0
     if window is not None:
         call("pase_out_bwd_gather_crop", window["gout"], window["ld"], window["col0"], rows,
@@ -1063,60 +1042,32 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
              bo[0], bo[1], plan.g, S1o, S2o)
     else:
         call("pase_out_bwd_gather_var", gflat, tab("out"), n, max(sz["Tq"]), emb, plan.g)
-    call("pase_out_bwd_apply", plan.g, plan.yout, bo[0], bo[1], bo[2], S1o, S2o, float(rows),
-         use_stats, rows, emb)
-    if pg:
-        call("pase_colsum", plan.g, emb, rows, emb, sb[plan.bs_bw:plan.bs_bw + emb])
-        plan.tn("g", plan.g, emb, rows, 0, True, "cat", plan.cat, Kc, rows, False, plan.dWcat,
-                Kc, emb, Kc, 1, rows, 1.0, 0, a_n=rows * emb)
-        _out_weight_grads(plan, G, params, sink, copies, grads)
-    call("pase_transpose_pad", plan.Wcat, Kc, plan.WcatT, emb, emb, Kc)
-    plan.nt("g", plan.g, emb, not pg, "WcatT", plan.WcatT, emb, True, plan.dcat, Kc, rows, Kc,
-            emb, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad", a_n=rows * emb)
+    _out_bwd(plan, params, sink, copies, grads, pg, S1o, S2o, use_stats, rows, rows * emb)
 
     if plan.rnn:
-        Cq, H, R = plan.Clast, plan.H, sz["xq_rows"]
+        H, R = plan.H, sz["xq_rows"]
         if window is not None:
             call("pase_qrnn_scan_bwd_carry_var", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg,
                  window["state"], window["dstate"], tab("qcarry"), 1, H)
         else:
             call("pase_qrnn_scan_bwd_var", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg,
                  tab("qbwd"), n, H)
-        if pg:
-            call("pase_colsum", plan.dYg, 3 * H, R, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
-            plan.tn("dYg", plan.dYg, 3 * H, R, 0, True, "xq", plan.xq, Cq, R, False, plan.dWq,
-                    2 * Cq, 3 * H, 2 * Cq, 1, R, 1.0, 0, a_n=R * 3 * H)
-            _qrnn_weight_grads(plan, sink, copies, grads)
-        call("pase_transpose_pad", plan.Wq, 2 * Cq, plan.WqT, 3 * H, 3 * H, 2 * Cq)
-        plan.nt("dYg", plan.dYg, 3 * H, not pg, "WqT", plan.WqT, 3 * H, True, plan.dsrc, 2 * Cq,
-                R, 2 * Cq, 3 * H, 1.0, None, R, R, R, 1, None, None, 0, akind="grad",
-                a_n=R * 3 * H)
-        top = (plan.dsrc, 0, 2 * Cq, 0, 0, plan.dsrc, 2 * Cq, 1)
-    else:
-        top = (plan.dcat, 0, Kc, 0, 0, None, 0, 0)
+        _qrnn_bwd(plan, sink, copies, grads, pg, R, (R, 0, R, 1, R), R * 3 * H)
 
     for l in range(plan.nblk - 1, -1, -1):
         g = G[l]
         C, pre, M = g.Cout, "blocks.%d." % l, sz["gemm_rows"][l]
         mean, invstd, scale, shift = plan.bn[l][0], plan.bn[l][1], plan.bn[l][2], plan.bn[l][3]
-        if l == plan.nblk - 1:
-            src = top
-        else:
-            nx = G[l + 1]
-            src = (plan.dxpad[l + 1], ybf, C, nx.padL, nx.padR, None, 0, 0)
-        pool = plan.dcat[plan.col_off[l]:] if plan.skips and l + 1 < plan.nblk else None
-        src = src + (pool, Kc)
-        amax = None if plan.amax is None else plan.amax[2 * l:2 * l + 2]
-        o = plan.bs_off[l]
+        # the table's "bwd" rows hold the sample offsets, the QRNN input's x_t columns included
+        src = _grad_src(plan, l, ybf, 0) + (_skip_pool(plan, l, plan.dcat), Kc)
+        S1, S2, dal, dbi, amax = _bn_grad_sums(plan, l)
         t, mT = tab(("bwd", l)), sz["max_Tout"][l]
-        S1, S2 = sb[o:o + C], sb[o + C:o + 2 * C]
         # eval mode: the sums feed parameter gradients only; train mode: the data gradient too
         if pg or amax is not None or training:
             call("pase_bn_prelu_bwd_reduce_var", plan.y[l], ybf, t, n, mT, C, mean, invstd,
-                 scale, shift, P(pre + "act.weight"), *src, S1, S2, sb[o + 2 * C:o + 3 * C],
-                 amax)
+                 scale, shift, P(pre + "act.weight"), *src, S1, S2, dal, amax)
         dst = (plan.dyz[l], plan.dyz_lo[l], fmt, sz["lead"][l],
-               sb[o + 3 * C:o + 4 * C] if pg and not g.sinc else None, amax, plan.gscale[l])
+               dbi if pg and not g.sinc else None, amax, plan.gscale[l])
         if training:
             call("pase_bn_prelu_bwd_apply_src_var_train", plan.y[l], ybf, t, n,
                  sz["max_span"][l], C, mean, invstd, P(pre + "norm.weight"), scale, shift,
@@ -1124,39 +1075,130 @@ def encoder_backward_packed(plan, mod, params, gflat, sink=None, dx=None, param_
         else:
             call("pase_bn_prelu_bwd_apply_src_var", plan.y[l], ybf, t, n, sz["max_span"][l], C,
                  invstd, P(pre + "norm.weight"), scale, shift, P(pre + "act.weight"), *src, *dst)
-        if g.sinc:
-            if pg:
-                plan.tn(("dyz", l), plan.dyz[l], g.Nn, M, g.dg_rows - 1, False, ("apad", l),
-                        plan.apad[l], g.lda, M, False, plan.dWt[l], g.K, g.Nn, g.K, 1, M, 1.0, 0)
-                _sinc_weight_grads(plan, mod, params, g, sink, grads)
-            if dx is not None:
-                f = g.fold
-                _sinc_dgrad_weights(plan, mod, P, g)
-                plan.nt(("dyz", l), plan.dyz[l], g.Nn, False, "Wdg", plan.Wdg, g.dg_K, True,
-                        plan.dxpad[0], f, M, f, g.dg_K, 1.0, None, M, M, M, 1, None, None, 0,
-                        akind="grad")
-                if window is not None:
-                    call("pase_reflect_fold_wave_acc", plan.dxpad[0], dx, window["seg_start"],
-                         sz["total"], g.padL, g.padR, int(window["fold_l"]),
-                         int(window["fold_r"]))
-                else:
-                    call("pase_reflect_fold_wave_var", plan.dxpad[0], tab("wave"), n,
-                         sz["max_T"], dx, g.padL, g.padR)
-        else:
-            if pg:
-                plan.tn(("dyz", l), plan.dyz[l], C, M, g.taps - 1, False, ("apad", l),
-                        plan.apad[l], g.lda, M, False, plan.dWt[l], g.K, C, g.K, 1, M, 1.0, 0)
-            if l > 0:
-                plan.nt(("dyz", l), plan.dyz[l], C, False, ("Wd", l), plan.Wd[l], g.taps * C,
-                        False, plan.dxpad[l], g.s * g.Cin, M, g.s * g.Cin, g.taps * C, 1.0, None,
-                        M, M, M, 1, None, None, 0, akind="grad")
+        # one sequence of M rows; dyz[l] leads by sz["lead"][l] frames
+        _block_grads(plan, mod, params, sink, grads, pg, l, (M, sz["lead"][l] // g.fold, M, 1, M),
+                     (M, M, M, M))
+        if g.sinc and dx is not None:
+            f = g.fold
+            _sinc_dgrad_weights(plan, mod, P, g)
+            plan.nt(("dyz", l), plan.dyz[l], g.Nn, False, "Wdg", plan.Wdg, g.dg_K, True,
+                    plan.dxpad[0], f, M, f, g.dg_K, 1.0, None, M, M, M, 1, None, None, 0,
+                    akind="grad")
+            if window is not None:
+                call("pase_reflect_fold_wave_acc", plan.dxpad[0], dx, window["seg_start"],
+                     sz["total"], g.padL, g.padR, int(window["fold_l"]), int(window["fold_r"]))
+            else:
+                call("pase_reflect_fold_wave_var", plan.dxpad[0], tab("wave"), n, sz["max_T"],
+                     dx, g.padL, g.padR)
+    return _bwd_end(plan, sink, copies, grads, pg)
 
+
+def _bwd_begin(plan, params, sink, dx, param_grads, who):
+    """The start of a backward sweep: refuse one with nothing to compute, allocate the backward
+    (and, dx given, the input-gradient) buffers, zero the reductions and re-lay out the conv
+    weights for the data-gradient GEMMs.  -> (sink, None without parameter gradients; the
+    output BatchNorm's sums S1, S2)."""
+    if not param_grads and dx is None:
+        raise ValueError("%s: nothing to compute (no parameter gradients, no dx)" % who)
+    plan.ensure_backward()
+    if dx is not None:
+        plan.ensure_input_grad()
+    sb, o, emb = plan.stats_b, plan.bs_out, plan.emb
+    sb.zero_()
+    if plan.amax is not None:
+        plan.amax.zero_()
+    _dgrad_weight_operands(plan, lambda name: _flat(params[name]))
+    return sink if param_grads else None, sb[o:o + emb], sb[o + emb:o + 2 * emb]
+
+
+def _out_bwd(plan, params, sink, copies, grads, pg, S1o, S2o, use_stats, rows, a_n):
+    """The output projection's backward from the cotangent of its `rows` frames in plan.g:
+    norm_out's backward in place (use_stats: train mode, with the sums S1o / S2o), with
+    parameter gradients (pg) the bias sum and the [W | skips] weight gradient, and the gradient
+    of plan.cat in plan.dcat.  a_n: elements of plan.g the GEMMs convert (None: all)."""
+    call, emb, Kc, bo, sb = ops.call, plan.emb, plan.Kc, plan.bn_out, plan.stats_b
+    call("pase_out_bwd_apply", plan.g, plan.yout, bo[0], bo[1], bo[2], S1o, S2o, float(rows),
+         use_stats, rows, emb)
+    if pg:
+        call("pase_colsum", plan.g, emb, rows, emb, sb[plan.bs_bw:plan.bs_bw + emb])
+        plan.tn("g", plan.g, emb, rows, 0, True, "cat", plan.cat, Kc, rows, False, plan.dWcat,
+                Kc, emb, Kc, 1, rows, 1.0, 0, a_n=a_n)
+        _out_weight_grads(plan, plan.geoms, params, sink, copies, grads)
+    call("pase_transpose_pad", plan.Wcat, Kc, plan.WcatT, emb, emb, Kc)
+    # the weight-gradient GEMM above converted g into the GEMM format; without it, this one does
+    plan.nt("g", plan.g, emb, not pg, "WcatT", plan.WcatT, emb, True, plan.dcat, Kc, rows, Kc,
+            emb, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad", a_n=a_n)
+
+
+def _qrnn_bwd(plan, sink, copies, grads, pg, M, wmap, a_n):
+    """The QRNN's backward after its scan wrote the gate gradients of M rows into plan.dYg: with
+    parameter gradients (pg) the bias sum and the gate weight gradient, whose GEMM runs over the
+    row map wmap = (pitchA, offA, pitchB, groups, rows_per_group) of dYg and the QRNN input; and
+    the gradient of the QRNN input [x_{t-1} | x_t] in plan.dsrc.  a_n as in _out_bwd."""
+    Cq, H, sb = plan.Clast, plan.H, plan.stats_b
+    if pg:
+        pA, oA, pB, groups, rpg = wmap
+        ops.call("pase_colsum", plan.dYg, 3 * H, M, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
+        plan.tn("dYg", plan.dYg, 3 * H, pA, oA, True, "xq", plan.xq, Cq, pB, False, plan.dWq,
+                2 * Cq, 3 * H, 2 * Cq, groups, rpg, 1.0, 0, a_n=a_n)
+        _qrnn_weight_grads(plan, sink, copies, grads)
+    ops.call("pase_transpose_pad", plan.Wq, 2 * Cq, plan.WqT, 3 * H, 3 * H, 2 * Cq)
+    plan.nt("dYg", plan.dYg, 3 * H, not pg, "WqT", plan.WqT, 3 * H, True, plan.dsrc, 2 * Cq,
+            M, 2 * Cq, 3 * H, 1.0, None, M, M, M, 1, None, None, 0, akind="grad", a_n=a_n)
+
+
+def _grad_src(plan, l, ybf, x_col):
+    """Block l's gradient source (A, A in bf16, A's row stride, left / right pad, B, B's row
+    stride, B's row shift): the next block's input gradient plan.dxpad[l + 1] inside its reflect
+    pads; for the last block the gradient of the QRNN input (A: its x_t columns from x_col on, B:
+    its x_{t-1} columns one row later) or of the output projection's operand, both fp32."""
+    if l + 1 < plan.nblk:
+        nx = plan.geoms[l + 1]
+        return plan.dxpad[l + 1], ybf, plan.geoms[l].Cout, nx.padL, nx.padR, None, 0, 0
+    if plan.rnn:
+        Cq = plan.Clast
+        return plan.dsrc[x_col:], 0, 2 * Cq, 0, 0, plan.dsrc, 2 * Cq, 1
+    return plan.dcat, 0, plan.Kc, 0, 0, None, 0, 0
+
+
+def _bn_grad_sums(plan, l):
+    """Block l's reductions in plan.stats_b (S1, S2, dalpha, dbias) and its 3xF16 gradient
+    maxima in plan.amax (None in the other precisions)."""
+    C, o = plan.geoms[l].Cout, plan.bs_off[l]
+    amax = None if plan.amax is None else plan.amax[2 * l:2 * l + 2]
+    return (*plan.stats_b[o:o + 4 * C].view(4, C), amax)
+
+
+def _block_grads(plan, mod, params, sink, grads, pg, l, wmap, dmap):
+    """From block l's output gradient in plan.dyz[l]: with parameter gradients (pg) its weight
+    gradient (the sinc layer: its cut-off gradients from it), and for conv blocks past the
+    first its input gradient in plan.dxpad[l].  wmap = (pitchA, offA, pitchB, groups,
+    rows_per_group): the weight-gradient GEMM's row map of dyz[l] and the padded operand; dmap
+    = (M, rows_in, t_valid, rows_out): the data-gradient GEMM's."""
+    g = plan.geoms[l]
+    if pg:
+        pA, oA, pB, groups, rpg = wmap
+        plan.tn(("dyz", l), plan.dyz[l], g.Nn, pA, oA, False, ("apad", l), plan.apad[l], g.lda,
+                pB, False, plan.dWt[l], g.K, g.Nn, g.K, groups, rpg, 1.0, 0)
+        if g.sinc:
+            _sinc_weight_grads(plan, mod, params, g, sink, grads)
+    if not g.sinc and l > 0:
+        M, rows_in, t_valid, rows_out = dmap
+        C = g.Cout
+        plan.nt(("dyz", l), plan.dyz[l], C, False, ("Wd", l), plan.Wd[l], g.taps * C, False,
+                plan.dxpad[l], g.s * g.Cin, M, g.s * g.Cin, g.taps * C, 1.0, None, rows_in,
+                t_valid, rows_out, 1, None, None, 0, akind="grad")
+
+
+def _bwd_end(plan, sink, copies, grads, pg):
+    """The end of a backward sweep: every parameter gradient written into the sink, or returned
+    (autograd); {} when there is none."""
     if not pg:
         return {}
     if sink is not None:
-        _emit_sunk_grads(plan, G, sink, copies, range(0, plan.nblk), True, "all")
+        _emit_sunk_grads(plan, plan.geoms, sink, copies, range(0, plan.nblk), True, "all")
         return {}
-    return _autograd_grads(plan, G, grads)
+    return _autograd_grads(plan, plan.geoms, grads)
 
 
 def _grad_sink(mod, names):
@@ -1626,64 +1668,27 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
     conv weight gradients by the batched re-layout, the sinc cut-offs by pase_sinc_grad,
     everything else by one batched strided copy -- and {} is returned: no per-parameter
     clones, no autograd accumulation kernels, no packing before the all-reduce."""
-    if not param_grads and dx is None:
-        raise ValueError("encoder_backward_steps: nothing to compute (no parameter gradients, "
-                         "no dx)")
-    plan.ensure_backward()
-    if dx is not None:
-        plan.ensure_input_grad()
-    if not param_grads:
-        sink = None
+    sink, S1o, S2o = _bwd_begin(plan, params, sink, dx, param_grads, "encoder_backward_steps")
     pg = param_grads
     call = ops.call
     G, N = plan.geoms, plan.N
     Tq, Kc, rows, emb = plan.Tq, plan.Kc, plan.rows, plan.emb
     P = lambda name: _flat(params[name])
     grads = {}
-    sb = plan.stats_b
-    sb.zero_()
-    if plan.amax is not None:
-        plan.amax.zero_()
+    copies = []          # sink mode: (src tensor view, rows, cols, src_ld, destination name)
     fmt, ybf = plan.precision.fmt, int(plan.precision.act_bf16)
-    _dgrad_weight_operands(plan, P)
     zeros = plan.zeros64
     bo = plan.bn_out
-    o = plan.bs_out
-    S1o, S2o = sb[o:o + emb], sb[o + emb:o + 2 * emb]
     call("pase_out_bwd_reduce", None if gout is None else gout.reshape(-1),
          None if gntc is None else gntc.reshape(-1), plan.yout, bo[0], bo[1], N, Tq, emb,
          plan.g, S1o, S2o)
     use_stats = 1 if (plan.norm_out and training) else 0
-    call("pase_out_bwd_apply", plan.g, plan.yout, bo[0], bo[1], bo[2], S1o, S2o, float(rows),
-         use_stats, rows, emb)
-    if pg:
-        call("pase_colsum", plan.g, emb, rows, emb, sb[plan.bs_bw:plan.bs_bw + emb])
-        plan.tn("g", plan.g, emb, rows, 0, True, "cat", plan.cat, Kc, rows, False, plan.dWcat,
-                Kc, emb, Kc, 1, rows, 1.0, 0)
-    call("pase_transpose_pad", plan.Wcat, Kc, plan.WcatT, emb, emb, Kc)
-    # the weight-gradient GEMM above converted g into the GEMM format; without it, this one does
-    plan.nt("g", plan.g, emb, not pg, "WcatT", plan.WcatT, emb, True, plan.dcat, Kc, rows, Kc,
-            emb, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad")
-    copies = []          # sink mode: (src tensor view, rows, cols, src_ld, destination name)
-    if pg:
-        _out_weight_grads(plan, G, params, sink, copies, grads)
+    _out_bwd(plan, params, sink, copies, grads, pg, S1o, S2o, use_stats, rows, None)
 
-    Cl = plan.Clast
     if plan.rnn:
-        Cq, H = Cl, plan.H
-        call("pase_qrnn_scan_bwd", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg, N, Tq, H)
-        if pg:
-            call("pase_colsum", plan.dYg, 3 * H, rows, 3 * H, sb[plan.bs_bq:plan.bs_bq + 3 * H])
-            plan.tn("dYg", plan.dYg, 3 * H, Tq, 0, True, "xq", plan.xq, Cq, Tq + 1, False,
-                    plan.dWq, 2 * Cq, 3 * H, 2 * Cq, N, Tq, 1.0, 0)
-            _qrnn_weight_grads(plan, sink, copies, grads)
-        call("pase_transpose_pad", plan.Wq, 2 * Cq, plan.WqT, 3 * H, 3 * H, 2 * Cq)
-        plan.nt("dYg", plan.dYg, 3 * H, not pg, "WqT", plan.WqT, 3 * H, True, plan.dsrc, 2 * Cq,
-                rows, 2 * Cq, 3 * H, 1.0, None, rows, rows, rows, 1, None, None, 0, akind="grad")
-        last_src = dict(A=plan.dsrc[Cq:], a_ss=Tq * 2 * Cq, a_rs=2 * Cq,
-                        B=plan.dsrc, b_ss=Tq * 2 * Cq, b_rs=2 * Cq, b_shift=1)
-    else:
-        last_src = dict(A=plan.dcat, a_ss=Tq * Kc, a_rs=Kc, B=None, b_ss=0, b_rs=0, b_shift=0)
+        call("pase_qrnn_scan_bwd", plan.Yg, plan.Cst, plan.dcat, Kc, plan.dYg, N, Tq, plan.H)
+        # the weight-gradient GEMM: N samples of Tq gate rows against Tq + 1 input rows
+        _qrnn_bwd(plan, sink, copies, grads, pg, rows, (Tq, 0, Tq + 1, N, Tq), None)
 
     if split is not None and (sink is None or not (0 < split < plan.nblk)):
         raise ValueError("encoder_backward_steps: split needs sink mode and 0 < split < nblk")
@@ -1698,29 +1703,21 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
         C = g.Cout
         pre = "blocks.%d." % l
         mean, invstd, scale, shift = plan.bn[l][0], plan.bn[l][1], plan.bn[l][2], plan.bn[l][3]
-        if l == plan.nblk - 1:
-            s = dict(last_src)
-            s.update(padL=0, padR=0, a_bf16=0)          # dsrc / dcat are fp32 in every mode
-        else:
-            nx = G[l + 1]
-            s = dict(A=plan.dxpad[l + 1], a_ss=nx.apad_floats, a_rs=C, padL=nx.padL,
-                     padR=nx.padR, B=None, b_ss=0, b_rs=0, b_shift=0, a_bf16=ybf)
-        if plan.skips and l + 1 < plan.nblk:
-            pool, pd = plan.dcat[plan.col_off[l]:], plan.pool_d[l]
-        else:
-            pool, pd = None, 0
-        doff = 0 if g.sinc else (g.taps - 1) * C
-        d_ss = g.Ty * C if g.sinc else g.Pd * C
-        dst = plan.dyz[l][doff:]
-        dst_lo = None if plan.dyz_lo[l] is None else plan.dyz_lo[l][doff:]
-        amax = None if plan.amax is None else plan.amax[2 * l:2 * l + 2]
-        o = plan.bs_off[l]
-        S1, S2, dal, dbi = sb[o:o + C], sb[o + C:o + 2 * C], sb[o + 2 * C:o + 3 * C], \
-            sb[o + 3 * C:o + 4 * C]
+        # per sample: the last block's sources (dsrc / dcat) hold Tq rows
+        A, a_bf16, a_rs, padL, padR, B, b_rs, b_shift = _grad_src(plan, l, ybf, plan.Clast)
+        a_ss = G[l + 1].apad_floats if l + 1 < plan.nblk else Tq * a_rs
+        pool = _skip_pool(plan, l, plan.dcat)
+        pd = 0 if pool is None else plan.pool_d[l]
+        # dyz[l] per sample: `pitch` rows, the first `lead` of them zero
+        lead, pitch = (0, g.rows_out) if g.sinc else (g.taps - 1, g.Pd)
+        d_ss = pitch * g.Nn
+        dst = plan.dyz[l][lead * C:]
+        dst_lo = None if plan.dyz_lo[l] is None else plan.dyz_lo[l][lead * C:]
+        S1, S2, dal, dbi, amax = _bn_grad_sums(plan, l)
         # pass 1 writes only its sums; pass 2 recomputes du = PReLU'(u) g from the same
         # gradient sources (no du tensor: one activation-sized write + read less per block)
-        src = (s["A"], s["a_bf16"], s["a_ss"], s["a_rs"], s["padL"], s["padR"],
-               s["B"], s["b_ss"], s["b_rs"], s["b_shift"], pool, Tq * Kc, Kc, pd, Tq)
+        src = (A, a_bf16, a_ss, a_rs, padL, padR, B, Tq * b_rs, b_rs, b_shift, pool, Tq * Kc, Kc,
+               pd, Tq)
         call("pase_bn_prelu_bwd_reduce", plan.y[l], ybf, g.Ty * C, N, g.T_out, C, mean, invstd,
              scale, shift, P(pre + "act.weight"), *src, None, d_ss, S1, S2, dal, amax)
         if training:
@@ -1731,31 +1728,15 @@ def encoder_backward_steps(plan, mod, params, gout, gntc, training, sink=None, s
              P(pre + "norm.weight"), scale, shift, P(pre + "act.weight"), a1, a2,
              float(N * g.T_out), *src, dst, dst_lo, fmt, d_ss, None if g.sinc else dbi, amax,
              plan.gscale[l])
-        if g.sinc and pg:
-            plan.tn(("dyz", l), plan.dyz[l], g.Nn, g.rows_out, 0, False, ("apad", l), plan.apad[l],
-                    g.lda, g.P, False, plan.dWt[l], g.K, g.Nn, g.K, N, g.rows_out, 1.0, 0)
-            _sinc_weight_grads(plan, mod, params, g, sink, grads)
-        elif not g.sinc:
-            if pg:
-                plan.tn(("dyz", l), plan.dyz[l], C, g.Pd, g.taps - 1, False, ("apad", l),
-                        plan.apad[l], g.lda, g.P, False, plan.dWt[l], g.K, C, g.K, N, g.T_out,
-                        1.0, 0)
-            if l > 0:
-                plan.nt(("dyz", l), plan.dyz[l], C, False, ("Wd", l), plan.Wd[l], g.taps * C, False,
-                        plan.dxpad[l], g.s * g.Cin, N * g.Pd, g.s * g.Cin, g.taps * C, 1.0, None,
-                        g.Pd, g.P, g.P, 1, None, None, 0, akind="grad")
+        _block_grads(plan, mod, params, sink, grads, pg, l, (pitch, lead, g.P, N, g.rows_out),
+                     (N * g.Pd, g.Pd, g.P, g.P))
         if g.sinc and dx is not None:
             _sinc_input_grad(plan, mod, P, g, dx)
 
-    if not pg:
+    if split is not None:
+        _emit_sunk_grads(plan, G, sink, copies, range(0, split), False, "lo")
         return {}
-    if sink is not None:
-        if split is not None:
-            _emit_sunk_grads(plan, G, sink, copies, range(0, split), False, "lo")
-        else:
-            _emit_sunk_grads(plan, G, sink, copies, range(0, plan.nblk), True, "all")
-        return {}
-    return _autograd_grads(plan, G, grads)
+    return _bwd_end(plan, sink, copies, grads, pg)
 
 
 def _out_weight_grads(plan, G, params, sink, copies, grads):
