@@ -41,5 +41,5 @@ def test_product_never_imports_oracle():
         for f in files:
             if f.endswith(".py"):
                 src = open(os.path.join(dirpath, f)).read()
-                assert not re.search(r"^\s*(import|from)\s+(pase_oracle|ref_harness|oracle|emul_ops)",
+                assert not re.search(r"^\s*(import|from)\s+(pase_oracle|ref_harness|oracle|emul)",
                                      src, re.M), f

@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-import emul_batch
+import emul
 from batch_corpus import CASES, HOP, KEYS, SPLIT, T, UTTS, build_corpus, digest
 from distortion_banks import build_banks, case_cfg
 from helpers import GOLDEN
@@ -147,7 +147,7 @@ def _check_batch(out, want, case, dist_chunk=None):
 
 @pytest.mark.parametrize("case", list(CASES))
 def test_emulated_pipeline_matches_golden_hashes(case, corpus, golden, monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_batch.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     meta = _meta(golden, case)
     b = _batcher(corpus, case)
     _seed(CASES[case]["seed"])
@@ -157,14 +157,14 @@ def test_emulated_pipeline_matches_golden_hashes(case, corpus, golden, monkeypat
 
 
 def test_silent_chunk_scales_to_nan(corpus, monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_batch.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     b = _batcher(corpus, "single_short")
     out = b([9])
     assert bool(torch.isnan(out["chunk"]).all()) and bool(torch.isnan(out["cchunk"]).all())
 
 
 def test_short_utterance_is_reflect_padded(corpus, monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_batch.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     wavs = _pool(corpus)
     b = DeviceBatcher(wavs, T, mi=False)
     out = b([4])

@@ -28,7 +28,7 @@ away from the kink, so an fp32 rounding cannot flip a gate."""
 import pytest
 import torch
 
-import emul_ops            # bit-level operand formats only (tf32 residual, fp16 gradient scale)
+import emul            # bit-level operand formats only (tf32 residual, fp16 gradient scale)
 from pase_b200 import _lib
 from pase_b200 import encoder as E
 
@@ -280,9 +280,9 @@ def _check_bwd(b, r):
         if b.lo_buf is not None:
             _untouched("dst_lo", b.lo_buf, shape, strides, b.doff)
             d, lo = hi.contiguous(), _view(b.out(b.lo_buf), shape, strides).contiguous()
-            rec = emul_ops._tf32_trunc(d) + lo
+            rec = emul.core._tf32_trunc(d) + lo
             _within("trunc_tf32(dst) + dst_lo", rec, d.double(), 2.0 ** -21 * d.double().abs())
-            assert torch.equal(lo, emul_ops._residual(d)), "dst_lo != residual(dst)"
+            assert torch.equal(lo, emul.core._residual(d)), "dst_lo != residual(dst)"
     elif b.fmt == 1:
         _within("dy (bf16)", hi, dy, _ulp(dy, 7) + 2.0 ** -20 * bound)
     else:
@@ -292,7 +292,7 @@ def _check_bwd(b, r):
         s1 = (b.S1in * (1.0 / M)).float().abs()
         s2 = (b.S2in * (1.0 / M)).float().abs()
         bnd = float((g32 * (b.amax[0] + s1 + b.amax[1] * s2)).max())
-        s = emul_ops.f16_grad_scale(bnd * 1.0001)
+        s = emul.core.f16_grad_scale(bnd * 1.0001)
         assert b.scale_out.tolist() == [1.0 / s, s], (b.scale_out.tolist(), s)
         v = hi.double() + _view(b.out(b.lo_buf), shape, strides).double() / 2048.0
         assert float(v.abs().max()) <= 16384.0
@@ -493,9 +493,9 @@ class Fwd(object):
                 _untouched("dst_lo", self.lo_buf, shape, strides, self.doff)
                 d = hi.contiguous()
                 lo = _view(self.lo_buf[self.doff:], shape, strides).contiguous()
-                rec = emul_ops._tf32_trunc(d) + lo
+                rec = emul.core._tf32_trunc(d) + lo
                 _within("trunc_tf32(dst) + dst_lo", rec, d.double(), 2.0 ** -21 * d.double().abs())
-                assert torch.equal(lo, emul_ops._residual(d)), "dst_lo != residual(dst)"
+                assert torch.equal(lo, emul.core._residual(d)), "dst_lo != residual(dst)"
         elif self.fmt == 1:
             _within("a (bf16)", hi, ref, _ulp(ref, 7))
         else:

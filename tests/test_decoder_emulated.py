@@ -1,12 +1,12 @@
 """The cchunk decoder's host logic (geometry, padded-row plan, polyphase weight layout, crop
-offsets, row maps of the three GEMMs) on the CPU, with the kernels emulated (tests/emul_ops.py):
+offsets, row maps of the three GEMMs) on the CPU, with the kernels emulated (tests/emul/):
 end to end against float64 conv_transpose1d + PReLU, and stage by stage through the checks and
 bounds of tests/test_decoder_gpu.py, at the geometries that file runs on the GPU."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-import emul_ops
+import emul
 import pase_b200.ops as ops
 from pase_b200 import functional as Fn
 from pase_b200.decoder import decoder_stack, _LayerGeom
@@ -20,7 +20,7 @@ CASES["workers+"] = (256, WPLUS["fmaps"], WPLUS["strides"], WPLUS["kwidths"], 2,
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_ops.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     monkeypatch.setattr(Fn, "PRECISION", Fn.PRECISION)       # restored after the test
 
 

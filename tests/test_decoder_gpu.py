@@ -50,7 +50,7 @@ import math
 import pytest
 import torch
 
-import emul_ops
+import emul
 from pase_b200 import gemm
 from pase_b200 import functional as Fn
 from pase_b200.decoder import decoder_stack
@@ -142,7 +142,7 @@ def _read(p, tc, x):
     """float64 value of an fp32 operand as the kernel multiplies it (single-pass modes round;
     the fp32-equivalent ones are compared against the fp32 value itself)."""
     if tc and p.name == "tf32":
-        return emul_ops._tf32_trunc(x.float()).double()
+        return emul.core._tf32_trunc(x.float()).double()
     if tc and p.name == "bf16":
         return x.float().to(torch.bfloat16).double()
     return x.double()
@@ -172,7 +172,7 @@ def _gemm_tol(p, tc, K, S, fa=None, fb=None):
 
 
 def f16_scale(dy, n):
-    return emul_ops.f16_grad_scale(float(dy[:n].abs().max()) * 1.0001)
+    return emul.core.f16_grad_scale(float(dy[:n].abs().max()) * 1.0001)
 
 
 # ---- float64 reference of one layer's polyphase GEMMs, from W by index arithmetic ----

@@ -15,7 +15,7 @@ import pytest
 import torch
 
 import distortions_oracle as DO
-import emul_distort
+import emul
 from distortion_banks import (CASES, FULL_CASES, build_banks, case_cfg, golden_view, make_chunk,
                               raw_banks)
 from helpers import GOLDEN
@@ -150,7 +150,7 @@ def test_cases_cover_the_bank_edges(banks):
 @pytest.mark.parametrize("name", ["reverb_4097", "overlap_reverb", "noise", "clip", "bandrop",
                                   "downsample", "pase_plus"])
 def test_emulated_pipeline_matches_oracle(name, banks, monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_distort.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     paths, raw = banks
     cfg, B, T, d, seed = case_cfg(name, paths)
     dist = config_distortions(device="cpu", **cfg)
@@ -166,7 +166,7 @@ def test_emulated_pipeline_matches_oracle(name, banks, monkeypatch):
 
 
 def test_call_writes_chunk_and_overlap(banks, monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_distort.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     paths, _ = banks
     cfg, B, T, d, seed = case_cfg("overlap", paths)
     dist = config_distortions(device="cpu", **cfg)

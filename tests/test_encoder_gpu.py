@@ -263,9 +263,9 @@ def test_tf32_mode_is_l2_equivalent():
 
 def _emulated_bf16_reference(cfg, seed, training, x, cot):
     """The SAME host orchestration with every kernel replaced by its torch spec
-    (tests/emul_ops.py) on CPU: a bf16-exact restatement (same rounding points, products of
+    (tests/emul/) on CPU: a bf16-exact restatement (same rounding points, products of
     the rounded operands accumulated in fp64)."""
-    import emul_ops
+    import emul
     import pase_b200.ops as ops
     from pase_b200 import encoder as enc
     m = WaveFe(**cfg)
@@ -273,7 +273,7 @@ def _emulated_bf16_reference(cfg, seed, training, x, cot):
     m.precision = "bf16"
     m.train(training)
     real = ops.call
-    ops.call = emul_ops.call
+    ops.call = emul.call
     try:
         m._sinc_consts(x.device)
         plan = m._plan(x.shape[0], x.shape[2], x.device)

@@ -3,7 +3,7 @@ eager pass equals what the unmodified reference computed (tests/golden/eval.pt, 
 tests/golden/make_eval_golden.py), the fused regression head under ``no_grad`` takes no
 residual buffer, the loss-only form of the fused epilogue's spec gives the loss of the full
 form, and GraphedEvalStep refuses what it cannot run.  CUDA kernels are replaced by their torch
-specs (tests/emul_ops.py, tests/emul_spc.py, tests/emul_eval.py); tests/test_eval_step_gpu.py
+specs (tests/emul/); tests/test_eval_step_gpu.py
 covers the kernels.
 """
 import copy
@@ -14,8 +14,7 @@ import random
 import pytest
 import torch
 
-import emul_eval
-import emul_ops
+import emul
 from helpers import GOLDEN, resolve_cfg, seeded_randn
 from pase_b200 import encoder as enc
 from pase_b200 import functional as Fn
@@ -29,7 +28,7 @@ from test_train_step import _cpu_batcher, build_corpus, make_model
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_eval.call)
+    monkeypatch.setattr(ops, "call", emul.call)
 
     def encode_cpu(self, x):
         self._sinc_consts(x.device)
@@ -105,7 +104,7 @@ def _fused_operands(seed=3):
 
 
 def test_fused_head_without_grad_takes_no_residual_buffer(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_eval.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     h, w, b, label, F, r = _fused_operands()
     prev = Fn.PRECISION
     Fn.set_precision("3xf16")
@@ -136,17 +135,17 @@ def test_emulated_loss_only_spec_equals_the_full_spec():
     ldr = 128
     hi, lo = torch.zeros(rows * K, dtype=torch.float16), torch.zeros(rows * K, dtype=torch.float16)
     whi, wlo = torch.zeros(N * K, dtype=torch.float16), torch.zeros(N * K, dtype=torch.float16)
-    emul_ops.call("pase_split_f16", h.reshape(-1), hi, lo, rows * K, None, None)
-    emul_ops.call("pase_split_f16", w.reshape(-1), whi, wlo, N * K, None, None)
+    emul.call("pase_split_f16", h.reshape(-1), hi, lo, rows * K, None, None)
+    emul.call("pase_split_f16", w.reshape(-1), whi, wlo, N * K, None, None)
     scale = torch.tensor([1.0 / 64, 64.0])
     full = torch.zeros(1, dtype=torch.float64)
     db = torch.zeros(N, dtype=torch.float64)
     rh, rl = (torch.zeros(rows * ldr, dtype=torch.float16) for _ in range(2))
     common = (hi, lo, rows, K, whi, wlo, K)
     tail = (rows, N, K, b, label.reshape(-1), label.shape[0], F, label.shape[2], r)
-    emul_ops.call("pase_tc_gemm_nt_ctxmse", *common, rh, rl, ldr, *tail, scale, full, db)
+    emul.call("pase_tc_gemm_nt_ctxmse", *common, rh, rl, ldr, *tail, scale, full, db)
     only = torch.zeros(1, dtype=torch.float64)
-    emul_eval.call("pase_tc_gemm_nt_ctxmse", *common, None, None, ldr, *tail, None, only, None)
+    emul.call("pase_tc_gemm_nt_ctxmse", *common, None, None, ldr, *tail, None, only, None)
     assert float(full) > 0 and torch.equal(only, full)
 
 

@@ -1,12 +1,11 @@
 """Host side of WaveFe.extract (packed variable-length inference) on CPU, every kernel launch
-replaced by its torch emulation (tests/emul_extract.py): the planner's offsets and table, the
+replaced by its torch emulation (tests/emul/): the planner's offsets and table, the
 packed forward against the eval goldens and the per-utterance forward, capacity splitting,
 the 32-bit index guard and a launch count independent of the number of utterances."""
 import pytest
 import torch
 
-import emul_extract
-import emul_ops
+import emul
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, assert_close
 import pase_b200.ops as ops
 from pase_b200 import encoder as enc
@@ -15,7 +14,7 @@ from pase_b200.frontend import EXTRACT_MAX_SAMPLES, WaveFe
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_extract.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     yield
 
 
@@ -126,7 +125,7 @@ def test_launches_independent_of_utterance_count(emulated, monkeypatch):
         wavs = [seeded_randn((471 + 37 * i,), i, 0.5) for i in range(n)]
         calls = []
         monkeypatch.setattr(ops, "call", lambda name, *a: (calls.append(name),
-                                                           emul_extract.call(name, *a))[1])
+                                                           emul.call(name, *a))[1])
         model._extract(wavs, "avg_concat", None, torch.device("cpu"))
         counts.append(calls)
     assert counts[0] == counts[1]

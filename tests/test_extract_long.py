@@ -1,5 +1,5 @@
 """Host side of WaveFe.extract_long / FeatureStream (windowed inference of one long recording)
-on CPU, every kernel launch replaced by its torch emulation (tests/emul_streams.py): the window
+on CPU, every kernel launch replaced by its torch emulation (tests/emul/): the window
 planner, the halos it derives against the float64 oracle, the windowed forward against the
 B=1 forward, the stream against extract_long, and argument errors raised before any launch."""
 import random
@@ -8,7 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import emul_streams
+import emul
 import pase_oracle as O
 from helpers import resolve_cfg, fill_state_dict, seeded_randn, assert_close
 import pase_b200.ops as ops
@@ -21,7 +21,7 @@ CPU = torch.device("cpu")
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_streams.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     yield
 
 

@@ -5,7 +5,7 @@ import copy
 import pytest
 import torch
 
-import emul_ops
+import emul
 import pase_b200.ops as ops
 from pase_b200.optim import FlatAdam
 
@@ -65,12 +65,12 @@ def _run(device, monkeypatch=None):
 
 
 def test_flat_adam_matches_torch_adam_emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_ops.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     nat, opt, x = _run("cpu")
     # facades: the reference scheduler's calling pattern (zero_grad per optimizer, backward,
     # step per optimizer) launches exactly once per iteration
     calls = []
-    real = emul_ops.call
+    real = emul.call
     monkeypatch.setattr(ops, "call", lambda name, *a: (calls.append(name), real(name, *a))[1])
     views = opt.views()
     before = [p.detach().clone() for p in nat.parameters()]

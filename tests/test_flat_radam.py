@@ -2,7 +2,7 @@
 written by tests/golden/make_radam_golden.py): the golden trajectories with Adam and RAdam
 groups in one engine, the state dict in the reference RAdam's format both ways, the per-group
 facades and Saver files, and the algorithm check.  CPU, with the emulated kernel
-(tests/emul_radam.py); tests/test_flat_radam_gpu.py runs the same checks on the CUDA kernel.
+(tests/emul/optim.py); tests/test_flat_radam_gpu.py runs the same checks on the CUDA kernel.
 
 Tolerance (TOL, as for Adam in tests/test_flat_adam.py): the segment table holds lr and the
 betas in fp32, where the reference uses Python floats.  The step size then differs by a few
@@ -17,7 +17,7 @@ import os
 import pytest
 import torch
 
-import emul_radam
+import emul
 import pase_b200.ops as ops
 from pase_b200 import Saver
 from pase_b200.optim import FlatAdam
@@ -237,7 +237,7 @@ def saver_interchange(device, tmp_path):
 
 @pytest.fixture
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_radam.call)
+    monkeypatch.setattr(ops, "call", emul.call)
 
 
 def test_golden_trajectories_mixed_engine_emulated(emulated):
@@ -258,7 +258,7 @@ def test_algorithm_in_segment_table_emulated(emulated):
     import struct
     gd = gold()
     engine, _ = setup(gd, "cpu")
-    codes = lambda: [struct.unpack_from(emul_radam.ROW, engine._segments().numpy().tobytes(),
+    codes = lambda: [struct.unpack_from(emul.optim.ROW, engine._segments().numpy().tobytes(),
                                         48 * i)[7] for i in range(len(engine.param_groups))]
     assert codes() == [0.0] + [1.0] * n_inst(gd)
     engine.param_groups[1]["algorithm"] = "adam"

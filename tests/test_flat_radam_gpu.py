@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 import torch
 
-import emul_radam
+import emul
 from test_flat_radam import run_golden, saver_interchange, state_roundtrip
 from pase_b200 import ops
 from pase_b200.optim import FlatAdam
@@ -47,7 +47,7 @@ def layout(algos):
 
 
 def table(rows, device="cuda"):
-    raw = b"".join(struct.pack(emul_radam.ROW, r["start"], r["end"], r["lr"], r["b1"], r["b2"],
+    raw = b"".join(struct.pack(emul.optim.ROW, r["start"], r["end"], r["lr"], r["b1"], r["b2"],
                                r["eps"], r["wd"], r["algo"], r["si"]) for r in rows)
     return torch.frombuffer(bytearray(raw), dtype=torch.int64).to(device)
 
@@ -78,7 +78,7 @@ def restate(rows, p, g, m, v, steps, grad_scale=1.0):
             denom = v[a:b].sqrt() / (1 - b2 ** t) ** 0.5 + eps
             p[a:b] -= lr / (1 - b1 ** t) * m[a:b] / denom
             continue
-        rect, step, decay = emul_radam.radam_constants(lr, b1, b2, wd, t)
+        rect, step, decay = emul.optim.radam_constants(lr, b1, b2, wd, t)
         p[a:b] += decay * p[a:b]
         p[a:b] -= step * (m[a:b] / (v[a:b].sqrt() + eps) if rect else m[a:b])
     return p, m, v

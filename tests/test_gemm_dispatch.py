@@ -1,5 +1,5 @@
 """pase_b200.gemm on the CPU: the tensor-core eligibility rule against the preconditions of the
-tensor-core entry points (tests/emul_ops.py asserts the PASE_CHECK_ARG checks of
+tensor-core entry points (tests/emul/core.py asserts the PASE_CHECK_ARG checks of
 csrc/gemm_tc.cu), the kernel each dispatcher picks, and the refusal of operands that exist only
 in a 16-bit format when the shape is outside the tensor-core path."""
 import itertools
@@ -7,7 +7,7 @@ import itertools
 import pytest
 import torch
 
-import emul_ops
+import emul
 import pase_b200.ops as ops
 from pase_b200 import gemm
 
@@ -20,14 +20,14 @@ def launches(monkeypatch):
 
     def record(name, *a):
         names.append(name)
-        return emul_ops.call(name, *a)
+        return emul.call(name, *a)
     monkeypatch.setattr(ops, "call", record)
     return names
 
 
 def _accepts(name, *args):
     try:
-        emul_ops.call(name, *args)
+        emul.call(name, *args)
     except AssertionError:
         return False
     return True

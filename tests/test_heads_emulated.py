@@ -5,7 +5,7 @@ import random
 import pytest
 import torch
 
-import emul_ops
+import emul
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, assert_close, \
     check_grads
 import pase_b200.ops as ops
@@ -17,7 +17,7 @@ from pase_b200.utils import parse_workers
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_ops.call)
+    monkeypatch.setattr(ops, "call", emul.call)
 
     def encode_cpu(self, x):
         self._sinc_consts(x.device)

@@ -175,9 +175,9 @@ def test_workers_plus_full_length_against_oracle(precision):
 def test_fused_regression_heads_gpu():
     """pase.fuse_regression_loss on the GPU (3xF16): the contextualised-MSE epilogue of the
     output GEMM gives the same losses and gradients as the unfused heads at T=32000, and the
-    fused GEMM kernel matches its spec (tests/emul_ops.py) on a ragged shape."""
+    fused GEMM kernel matches its spec (tests/emul/heads.py) on a ragged shape."""
     import copy
-    import emul_ops
+    import emul
     from pase_b200 import _lib
     from helpers import resolve_cfg, fill_state_dict, rel_l2
     from pase_b200.pase import pase as native_pase, total_loss
@@ -200,7 +200,7 @@ def test_fused_regression_heads_gpu():
             torch.zeros(1, dtype=torch.float64), torch.zeros(ldr, dtype=torch.float64)]
     cpu = [a.clone() if isinstance(a, torch.Tensor) else a for a in args]
     dev = [a.cuda() if isinstance(a, torch.Tensor) else a for a in args]
-    emul_ops.call("pase_tc_gemm_nt_ctxmse", *cpu)
+    emul.call("pase_tc_gemm_nt_ctxmse", *cpu)
     _lib.call("pase_tc_gemm_nt_ctxmse", *dev)
     torch.cuda.synchronize()
     vc = cpu[7].float() + cpu[8].float() / 2048.0

@@ -1,11 +1,11 @@
 """Host-side orchestration of pase_b200 (geometry, buffer plan, padding / folding index
 math, gradient routing) checked on CPU against the reference's golden vectors, with every
-kernel launch replaced by its torch emulation (tests/emul_ops.py).  This does NOT exercise
+kernel launch replaced by its torch emulation (tests/emul/).  This does NOT exercise
 the CUDA kernels -- the `-m gpu` tests do -- it proves the decomposition is exact."""
 import pytest
 import torch
 
-import emul_ops
+import emul
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, assert_close, \
     check_grads
 import pase_b200.ops as ops
@@ -15,7 +15,7 @@ from pase_b200.frontend import WaveFe
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_ops.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     yield
 
 
@@ -142,7 +142,7 @@ def test_weight_batch_table_is_cached_and_rebuilt(emulated, monkeypatch):
     model.train(True)
     x = seeded_randn((meta["N"], 1, meta["T"]), meta["seed"] + 1, 0.5)
     seen = []
-    real = emul_ops.call
+    real = emul.call
 
     def spy(name, *a):
         if name == "pase_conv_w_batch":

@@ -1,11 +1,11 @@
 """The waveform gradient of WaveFe (DESIGN.md section 17) on the CPU with emulated kernels
-(tests/emul_input_grad.py): the host-side routing, the sinc layer's haloed / banded polyphase
+(tests/emul/): the host-side routing, the sinc layer's haloed / banded polyphase
 GEMM formulation and the reflect fold-back against float64 autograd through the oracle, and the
 launches of the data-gradient-only sweep of a frozen encoder."""
 import pytest
 import torch
 
-import emul_input_grad
+import emul
 import pase_oracle as O
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, rel_l2
 import pase_b200.ops as ops
@@ -15,7 +15,7 @@ from pase_b200.frontend import WaveFe
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_input_grad.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     yield
 
 
@@ -138,7 +138,7 @@ def _record(monkeypatch, plan_of):
         plan = plan_of()
         owned = {t.untyped_storage().data_ptr() for t in plan.tensors()} if plan else set()
         seen.append((name, tuple(norm(a, owned) for a in args)))
-        return emul_input_grad.call(name, *args)
+        return emul.call(name, *args)
     monkeypatch.setattr(ops, "call", spy)
     return seen
 

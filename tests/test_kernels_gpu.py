@@ -1,9 +1,9 @@
 """Every C-ABI kernel, called through ctypes on the GPU, against its torch
-semantic spec (tests/emul_ops.py) on identical random inputs."""
+semantic spec (tests/emul/) on identical random inputs."""
 import pytest
 import torch
 
-import emul_ops
+import emul
 from pase_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -14,7 +14,7 @@ def run_both(name, args, rtol=1e-4, atol=1e-5, cmp_scale=None, skip=()):
     CUDA kernel on device copies; compares every tensor argument afterwards."""
     cpu = [a.clone() if isinstance(a, torch.Tensor) else a for a in args]
     dev = [a.cuda() if isinstance(a, torch.Tensor) else a for a in args]
-    emul_ops.call(name, *cpu)
+    emul.call(name, *cpu)
     _lib.call(name, *dev)
     torch.cuda.synchronize()
     for i, (c, d) in enumerate(zip(cpu, dev)):
@@ -192,7 +192,7 @@ def test_scatter_copy(njobs):
         return torch.tensor([[s.data_ptr() + 4 * so_, d.data_ptr() + 4 * do_, r, c, sl, dl]
                              for (r, c, sl, dl), so_, do_ in zip(shapes, s_off, d_off)],
                             dtype=torch.int64).reshape(-1)
-    emul_ops.pase_scatter_copy(table(src, ref), njobs, total)
+    emul.core.pase_scatter_copy(table(src, ref), njobs, total)
     _lib.call("pase_scatter_copy", table(srcd, dstd).cuda(), njobs, total)
     torch.cuda.synchronize()
     out = dstd.cpu()
@@ -278,9 +278,9 @@ def test_bn_prelu_pad_fwd(N, T, C, padL, padR, pool_d, with_lo):
         # the residual is a discontinuous function of the last bits of dst, so it is checked
         # against the GPU's own dst: trunc_tf32(dst) + lo == dst to 2^-21
         d, lo = dev[9].cpu(), dev[10].cpu()
-        rec = emul_ops._tf32_trunc(d) + lo
+        rec = emul.core._tf32_trunc(d) + lo
         assert float((rec - d).abs().max()) <= float(d.abs().max()) * 2.0 ** -21
-        assert torch.equal(lo, emul_ops._residual(d))
+        assert torch.equal(lo, emul.core._residual(d))
 
 
 @pytest.mark.parametrize("y_bf16,fmt", [(1, 1), (0, 2), (1, 0), (0, 1)])
@@ -305,7 +305,7 @@ def test_bn_prelu_pad_fwd_16bit(N, T, C, padL, padR, pool_d, y_bf16, fmt):
             pool_T * 200, 200, pool_d, pool_T]
     cpu = [a.clone() if isinstance(a, torch.Tensor) else a for a in args]
     dev = [a.cuda() if isinstance(a, torch.Tensor) else a for a in args]
-    emul_ops.call("pase_bn_prelu_pad_fwd", *cpu)
+    emul.call("pase_bn_prelu_pad_fwd", *cpu)
     _lib.call("pase_bn_prelu_pad_fwd", *dev)
     torch.cuda.synchronize()
     if fmt == 2:
@@ -355,7 +355,7 @@ def test_bn_prelu_bwd(N, T, C, padL, padR, pool_d, useB):
             torch.zeros(C, dtype=torch.float64), am, sc]
     cpu2 = [a.clone() if isinstance(a, torch.Tensor) else a for a in args]
     dev2 = [a.cuda() if isinstance(a, torch.Tensor) else a for a in args]
-    emul_ops.call("pase_bn_prelu_bwd_apply", *cpu2)
+    emul.call("pase_bn_prelu_bwd_apply", *cpu2)
     _lib.call("pase_bn_prelu_bwd_apply", *dev2)
     torch.cuda.synchronize()
     assert torch.equal(cpu2[19], dev2[19].cpu()), (cpu2[19], dev2[19])
@@ -365,8 +365,8 @@ def test_bn_prelu_bwd(N, T, C, padL, padR, pool_d, useB):
     assert float(vd.abs().max()) <= 16384.0 and float(vd.abs().max()) >= 16384.0 / 64
     assert float((vc - vd).abs().max()) <= 2e-5 * float(vc.abs().max())
     ref = torch.zeros(N * T * C)
-    emul_ops.call("pase_bn_prelu_bwd_apply", y, 0, T * C, N, T, C, mean, invstd, gamma, s1, s2,
-                  float(N * T), du, ref, None, 0, T * C, None, None, None)
+    emul.call("pase_bn_prelu_bwd_apply", y, 0, T * C, N, T, C, mean, invstd, gamma, s1, s2,
+              float(N * T), du, ref, None, 0, T * C, None, None, None)
     assert float((vd / s - ref).abs().max()) <= 1e-5 * float(ref.abs().max())
 
 
@@ -406,7 +406,7 @@ def test_bn_prelu_bwd_no_du(N, T, C, padL, padR, pool_d, useB, fmt):
                                    am if fmt == 2 else None, sc if fmt == 2 else None]
     cpu2 = [a.clone() if isinstance(a, torch.Tensor) else a for a in args]
     dev2 = [a.cuda() if isinstance(a, torch.Tensor) else a for a in args]
-    emul_ops.call("pase_bn_prelu_bwd_apply_src", *cpu2)
+    emul.call("pase_bn_prelu_bwd_apply_src", *cpu2)
     _lib.call("pase_bn_prelu_bwd_apply_src", *dev2)
     torch.cuda.synchronize()
     i_hi, i_lo, i_db, i_sc = 30, 31, 34, 36
@@ -425,12 +425,12 @@ def test_bn_prelu_bwd_no_du(N, T, C, padL, padR, pool_d, useB, fmt):
     if not bf:
         # identical to the two-pass form with a stored du
         du = torch.zeros(N * T * C)
-        emul_ops.call("pase_bn_prelu_bwd_reduce", y, 0, T * C, N, T, C, mean, invstd, scale, shift,
-                      alpha, *src, du, T * C, torch.zeros(C, dtype=torch.float64),
-                      torch.zeros(C, dtype=torch.float64), torch.zeros(C, dtype=torch.float64), None)
+        emul.call("pase_bn_prelu_bwd_reduce", y, 0, T * C, N, T, C, mean, invstd, scale, shift,
+                  alpha, *src, du, T * C, torch.zeros(C, dtype=torch.float64),
+                  torch.zeros(C, dtype=torch.float64), torch.zeros(C, dtype=torch.float64), None)
         ref = torch.zeros(N * T * C)
-        emul_ops.call("pase_bn_prelu_bwd_apply", y, 0, T * C, N, T, C, mean, invstd, gamma, s1, s2,
-                      float(N * T), du, ref, None, 0, T * C, None, None, None)
+        emul.call("pase_bn_prelu_bwd_apply", y, 0, T * C, N, T, C, mean, invstd, gamma, s1, s2,
+                  float(N * T), du, ref, None, 0, T * C, None, None, None)
         s = float(cpu2[i_sc][1]) if fmt == 2 else 1.0
         assert float((vd / s - ref).abs().max()) <= 2e-5 * float(ref.abs().max())
 

@@ -1,12 +1,12 @@
 """WaveFe.encode_long (DESIGN.md section 20) on the CPU with emulated kernels
-(tests/emul_long_grad.py): features, waveform and parameter gradients of recordings of three
+(tests/emul/): features, waveform and parameter gradients of recordings of three
 or more windows against float64 autograd through the oracle, a cotangent on one crop, short
 recordings against encode_packed, the frozen sweep, grad_sink, the plan-generation guard shared
 with encode_packed, and the refusals, all raised before any launch."""
 import pytest
 import torch
 
-import emul_long_grad
+import emul
 import pase_oracle as O
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, rel_l2
 import pase_b200.ops as ops
@@ -20,7 +20,7 @@ MINI = {"mini": "enc_mini_train_1763", "mininornn": "enc_mininornn_train_1600"}
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_long_grad.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     yield
 
 
@@ -152,7 +152,7 @@ def test_frozen_sweep(emulated, monkeypatch):
     freeze(model)
     names = []
     monkeypatch.setattr(ops, "call",
-                        lambda n, *a: (names.append(n), emul_long_grad.call(n, *a))[1])
+                        lambda n, *a: (names.append(n), emul.call(n, *a))[1])
     _, dx, grads = run_long(model, x, cot, w)
     assert torch.equal(dx, dx_full) and not grads
     assert "pase_sinc_grad" not in names and "pase_axpy" not in names

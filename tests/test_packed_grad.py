@@ -1,12 +1,12 @@
 """WaveFe.encode_packed (DESIGN.md section 18) on the CPU with emulated kernels
-(tests/emul_packed_grad.py): per-utterance waveform gradients and summed parameter gradients
+(tests/emul/): per-utterance waveform gradients and summed parameter gradients
 against float64 autograd through the oracle, independence from the neighbours in the pack, the
 refusals, the generation guard, launches independent of the number of utterances and the
 zero-row rule of the backward layout."""
 import pytest
 import torch
 
-import emul_packed_grad
+import emul
 import pase_oracle as O
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, rel_l2
 import pase_b200.ops as ops
@@ -20,7 +20,7 @@ MINI = {"mini": "enc_mini_train_1763", "mininornn": "enc_mininornn_train_1600"}
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_packed_grad.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     yield
 
 
@@ -155,7 +155,7 @@ def test_launches_independent_of_count(monkeypatch):
 
     def counting(name, *args):
         launches.append(name)
-        return emul_packed_grad.call(name, *args)
+        return emul.call(name, *args)
 
     monkeypatch.setattr(ops, "call", counting)
     model = make_model("mini", "3xtf32")

@@ -1,10 +1,9 @@
 """The references, bounds and table constructions of tests/test_packed_kernels_gpu.py run on the
 CPU against the fp32 emulations the CPU suite uses in place of the packed and windowed kernels
-(tests/emul_extract.py, emul_packed_grad.py, emul_packed_train.py, emul_long_grad.py,
-emul_streams.py), and the host-side layout invariants those kernels rely on: every padded
-operand starts on a folded-row boundary, every utterance's zero tail covers the next one's
-halo, table values stay below INDEX_LIMIT, and no pack holds more utterances than a launch
-grid has rows.  Bit equality with the uniform kernels and the tensor-core tail plan depend on
+(tests/emul/packed.py, tests/emul/windowed.py), and the host-side layout invariants those
+kernels rely on: every padded operand starts on a folded-row boundary, every utterance's zero
+tail covers the next one's halo, table values stay below INDEX_LIMIT, and no pack holds more
+utterances than a launch grid has rows.  Bit equality with the uniform kernels and the tensor-core tail plan depend on
 the hardware and stay in the GPU file."""
 import numpy as np
 import pytest

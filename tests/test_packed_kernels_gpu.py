@@ -16,7 +16,7 @@ unchanged after the call, so a store outside the contract fails even where a lat
 overwrite it.
 
 Bounds (u = 2^-24) are those of the uniform kernels' tests, imported from them:
-  GEMMs: the exact products of the operands as the tensor core reads them (emul_ops._operand),
+  GEMMs: the exact products of the operands as the tensor core reads them (emul.core._operand),
     accumulated in float64; error within 2 K u sum|a b| + 2^-20 sum|a b| (the 3x modes drop the
     lo x lo term) + 1 ulp of the bias add; bf16 output one more bf16 rounding.  colsum and
     colsumsq within 2^-16 of the sum of magnitudes of the stored values, against float64 sums
@@ -35,9 +35,7 @@ import numpy as np
 import pytest
 import torch
 
-import emul_long_grad
-import emul_ops
-import emul_packed_train
+import emul
 from pase_b200 import _lib
 from pase_b200 import encoder as E
 from test_qrnn_sinc_out_gpu import (GUARD, K_QRNN, SENT, U, Qrnn, _check_all, _full, _report,
@@ -57,10 +55,8 @@ def _call(dev, name, *args):
     if torch.device(dev).type == "cuda":
         _lib.call(name, *args)
         torch.cuda.synchronize()
-    elif hasattr(emul_packed_train, name):
-        emul_packed_train.call(name, *args)
     else:
-        emul_long_grad.call(name, *args)
+        emul.call(name, *args)
 
 
 def _gpu(dev):
@@ -229,11 +225,11 @@ class VarGemm(object):
         """Stored elements against float64, guards everywhere else, sums against float64
         sums of the stored values."""
         mode = 0 if self.mode is None else self.mode
-        Aop = emul_ops._operand(self.Ah.cpu(), None if self.Al is None else self.Al.cpu(),
-                                mode).to(self.dev).double() if self.mode is not None \
+        Aop = emul.core._operand(self.Ah.cpu(), None if self.Al is None else self.Al.cpu(),
+                                 mode).to(self.dev).double() if self.mode is not None \
             else self.Ah.double()
-        Bop = emul_ops._operand(self.Bh.cpu(), None if self.Bl is None else self.Bl.cpu(),
-                                mode).to(self.dev).double() if self.mode is not None \
+        Bop = emul.core._operand(self.Bh.cpu(), None if self.Bl is None else self.Bl.cpu(),
+                                 mode).to(self.dev).double() if self.mode is not None \
             else self.Bh.double()
         Bm = Bop[:self.N * self.K].view(self.N, self.K)
         out, spans = [], []
@@ -401,14 +397,14 @@ class Wave(object):
 
     def ref_pad(self, i):
         o, T = int(self.x_off[i]), self.lengths[i]
-        idx = emul_ops._reflect(torch.arange(T + self.padL + self.padR) - self.padL, T)
+        idx = emul.core._reflect(torch.arange(T + self.padL + self.padR) - self.padL, T)
         return self.x[o:o + T].double()[idx.to(self.dev)]
 
     def ref_fold(self, i, fold_l=1, fold_r=1):
         """float64 fold of utterance i's pad gradient and the magnitudes of its terms."""
         o, T, pL, pR = int(self.d_off[i]), self.lengths[i], self.padL, self.padR
         d = self.dpad[o:o + T + pL + pR].double()
-        idx = emul_ops._reflect(torch.arange(T + pL + pR) - pL, T).to(self.dev)
+        idx = emul.core._reflect(torch.arange(T + pL + pR) - pL, T).to(self.dev)
         keep = torch.ones(T + pL + pR, dtype=torch.bool, device=self.dev)
         if not fold_l:
             keep[:pL] = False
@@ -491,7 +487,7 @@ def fold_acc_checks(dev, seed=0):
     for x0, T, fl, fr in x0s:
         d = torch.randn(T + pL + pR, generator=gen).to(dev)
         _call(dev, "pase_reflect_fold_wave_acc", d, dx, x0, T, pL, pR, fl, fr)
-        idx = emul_ops._reflect(torch.arange(T + pL + pR) - pL, T).to(dev)
+        idx = emul.core._reflect(torch.arange(T + pL + pR) - pL, T).to(dev)
         keep = torch.ones(T + pL + pR, dtype=torch.bool, device=dev)
         if not fl:
             keep[:pL] = False
@@ -791,7 +787,7 @@ def bn_fwd_checks(b, sep=1, pool=True, padL=0, padR=0):
         # the fp32 affine rounds relative to its terms, then the gate's product once more
         am = gate.abs() * 2 * U * ((y.double() * p["scale"].double()).abs()
                                    + p["shift"].double().abs())
-        idx = emul_ops._reflect(torch.arange(Tp[i]) - padL, T).to(b.dev)
+        idx = emul.core._reflect(torch.arange(Tp[i]) - padL, T).to(b.dev)
         ref = a[idx]
         got = dst[d0:d0 + Tp[i] * C].view(Tp[i], C).double()
         tol = am[idx] + 2 * _ulp32(ref)
@@ -1379,7 +1375,7 @@ def test_64bit_offsets():
         buf[x0:x0 + Tw] = 0.0
         d = torch.randn(Tw + pL + pR, generator=gen, device="cuda")
         _call("cuda", "pase_reflect_fold_wave_acc", d, buf, x0, Tw, pL, pR, 1, 1)
-        idx = emul_ops._reflect(torch.arange(Tw + pL + pR) - pL, Tw).cuda()
+        idx = emul.core._reflect(torch.arange(Tw + pL + pR) - pL, Tw).cuda()
         refd = torch.zeros(Tw, dtype=torch.float64, device="cuda").index_add_(0, idx, d.double())
         mag = torch.zeros(Tw, dtype=torch.float64, device="cuda").index_add_(
             0, idx, d.double().abs())

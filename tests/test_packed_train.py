@@ -1,5 +1,5 @@
 """WaveFe.encode_packed_train (DESIGN.md section 19) on the CPU with emulated kernels
-(tests/emul_packed_train.py): features, per-utterance waveform gradients, parameter gradients,
+(tests/emul/): features, per-utterance waveform gradients, parameter gradients,
 running statistics and counters against a float64 oracle whose BatchNorms see the
 time-concatenation of the utterances; equality with the uniform train forward at equal lengths;
 the coupling through the batch statistics; the refusals; the shared plan's generation guard;
@@ -8,7 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import emul_packed_train
+import emul
 import pase_oracle as O
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, rel_l2
 import pase_b200.ops as ops
@@ -22,7 +22,7 @@ MINI = {"mini": "enc_mini_train_1763", "mininornn": "enc_mininornn_train_1600"}
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_packed_train.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     yield
 
 
@@ -262,7 +262,7 @@ def test_launches_independent_of_count(monkeypatch):
 
     def counting(name, *args):
         launches.append(name)
-        return emul_packed_train.call(name, *args)
+        return emul.call(name, *args)
 
     monkeypatch.setattr(ops, "call", counting)
     model = make_model("mini", "3xtf32")

@@ -47,12 +47,12 @@ x is at most 2u |x|, so each of these functions is off by at most 4u relative.
     convention); the applied gradient within 2^-20 |scale| (|g| + |S1/M| + |xhat| |S2/M|).
   bn_finalize: 1 fp32 ulp, plus the fp64 cancellation of q/M - m^2 carried to each output.
 Each case prints its worst error as a fraction of its bound.  test_bounds_hold_for_emulation
-runs the fp32 torch emulation (tests/emul_ops.py) through the same references and bounds on the
+runs the fp32 torch emulation (tests/emul/) through the same references and bounds on the
 CPU, and shows that moving one element by twice its bound fails."""
 import pytest
 import torch
 
-import emul_ops
+import emul
 from pase_b200 import _lib
 from pase_b200 import encoder as E
 
@@ -111,7 +111,7 @@ def _call(dev, name, *args):
         _lib.call(name, *args)
         torch.cuda.synchronize()
     else:
-        emul_ops.call(name, *args)
+        emul.call(name, *args)
 
 
 # ---- PASE+ geometry ----

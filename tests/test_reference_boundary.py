@@ -7,7 +7,7 @@ written by tests/golden/make_golden.py::boundary_case from the reference's own c
       drove the reference model for two optimisation steps.  The same step sequence drives the
       native ``pase_b200.pase.pase`` model on the same weights and batch; losses are compared
       step by step, then the weights after the second update.  (CUDA kernels replaced by their
-      torch specs, tests/emul_ops.py; the GPU tests cover the kernels.)
+      torch specs, tests/emul/; the GPU tests cover the kernels.)
   (2) Checkpoints: files written by the reference ``Saver`` / ``Model.save`` load into the
       native modules (``load_pretrained``, ``Model.load``); the native Saver writes the same
       index file, the same rotation and checkpoints of the same structure and content
@@ -21,7 +21,7 @@ import random
 import pytest
 import torch
 
-import emul_ops
+import emul
 from helpers import GOLDEN, load_golden, resolve_cfg, fill_state_dict, seeded_randn, sample_view
 import pase_b200.ops as ops
 from pase_b200 import encoder as enc, wf_builder
@@ -41,7 +41,7 @@ def _boundary():
 
 @pytest.fixture()
 def emulated(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_ops.call)
+    monkeypatch.setattr(ops, "call", emul.call)
 
     def encode_cpu(self, x):
         self._sinc_consts(x.device)

@@ -1,5 +1,5 @@
 """Host side of WaveFe.streams() / StreamPool on CPU, every kernel launch replaced by its torch
-emulation (tests/emul_streams.py): many staggered streams against one one-stream pool each fed
+emulation (tests/emul/): many staggered streams against one one-stream pool each fed
 the same blocks, against the recording pushed whole and against the B=1 forward, slot reuse, a
 finish folded into the last block, the pack bound, and refusals raised before any launch with no
 stream changed.  The emulated GEMMs round differently for different segment lengths, so here a
@@ -10,7 +10,7 @@ import random
 import pytest
 import torch
 
-import emul_streams
+import emul
 from helpers import resolve_cfg, fill_state_dict, seeded_randn, assert_close
 import pase_b200.ops as ops
 from pase_b200 import encoder as enc
@@ -32,7 +32,7 @@ def gathers(monkeypatch):
         seen.names.append(name)
         if name == "pase_stream_gather":
             seen.append(args[4][:8 * args[5]].view(-1, 8).clone())
-        return emul_streams.call(name, *args)
+        return emul.call(name, *args)
     monkeypatch.setattr(ops, "call", call)
     yield seen
 

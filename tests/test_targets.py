@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-import emul_ops
+import emul
 import pase_b200.ops as ops
 from pase_b200.targets import LPS, savgol_taps
 
@@ -64,7 +64,7 @@ def test_savgol_taps_equal_scipy():
 
 @pytest.mark.parametrize("T,win,der", [(3200, 400, 2), (4001, 512, 2), (1600, 400, 0)])
 def test_lps_host_logic_against_oracle(monkeypatch, T, win, der):
-    monkeypatch.setattr(ops, "call", emul_ops.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     monkeypatch.setattr(torch.Tensor, "is_cuda", property(lambda self: True))
     wav = _wave(2, T, 3)
     lps = LPS(n_fft=2048, hop=160, win=win, der_order=der, device="cpu")
@@ -91,7 +91,7 @@ def test_lps_kernels_gpu(N, T, win):
     x = _wave(N, T, 5).reshape(-1)
     start0 = (n_fft - win) // 2 - n_fft // 2
     hi, lo = (torch.zeros(N * frames * lda, dtype=torch.float16) for _ in range(2))
-    emul_ops.call("pase_frame_wave", x, N, T, hop, win, start0, frames, hi, lo, lda)
+    emul.call("pase_frame_wave", x, N, T, hop, win, start0, frames, hi, lo, lda)
     dh, dl = hi.cuda().zero_(), lo.cuda().zero_()
     _lib.call("pase_frame_wave", x.cuda(), N, T, hop, win, start0, frames, dh, dl, lda)
     assert torch.equal(dh.cpu(), hi) and torch.equal(dl.cpu(), lo)
@@ -104,8 +104,8 @@ def test_lps_kernels_gpu(N, T, win):
     mean, std = torch.randn(F, generator=g), torch.rand(F, generator=g) + 0.5
     for st in (None, (mean, std)):
         ref = torch.zeros(N * F * frames)
-        emul_ops.call("pase_lps_post", C, ldc, N, frames, nbins, 2, 9, fir,
-                      None if st is None else st[0], None if st is None else st[1], ref)
+        emul.call("pase_lps_post", C, ldc, N, frames, nbins, 2, 9, fir,
+                  None if st is None else st[0], None if st is None else st[1], ref)
         out = torch.zeros(N * F * frames).cuda()
         _lib.call("pase_lps_post", C.cuda(), ldc, N, frames, nbins, 2, 9, fir.cuda(),
                   None if st is None else st[0].cuda(), None if st is None else st[1].cuda(), out)

@@ -13,7 +13,7 @@ import math
 import pytest
 import torch
 
-import emul_ops
+import emul
 from pase_b200 import _lib
 from test_kernels_gpu import R
 
@@ -39,9 +39,9 @@ def _split(x, weights=False):
     lo = torch.zeros_like(x)
     if weights:
         hi = torch.zeros_like(x)
-        emul_ops.pase_split_tf32(x, hi, lo, x.numel())
+        emul.core.pase_split_tf32(x, hi, lo, x.numel())
         return hi, lo
-    emul_ops.pase_split_tf32(x, None, lo, x.numel())
+    emul.core.pase_split_tf32(x, None, lo, x.numel())
     return x.clone(), lo
 
 
@@ -62,7 +62,7 @@ def _run(name, args, offset_args=()):
     dev = [a.cuda() if isinstance(a, torch.Tensor) else a for a in args]
     for i in offset_args:
         cpu[i], dev[i] = cpu[i][1:], dev[i][1:]
-    emul_ops.call(name, *cpu)
+    emul.call(name, *cpu)
     _lib.call(name, *dev)
     torch.cuda.synchronize()
     return cpu, dev
@@ -79,7 +79,7 @@ def test_split_kernel_bit_exact():
     dl2 = torch.zeros_like(x).cuda()
     _lib.call("pase_split_tf32", x.cuda(), None, dl2, x.numel())       # activation form
     assert torch.equal(dl2.cpu(), lo_a)
-    xt = emul_ops._tf32_trunc(x)
+    xt = emul.core._tf32_trunc(x)
     assert float((x - xt - lo_a).abs().max()) <= float(x.abs().max()) * 2.0 ** -21
 
 
@@ -369,7 +369,7 @@ def test_tc_gemm_tn_back_to_back(mode):
     torch.cuda.synchronize()
     for args, dev, shp in zip(runs, devs, (_SPLIT_A, _SPLIT_B)):
         cpu = [a.clone() if isinstance(a, torch.Tensor) else a for a in args]
-        emul_ops.call("pase_tc_gemm_tn", *cpu)
+        emul.call("pase_tc_gemm_tn", *cpu)
         _tn_check(cpu, dev, mode, shp[0], shp[1], shp[9])
 
 
@@ -398,7 +398,7 @@ def test_tc_gemm_tn_graph_replay(mode):
         g.replay()
         torch.cuda.synchronize()
         cpu = [a.clone() if isinstance(a, torch.Tensor) else a for a in new]
-        emul_ops.call("pase_tc_gemm_tn", *cpu)
+        emul.call("pase_tc_gemm_tn", *cpu)
         _tn_check(cpu, dev, mode, shp[0], shp[1], shp[9])
 
 

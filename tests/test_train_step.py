@@ -12,8 +12,7 @@ import numpy as np
 import pytest
 import torch
 
-import emul_batch
-import emul_spc
+import emul
 from helpers import resolve_cfg
 from pase_b200 import functional as Fn
 from pase_b200 import ops
@@ -162,7 +161,7 @@ def check_strided_rows(device):
 
 
 def test_emulated_spc_gather_strided_rows(monkeypatch):
-    monkeypatch.setattr(ops, "call", emul_spc.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     check_strided_rows("cpu")
 
 
@@ -175,7 +174,7 @@ def test_emulated_spc_gather_matches_torch_gather(ci, monkeypatch):
     x = torch.randn(B * T, C, generator=gen)
     g = torch.randn(2 * B, (N + 1) * C, generator=gen)
     ref_y, ref_dx = spc_reference(x, g, case, frames)
-    monkeypatch.setattr(ops, "call", emul_spc.call)
+    monkeypatch.setattr(ops, "call", emul.call)
     xr = x.clone().requires_grad_(True)
     y = Fn.spc_gather(xr, B, T, N, sp, frames)
     y.backward(g)
@@ -200,7 +199,7 @@ def test_planner_draws_what_eager_spc_forward_consumes(monkeypatch):
     def spy(name, *a):
         if name == "pase_spc_gather":
             seen.append(tuple(a[2].tolist()))
-        return emul_spc.call(name, *a)
+        return emul.call(name, *a)
     monkeypatch.setattr(ops, "call", spy)
     from pase_b200.minions import cls_worker_maker
     from pase_b200.losses import ContextualizedLoss
@@ -264,11 +263,7 @@ def emulated(monkeypatch):
     def call(name, *a):
         if name == "pase_spc_gather":
             _SEEN.append(tuple(a[2].tolist()))
-        if name.startswith("pase_spc_"):
-            return emul_spc.call(name, *a)
-        if name in ("pase_chunk_gather", "pase_frames_gather"):
-            return emul_batch.call(name, *a)
-        return emul_spc.call(name, *a)
+        return emul.call(name, *a)
     monkeypatch.setattr(ops, "call", call)
     yield
 
@@ -344,8 +339,8 @@ def test_spc_head_refuses_a_chunk_too_short_for_its_frames():
 
 
 def test_flat_adam_table_keeps_its_address(monkeypatch):
-    import emul_ops
-    monkeypatch.setattr(ops, "call", emul_ops.call)
+    import emul
+    monkeypatch.setattr(ops, "call", emul.call)
     net = torch.nn.Sequential(torch.nn.Linear(5, 7), torch.nn.Linear(7, 3))
     opt = FlatAdam([{"params": list(net[0].parameters()), "lr": 1e-2},
                     {"params": list(net[1].parameters())}], lr=1e-3)

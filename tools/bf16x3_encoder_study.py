@@ -2,7 +2,7 @@
 """CPU study: would the whole PASE+ encoder still meet the parity bar if every tensor-core
 GEMM used three bf16 products of a two-term bf16 operand split (a1 b1 + a1 b2 + a2 b1)
 instead of 3xTF32?  Runs the host orchestration of pase_b200 with the torch emulation of the
-kernels (tests/emul_ops.py), swaps the product model of the two GEMM entry points, and
+kernels (tests/emul/), swaps the product model of the two GEMM entry points, and
 compares forward outputs and gradients with the golden vectors of the unmodified reference.
 Measurement helper for the next round's kernel work; not part of the library or the tests.
 """
@@ -15,7 +15,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for _p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden")):
     sys.path.insert(0, _p)
 
-import emul_ops                                              # noqa: E402
+import emul                                                  # noqa: E402
 from helpers import load_golden, resolve_cfg, fill_state_dict, seeded_randn, rel_l2   # noqa: E402
 from detweights import sample_view                            # noqa: E402
 import pase_b200.ops as ops                                  # noqa: E402
@@ -45,12 +45,12 @@ class Bf16x3(object):
         a[:lim] = Ahi[:lim]                                  # activations: the raw fp32 array
         b = Bhi[:N * ldb].clone()
         if Blo is not None:
-            b += emul_ops._like(Blo, Bhi)[:N * ldb]          # weights: hi + lo = the fp32 value
+            b += emul.core._like(Blo, Bhi)[:N * ldb]         # weights: hi + lo = the fp32 value
         first = True
         for x, y in terms(a, b):
-            emul_ops.pase_gemm_nt(x, R, y, ldb, C, ldc, M, N, K, alpha, bias if first else None,
-                                  rows_in, t_valid, rows_out, fold, None, None,
-                                  accumulate if first else 1)
+            emul.core.pase_gemm_nt(x, R, y, ldb, C, ldc, M, N, K, alpha, bias if first else None,
+                                   rows_in, t_valid, rows_out, fold, None, None,
+                                   accumulate if first else 1)
             first = False
         if colsum is not None:                               # statistics of the final values
             m = torch.arange(M)
@@ -59,7 +59,7 @@ class Bf16x3(object):
             cpf = N // fold
             valid = (u[keep][:, None] * fold + (torch.arange(N) // cpf)[None, :]) < t_valid
             orow = (g * rows_out + u)[keep]
-            Cv = emul_ops._as(C, (int(orow.max()) + 1, N), (ldc, 1))[orow]
+            Cv = emul.core._as(C, (int(orow.max()) + 1, N), (ldc, 1))[orow]
             ov = torch.where(valid, Cv, torch.zeros_like(Cv)).double()
             colsum[:N] += ov.sum(0)
             colsumsq[:N] += (ov * ov).sum(0)
@@ -74,14 +74,14 @@ class Bf16x3(object):
         b[:lim] = Bhi[:lim]
         first = True
         for x, y in terms(Ahi.clone(), b):
-            emul_ops.pase_gemm_tn(x, lda, pitchA, offA, y, R, pitchB, 0, C, ldc, I, J, groups,
-                                  rows_per_group, alpha, accumulate if first else 1)
+            emul.core.pase_gemm_tn(x, lda, pitchA, offA, y, R, pitchB, 0, C, ldc, I, J, groups,
+                                   rows_per_group, alpha, accumulate if first else 1)
             first = False
 
 
 def _tf32_terms(a, b):
     """(x, y) factor pairs of the mixed scheme: TF32 main product + two bf16 corrections."""
-    ah, bh = emul_ops._tf32_trunc(a), emul_ops._tf32_rn(b)
+    ah, bh = emul.core._tf32_trunc(a), emul.core._tf32_rn(b)
     return ((ah, bh), (bf16(a - ah), bf16(b)), (bf16(a), bf16(b - bh)))
 
 
@@ -115,18 +115,18 @@ def run(name, model_fns):
     model.load_state_dict(fill_state_dict(model.state_dict(), meta["seed"]))
     model.train(meta["training"])
     x = seeded_randn((meta["N"], 1, meta["T"]), meta["seed"] + 1, 0.5)
-    saved = (emul_ops.pase_tc_gemm_nt, emul_ops.pase_tc_gemm_tn)
+    saved = (emul.core.pase_tc_gemm_nt, emul.core.pase_tc_gemm_tn)
     if model_fns is not None:
-        emul_ops.pase_tc_gemm_nt, emul_ops.pase_tc_gemm_tn = model_fns
+        emul.core.pase_tc_gemm_nt, emul.core.pase_tc_gemm_tn = model_fns
     real = ops.call
-    ops.call = emul_ops.call
+    ops.call = emul.call
     try:
         y, _ = run_encoder_cpu(model, x)
         cot = seeded_randn(tuple(y.shape), meta["seed"] + 2)
         (y * cot).sum().backward()
     finally:
         ops.call = real
-        emul_ops.pase_tc_gemm_nt, emul_ops.pase_tc_gemm_tn = saved
+        emul.core.pase_tc_gemm_nt, emul.core.pase_tc_gemm_tn = saved
     yg = gold["y"]
     err = (y.detach() - yg).abs()
     worst = float((err / (1e-5 + 1e-3 * yg.abs())).max())    # <= 1 meets rtol 1e-3 / atol 1e-5

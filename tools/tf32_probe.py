@@ -5,14 +5,14 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import torch
 from pase_b200 import _lib
-import emul_ops
+import emul
 
 torch.manual_seed(0)
 M = N = 128
 K = 256
 A, B = torch.randn(M * K + 64), torch.randn(N * K)
-At = emul_ops._tf32_trunc(A)
-Bt = emul_ops._tf32_trunc(B)
+At = emul.core._tf32_trunc(A)
+Bt = emul.core._tf32_trunc(B)
 outs = []
 for a, b in ((A, B), (At, Bt)):
     C = torch.zeros(M * N).cuda()
