@@ -2,6 +2,7 @@
 // All HBM-bound: channel-last float4 accesses, one pass per tensor.
 #include "common.cuh"
 #include "bn_stream.cuh"
+#include <type_traits>
 
 namespace {
 
@@ -19,40 +20,12 @@ constexpr int FWD_THREADS = 128;
 template <int DF>
 constexpr int fwd_min_blocks() { return DF == PASE_FMT_F32 ? 6 : 7; }
 
+// One utterance's reflect pad: dst[d0 + tau] = xn[reflect(tau - padL)] for tau < Tp.
 // DF: operand format of the padded waveform (block 0's GEMM operand)
 template <int DF>
-__global__ void reflect_pad_wave_kernel(const float* __restrict__ x, void* __restrict__ dst_v,
-                                        void* __restrict__ dst_lo_v, int T, int padL, int Tp,
-                                        long pitch) {
-  pdl_wait();
-  const int n = blockIdx.y;
-  for (int tau = blockIdx.x * blockDim.x + threadIdx.x; tau < Tp; tau += gridDim.x * blockDim.x) {
-    const float v = x[(long)n * T + reflect_idx(tau - padL, T)];
-    const long o = (long)n * pitch + tau;
-    if constexpr (DF == PASE_FMT_F32) {
-      reinterpret_cast<float*>(dst_v)[o] = v;
-      if (dst_lo_v != nullptr) reinterpret_cast<float*>(dst_lo_v)[o] = tf32_residual(v);
-    } else if constexpr (DF == PASE_FMT_BF16) {
-      reinterpret_cast<__nv_bfloat16*>(dst_v)[o] = __float2bfloat16_rn(v);
-    } else {
-      __half h, l;
-      f16_split(v, h, l);
-      reinterpret_cast<__half*>(dst_v)[o] = h;
-      reinterpret_cast<__half*>(dst_lo_v)[o] = l;
-    }
-  }
-}
-
-// Packed variable-length form: blockIdx.y = utterance, tab row {x_off, T, dst_off}.
-template <int DF>
-__global__ void reflect_pad_wave_var_kernel(const float* __restrict__ x, const int* __restrict__ tab,
-                                            void* __restrict__ dst_v, void* __restrict__ dst_lo_v,
-                                            int padL, int padR) {
-  pdl_wait();
-  const int* r = tab + 3 * blockIdx.y;
-  const float* xn = x + __ldg(r);
-  const int T = __ldg(r + 1), Tp = T + padL + padR;
-  const long d0 = __ldg(r + 2);
+__device__ __forceinline__ void reflect_pad_wave_utt(const float* __restrict__ xn, int T, int padL,
+                                                     int Tp, void* __restrict__ dst_v,
+                                                     void* __restrict__ dst_lo_v, long d0) {
   for (int tau = blockIdx.x * blockDim.x + threadIdx.x; tau < Tp; tau += gridDim.x * blockDim.x) {
     const float v = xn[reflect_idx(tau - padL, T)];
     const long o = d0 + tau;
@@ -68,6 +41,34 @@ __global__ void reflect_pad_wave_var_kernel(const float* __restrict__ x, const i
       reinterpret_cast<__half*>(dst_lo_v)[o] = l;
     }
   }
+}
+
+template <int DF>
+__global__ void reflect_pad_wave_kernel(const float* __restrict__ x, void* __restrict__ dst_v,
+                                        void* __restrict__ dst_lo_v, int T, int padL, int Tp,
+                                        long pitch) {
+  pdl_wait();
+  const int n = blockIdx.y;
+  reflect_pad_wave_utt<DF>(x + (long)n * T, T, padL, Tp, dst_v, dst_lo_v, (long)n * pitch);
+}
+
+// Packed variable-length form: blockIdx.y = utterance, tab row {x_off, T, dst_off}.
+template <int DF>
+__global__ void reflect_pad_wave_var_kernel(const float* __restrict__ x, const int* __restrict__ tab,
+                                            void* __restrict__ dst_v, void* __restrict__ dst_lo_v,
+                                            int padL, int padR) {
+  pdl_wait();
+  const int* r = tab + 3 * blockIdx.y;
+  const int T = __ldg(r + 1);
+  reflect_pad_wave_utt<DF>(x + __ldg(r), T, padL, T + padL + padR, dst_v, dst_lo_v, __ldg(r + 2));
+}
+
+// Calls f(std::integral_constant<int, DF>()) for the operand format fmt (checked by the caller).
+template <typename F>
+void with_fmt(int fmt, F f) {
+  if (fmt == PASE_FMT_F32) f(std::integral_constant<int, PASE_FMT_F32>());
+  else if (fmt == PASE_FMT_BF16) f(std::integral_constant<int, PASE_FMT_BF16>());
+  else f(std::integral_constant<int, PASE_FMT_F16X2>());
 }
 
 __global__ void bn_finalize_kernel(const double* __restrict__ colsum,
@@ -983,52 +984,6 @@ bn_prelu_bwd_apply_src_var_train_kernel(
       B, b_rs, b_shift, pool, p_rs, dst_v, dst_lo_v, lead, dbias, amax, scale_out);
 }
 
-// pase_out_bwd_reduce over packed utterances: tab rows {row0, T, o_off} (blockIdx.z), tiles of
-// 32 frames x 32 channels; g_ntc[(row0 + t)*C + c] = dout[o_off + c*T + t], S1 += g,
-// S2 += g*xhat
-__global__ void out_bwd_reduce_var_kernel(const float* __restrict__ dout,
-                                          const int* __restrict__ tab,
-                                          const float* __restrict__ y,
-                                          const float* __restrict__ mean,
-                                          const float* __restrict__ invstd, int C,
-                                          float* __restrict__ g_ntc, double* __restrict__ S1,
-                                          double* __restrict__ S2) {
-  pdl_wait();
-  __shared__ float tile[32][33];
-  __shared__ double r1[32], r2[32];
-  const int* r = tab + 3 * blockIdx.z;
-  const long row0 = __ldg(r), o = __ldg(r + 2);
-  const int T = __ldg(r + 1);
-  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  if (t0 >= T) return;                       // the whole block: before any barrier
-  if (threadIdx.y == 0) { r1[threadIdx.x] = 0.0; r2[threadIdx.x] = 0.0; }
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int c = c0 + i, t = t0 + threadIdx.x;
-    tile[i][threadIdx.x] = (t < T && c < C) ? dout[o + (long)c * T + t] : 0.f;
-  }
-  __syncthreads();
-  float a1 = 0.f, a2 = 0.f;
-  const int c = c0 + threadIdx.x;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int t = t0 + i;
-    if (t < T && c < C) {
-      const long off = (row0 + t) * C + c;
-      const float g = tile[threadIdx.x][i];
-      g_ntc[off] = g;
-      const float xh = (y[off] - mean[c]) * invstd[c];
-      a1 += g;
-      a2 += g * xh;
-    }
-  }
-  atomicAdd(&r1[threadIdx.x], (double)a1);
-  atomicAdd(&r2[threadIdx.x], (double)a2);
-  __syncthreads();
-  if (threadIdx.y == 0 && c < C) {
-    atomicAdd(S1 + c, r1[threadIdx.x]);
-    atomicAdd(S2 + c, r2[threadIdx.x]);
-  }
-}
-
 // g[row0 + t, c] = dout[o_off + c T + t] for tab rows {row0, T, o_off} (pase_out_bwd_reduce's
 // layout change, one utterance per blockIdx.y)
 __global__ void __launch_bounds__(256)
@@ -1141,26 +1096,38 @@ __global__ void cast_d2f_kernel(const double* __restrict__ src, float* __restric
 }
 
 // ---- output affine + (N*T,C) -> (N,C,T) ----
-__global__ void out_affine_nct_kernel(const float* __restrict__ y, const float* __restrict__ scale,
-                                      const float* __restrict__ shift, float* __restrict__ out,
-                                      float* __restrict__ out_ntc, int T, int C) {
-  pdl_wait();
+// One 32 frames x 32 channels tile (blockIdx.x, blockIdx.y) of one utterance whose T frames are
+// rows row0 .. row0+T-1 of y: h = y*scale+shift goes to o[c*ldo + t] and, when out_ntc is given,
+// to the same rows of out_ntc.
+__device__ __forceinline__ void out_affine_tile(const float* __restrict__ y,
+                                                const float* __restrict__ scale,
+                                                const float* __restrict__ shift,
+                                                float* __restrict__ o, long ldo,
+                                                float* __restrict__ out_ntc, long row0, int T,
+                                                int C) {
   __shared__ float tile[32][33];
-  const int n = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const int t = t0 + i, c = c0 + threadIdx.x;
     if (t < T && c < C) {
-      const float v = fmaf(y[((long)n * T + t) * C + c], scale[c], shift[c]);
+      const float v = fmaf(y[(row0 + t) * C + c], scale[c], shift[c]);
       tile[i][threadIdx.x] = v;
-      if (out_ntc) out_ntc[((long)n * T + t) * C + c] = v;
+      if (out_ntc) out_ntc[(row0 + t) * C + c] = v;
     }
   }
   __syncthreads();
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const int c = c0 + i, t = t0 + threadIdx.x;
-    if (t < T && c < C) out[((long)n * C + c) * T + t] = tile[threadIdx.x][i];
+    if (t < T && c < C) o[(long)c * ldo + t] = tile[threadIdx.x][i];
   }
+}
+
+__global__ void out_affine_nct_kernel(const float* __restrict__ y, const float* __restrict__ scale,
+                                      const float* __restrict__ shift, float* __restrict__ out,
+                                      float* __restrict__ out_ntc, int T, int C) {
+  pdl_wait();
+  const int n = blockIdx.z;
+  out_affine_tile(y, scale, shift, out + (long)n * C * T, T, out_ntc, (long)n * T, T, C);
 }
 
 // Packed variable-length output: blockIdx.y = utterance, tab row {y_row, T, out_off}; block
@@ -1217,31 +1184,17 @@ out_affine_var_kernel(const float* __restrict__ y, const float* __restrict__ sca
 }
 
 // Windowed output (StreamPool, so FeatureStream and WaveFe.extract_long): segment blockIdx.z's
-// row {row0, T, ocol, ldo, col0} writes rows row0 .. row0+T-1 of y, as h = y*scale+shift (the
-// fmaf of out_affine_nct_kernel), into columns col0 .. col0+T-1 of the (C, ldo) block that
-// starts at element ocol*C of out.  32x32 tiles.
+// row {row0, T, ocol, ldo, col0} writes rows row0 .. row0+T-1 of y, as h = y*scale+shift, into
+// columns col0 .. col0+T-1 of the (C, ldo) block that starts at element ocol*C of out.
 __global__ void out_place_var_kernel(const float* __restrict__ y, const float* __restrict__ scale,
                                      const float* __restrict__ shift, float* __restrict__ out,
                                      const int* __restrict__ tab, int C) {
   pdl_wait();
-  __shared__ float tile[32][33];
   const int* row = tab + 5 * blockIdx.z;
-  const long row0 = __ldg(row);
   const int T = __ldg(row + 1);
-  const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  if (t0 >= T) return;                        // uniform over the block
-  const long ldo = __ldg(row + 3), col0 = __ldg(row + 4);
-  float* o = out + (long)__ldg(row + 2) * C;
-  const float* yr = y + row0 * C;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int t = t0 + i, c = c0 + threadIdx.x;
-    if (t < T && c < C) tile[i][threadIdx.x] = fmaf(yr[(long)t * C + c], scale[c], shift[c]);
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int c = c0 + i, t = t0 + threadIdx.x;
-    if (t < T && c < C) o[(long)c * ldo + col0 + t] = tile[threadIdx.x][i];
-  }
+  if ((int)blockIdx.x * 32 >= T) return;      // uniform over the block
+  out_affine_tile(y, scale, shift, out + (long)__ldg(row + 2) * C + __ldg(row + 4), __ldg(row + 3),
+                  nullptr, __ldg(row), T, C);
 }
 
 // select_output over a whole (C, T) output in place: one block per channel.  The time mean is
@@ -1273,22 +1226,24 @@ out_select_kernel(float* __restrict__ out, long T, int C, int mode) {
   }
 }
 
-// g[n,t,c] = dout_nct[n,c,t] (+ dout_ntc[n,t,c]); S1 += g, S2 += g*xhat
-__global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
-                                      const float* __restrict__ dout_ntc,
-                                      const float* __restrict__ y, const float* __restrict__ mean,
-                                      const float* __restrict__ invstd, int T, int C,
-                                      float* __restrict__ g_ntc, double* __restrict__ S1,
-                                      double* __restrict__ S2) {
-  pdl_wait();
+// One 32 frames x 32 channels tile (blockIdx.x, blockIdx.y) of one utterance whose T frames are
+// rows row0 .. row0+T-1 of g_ntc / y / dout_ntc and columns of the (C, T) block at dout + o:
+// g = dout (0 when dout is null) + dout_ntc (when given), stored at g_ntc; S1 += g, S2 += g*xhat.
+__device__ __forceinline__ void out_bwd_reduce_tile(const float* __restrict__ dout, long o,
+                                                    const float* __restrict__ dout_ntc,
+                                                    const float* __restrict__ y,
+                                                    const float* __restrict__ mean,
+                                                    const float* __restrict__ invstd, long row0,
+                                                    int T, int C, float* __restrict__ g_ntc,
+                                                    double* __restrict__ S1,
+                                                    double* __restrict__ S2) {
   __shared__ float tile[32][33];
   __shared__ double r1[32], r2[32];   // fp64: order-independent to fp32 precision
-  const int n = blockIdx.z;
   const int t0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
   if (threadIdx.y == 0) { r1[threadIdx.x] = 0.0; r2[threadIdx.x] = 0.0; }
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const int c = c0 + i, t = t0 + threadIdx.x;
-    tile[i][threadIdx.x] = (dout && t < T && c < C) ? dout[((long)n * C + c) * T + t] : 0.f;
+    tile[i][threadIdx.x] = (dout && t < T && c < C) ? dout[o + (long)c * T + t] : 0.f;
   }
   __syncthreads();
   float a1 = 0.f, a2 = 0.f;
@@ -1296,11 +1251,11 @@ __global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const int t = t0 + i;
     if (t < T && c < C) {
-      const long o = ((long)n * T + t) * C + c;
+      const long off = (row0 + t) * C + c;
       float g = tile[threadIdx.x][i];
-      if (dout_ntc) g += dout_ntc[o];
-      g_ntc[o] = g;
-      const float xh = (y[o] - mean[c]) * invstd[c];
+      if (dout_ntc) g += dout_ntc[off];
+      g_ntc[off] = g;
+      const float xh = (y[off] - mean[c]) * invstd[c];
       a1 += g;
       a2 += g * xh;
     }
@@ -1312,6 +1267,36 @@ __global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
     atomicAdd(S1 + c, r1[threadIdx.x]);
     atomicAdd(S2 + c, r2[threadIdx.x]);
   }
+}
+
+// g[n,t,c] = dout_nct[n,c,t] (+ dout_ntc[n,t,c]); S1 += g, S2 += g*xhat
+__global__ void out_bwd_reduce_kernel(const float* __restrict__ dout,
+                                      const float* __restrict__ dout_ntc,
+                                      const float* __restrict__ y, const float* __restrict__ mean,
+                                      const float* __restrict__ invstd, int T, int C,
+                                      float* __restrict__ g_ntc, double* __restrict__ S1,
+                                      double* __restrict__ S2) {
+  pdl_wait();
+  const int n = blockIdx.z;
+  out_bwd_reduce_tile(dout, (long)n * C * T, dout_ntc, y, mean, invstd, (long)n * T, T, C, g_ntc,
+                      S1, S2);
+}
+
+// pase_out_bwd_reduce over packed utterances: tab rows {row0, T, o_off} (blockIdx.z), tiles of
+// 32 frames x 32 channels; g_ntc[(row0 + t)*C + c] = dout[o_off + c*T + t], S1 += g,
+// S2 += g*xhat
+__global__ void out_bwd_reduce_var_kernel(const float* __restrict__ dout,
+                                          const int* __restrict__ tab,
+                                          const float* __restrict__ y,
+                                          const float* __restrict__ mean,
+                                          const float* __restrict__ invstd, int C,
+                                          float* __restrict__ g_ntc, double* __restrict__ S1,
+                                          double* __restrict__ S2) {
+  pdl_wait();
+  const int* r = tab + 3 * blockIdx.z;
+  const int T = __ldg(r + 1);
+  if ((int)blockIdx.x * 32 >= T) return;     // the whole block: before any barrier
+  out_bwd_reduce_tile(dout, __ldg(r + 2), nullptr, y, mean, invstd, __ldg(r), T, C, g_ntc, S1, S2);
 }
 
 // in place on g (N*T,C): dy = scale_c*(g - use*(S1/M + xhat*S2/M))
@@ -1502,13 +1487,10 @@ int pase_reflect_pad_wave(const float* x, void* dst, void* dst_lo, int dst_fmt, 
   const int Tp = T + padL + padR;
   PASE_CHECK_ARG(pitch >= Tp, "pase_reflect_pad_wave: pitch %ld < padded length %d", pitch, Tp);
   dim3 grid(blocks_for(Tp, 256, 4), N);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dst_fmt == PASE_FMT_F32)
-    PASE_LAUNCH((reflect_pad_wave_kernel<PASE_FMT_F32>), grid, 256, 0, st, x, dst, dst_lo, T, padL, Tp, pitch);
-  else if (dst_fmt == PASE_FMT_BF16)
-    PASE_LAUNCH((reflect_pad_wave_kernel<PASE_FMT_BF16>), grid, 256, 0, st, x, dst, dst_lo, T, padL, Tp, pitch);
-  else
-    PASE_LAUNCH((reflect_pad_wave_kernel<PASE_FMT_F16X2>), grid, 256, 0, st, x, dst, dst_lo, T, padL, Tp, pitch);
+  with_fmt(dst_fmt, [&](auto df) {
+    PASE_LAUNCH((reflect_pad_wave_kernel<decltype(df)::value>), grid, 256, 0, stream, x, dst,
+                dst_lo, T, padL, Tp, pitch);
+  });
   PASE_LAUNCH_CHECK("pase_reflect_pad_wave");
   return PASE_OK;
 }
@@ -1522,13 +1504,10 @@ int pase_reflect_pad_wave_var(const float* x, const int* tab, int nseg, int max_
   PASE_CHECK_ARG(dst_fmt >= 0 && dst_fmt <= 2 && (dst_fmt != PASE_FMT_F16X2 || dst_lo),
                  "pase_reflect_pad_wave_var: bad dst_fmt %d / missing lo", dst_fmt);
   dim3 grid(blocks_for((long)max_T + padL + padR, 256, 4), nseg);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dst_fmt == PASE_FMT_F32)
-    PASE_LAUNCH((reflect_pad_wave_var_kernel<PASE_FMT_F32>), grid, 256, 0, st, x, tab, dst, dst_lo, padL, padR);
-  else if (dst_fmt == PASE_FMT_BF16)
-    PASE_LAUNCH((reflect_pad_wave_var_kernel<PASE_FMT_BF16>), grid, 256, 0, st, x, tab, dst, dst_lo, padL, padR);
-  else
-    PASE_LAUNCH((reflect_pad_wave_var_kernel<PASE_FMT_F16X2>), grid, 256, 0, st, x, tab, dst, dst_lo, padL, padR);
+  with_fmt(dst_fmt, [&](auto df) {
+    PASE_LAUNCH((reflect_pad_wave_var_kernel<decltype(df)::value>), grid, 256, 0, stream, x, tab,
+                dst, dst_lo, padL, padR);
+  });
   PASE_LAUNCH_CHECK("pase_reflect_pad_wave_var");
   return PASE_OK;
 }

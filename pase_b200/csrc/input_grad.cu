@@ -56,18 +56,28 @@ sinc_dgrad_weight_kernel(const float* __restrict__ filt, float* __restrict__ Wdg
   }
 }
 
+// One utterance's fold: o[t] = (+= when ACC) its padded-waveform gradient at t, plus the mirrored
+// pad gradient on the sides where the pad reflects the utterance itself (fold_l / fold_r)
+template <bool ACC>
+__device__ __forceinline__ void reflect_fold_wave_utt(const float* __restrict__ d,
+                                                      float* __restrict__ o, int T, int padL,
+                                                      int padR, bool fold_l, bool fold_r) {
+  for (int t = blockIdx.x * THREADS + threadIdx.x; t < T; t += gridDim.x * THREADS) {
+    float v = d[t + padL];
+    if (fold_l && t >= 1 && t <= padL) v += d[padL - t];                           // left mirror
+    if (fold_r && t >= T - 1 - padR && t <= T - 2) v += d[padL + 2 * (T - 1) - t]; // right mirror
+    if constexpr (ACC) o[t] += v;
+    else o[t] = v;
+  }
+}
+
 __global__ void __launch_bounds__(THREADS)
 reflect_fold_wave_kernel(const float* __restrict__ dpad, long pitch, float* __restrict__ dx, int T,
                          int padL, int padR) {
   pdl_wait();
   const int n = blockIdx.y;
-  const float* d = dpad + (long)n * pitch;
-  for (int t = blockIdx.x * THREADS + threadIdx.x; t < T; t += gridDim.x * THREADS) {
-    float v = d[t + padL];
-    if (t >= 1 && t <= padL) v += d[padL - t];                               // left mirror
-    if (t >= T - 1 - padR && t <= T - 2) v += d[padL + 2 * (T - 1) - t];     // right mirror
-    dx[(long)n * T + t] = v;
-  }
+  reflect_fold_wave_utt<false>(dpad + (long)n * pitch, dx + (long)n * T, T, padL, padR, true,
+                               true);
 }
 
 // pase_reflect_fold_wave for utterance blockIdx.y of a packed waveform: tab row {x_off, T, dst_off}
@@ -76,31 +86,17 @@ reflect_fold_wave_var_kernel(const float* __restrict__ dpad, const int* __restri
                              float* __restrict__ dx, int padL, int padR) {
   pdl_wait();
   const int* r = tab + 3 * blockIdx.y;
-  const int T = __ldg(r + 1);
-  const float* d = dpad + __ldg(r + 2);
-  float* o = dx + __ldg(r);
-  for (int t = blockIdx.x * THREADS + threadIdx.x; t < T; t += gridDim.x * THREADS) {
-    float v = d[t + padL];
-    if (t >= 1 && t <= padL) v += d[padL - t];                               // left mirror
-    if (t >= T - 1 - padR && t <= T - 2) v += d[padL + 2 * (T - 1) - t];     // right mirror
-    o[t] = v;
-  }
+  reflect_fold_wave_utt<false>(dpad + __ldg(r + 2), dx + __ldg(r), __ldg(r + 1), padL, padR, true,
+                               true);
 }
 
 // One window of a recording (WaveFe.encode_long): dx[x0 + t] += the window's padded-waveform
-// gradient at t, with the mirrored pad gradient added only on the sides where the window's pad is
-// the recording's own (fold_l / fold_r)
+// gradient at t, folding the pad only on the sides where the window's pad is the recording's own
 __global__ void __launch_bounds__(THREADS)
 reflect_fold_wave_acc_kernel(const float* __restrict__ d, float* __restrict__ dx, long x0, int T,
                              int padL, int padR, int fold_l, int fold_r) {
   pdl_wait();
-  float* o = dx + x0;
-  for (int t = blockIdx.x * THREADS + threadIdx.x; t < T; t += gridDim.x * THREADS) {
-    float v = d[t + padL];
-    if (fold_l && t >= 1 && t <= padL) v += d[padL - t];                           // left mirror
-    if (fold_r && t >= T - 1 - padR && t <= T - 2) v += d[padL + 2 * (T - 1) - t]; // right mirror
-    o[t] += v;
-  }
+  reflect_fold_wave_utt<true>(d, dx + x0, T, padL, padR, fold_l, fold_r);
 }
 
 inline unsigned grid_for(long total) {

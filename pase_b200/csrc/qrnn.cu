@@ -79,12 +79,10 @@ qrnn_scan_fwd_carry_var_kernel(const float* __restrict__ Y, float* __restrict__ 
 
 // One sample's sequential backward scan of hidden unit c over its T steps, last to first: y /
 // cp / dhp / dy point at its first step, cm0 is the cell state before it and carry the cell-state
-// gradient entering from after its last step.  Returns the gradient of cm0.  The per-step
-// arithmetic is that of qrnn_scan_bwd_kernel and qrnn_scan_bwd_seq_var_kernel below (whose cm0
-// and carry are 0), in an unrolled group or in the remainder alike, so a backward cut into
-// windows that carry the gradient reproduces the whole scan's bits (pase_qrnn_scan_bwd_carry_var).
-// Those two kernels keep their own copies of the loop: routing them through this function
-// changes their SASS.
+// gradient entering from after its last step (both 0 for a whole utterance).  Returns the
+// gradient of cm0.  Every step runs the same arithmetic whether it falls in an unrolled group or
+// in the remainder, so a backward cut into windows that carry the gradient reproduces the whole
+// scan's bits (pase_qrnn_scan_bwd_carry_var).
 __device__ __forceinline__ float qrnn_bwd_seq(const float* __restrict__ y,
                                               const float* __restrict__ cp,
                                               const float* __restrict__ dhp, long lddh,
@@ -137,51 +135,11 @@ qrnn_scan_bwd_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
                      int H) {
   pdl_wait();
   const int n = blockIdx.y;
+  const long row0 = (long)n * T;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= H) return;
-  const float* y = Y + (long)n * T * 3 * H + c;
-  const float* cp = Cst + (long)n * T * H + c;
-  const float* dhp = dh + (long)n * T * lddh + c;
-  float* dy = dY + (long)n * T * 3 * H + c;
-  float carry = 0.f;
-  int t = T - 1;
-  // the loads do not depend on the recurrence: issue UNROLL time steps of them up front
-  for (; t - (UNROLL - 1) >= 0; t -= UNROLL) {
-    float z[UNROLL], f[UNROLL], o[UNROLL], c[UNROLL], cm[UNROLL], g[UNROLL];
-#pragma unroll
-    for (int i = 0; i < UNROLL; ++i) {
-      const int tt = t - i;
-      const float* yr = y + (long)tt * 3 * H;
-      z[i] = yr[0]; f[i] = yr[H]; o[i] = yr[2 * H];
-      c[i] = cp[(long)tt * H];
-      cm[i] = tt > 0 ? cp[(long)(tt - 1) * H] : 0.f;
-      g[i] = dhp[(long)tt * lddh];
-    }
-#pragma unroll
-    for (int i = 0; i < UNROLL; ++i) {
-      const int tt = t - i;
-      const float zz = tanhf(z[i]), ff = sigmoidf_(f[i]), oo = sigmoidf_(o[i]);
-      const float dc = g[i] * oo + carry;
-      carry = dc * (1.f - ff);
-      float* dr = dy + (long)tt * 3 * H;
-      dr[0] = dc * ff * (1.f - zz * zz);
-      dr[H] = dc * (zz - cm[i]) * ff * (1.f - ff);
-      dr[2 * H] = g[i] * c[i] * oo * (1.f - oo);
-    }
-  }
-  for (; t >= 0; --t) {
-    const float* yr = y + (long)t * 3 * H;
-    const float zz = tanhf(yr[0]), ff = sigmoidf_(yr[H]), oo = sigmoidf_(yr[2 * H]);
-    const float ct = cp[(long)t * H];
-    const float cm1 = t > 0 ? cp[(long)(t - 1) * H] : 0.f;
-    const float g = dhp[(long)t * lddh];
-    const float dc = g * oo + carry;
-    carry = dc * (1.f - ff);
-    float* dr = dy + (long)t * 3 * H;
-    dr[0] = dc * ff * (1.f - zz * zz);
-    dr[H] = dc * (zz - cm1) * ff * (1.f - ff);
-    dr[2 * H] = g * ct * oo * (1.f - oo);
-  }
+  qrnn_bwd_seq(Y + row0 * 3 * H + c, Cst + row0 * H + c, dh + row0 * lddh + c, lddh,
+               dY + row0 * 3 * H + c, T, H, 0.f, 0.f);
 }
 
 // ---- time-segmented scans ----
@@ -254,22 +212,23 @@ qrnn_scan_fwd_seg_kernel(const float* __restrict__ Y, float* __restrict__ h, lon
   qrnn_fwd_seg(Y, h, ldh, Cst, (long)blockIdx.y * T, T, H, sA, sB);
 }
 
-template <int NSEG_MAX>
-__global__ void __launch_bounds__(32 * NSEG_MAX, 1)
-qrnn_scan_bwd_seg_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
-                         const float* __restrict__ dh, long lddh, float* __restrict__ dY, int T,
-                         int H) {
-  pdl_wait();
-  __shared__ float sA[MAX_SEGS][33], sB[MAX_SEGS][33];
-  const int lane = threadIdx.x, seg = threadIdx.y, n = blockIdx.y, nseg = blockDim.y;
+// One sample's segmented backward: rows row0 .. row0+T-1 of Y / Cst / dh, gate gradients to rows
+// drow0 .. drow0+T-1 of dY; segment threadIdx.y of blockDim.y.  Segments past the end scan
+// nothing and pass the carry through.
+__device__ __forceinline__ void qrnn_bwd_seg(const float* __restrict__ Y,
+                                             const float* __restrict__ Cst,
+                                             const float* __restrict__ dh, long lddh,
+                                             float* __restrict__ dY, long row0, long drow0, int T,
+                                             int H, float (*sA)[33], float (*sB)[33]) {
+  const int lane = threadIdx.x, seg = threadIdx.y, nseg = blockDim.y;
   const int c = blockIdx.x * 32 + lane;
   const bool live = c < H;
   const int t0 = seg * SEG;
   const int len = (T - t0) < SEG ? (T - t0) : SEG;
-  const float* y = Y + ((long)n * T + t0) * 3 * H + c;
-  const float* cp = Cst + ((long)n * T + t0) * H + c;
-  const float* dhp = dh + ((long)n * T + t0) * lddh + c;
-  float* dy = dY + ((long)n * T + t0) * 3 * H + c;
+  const float* y = Y + (row0 + t0) * 3 * H + c;
+  const float* cp = Cst + (row0 + t0) * H + c;
+  const float* dhp = dh + (row0 + t0) * lddh + c;
+  float* dy = dY + (drow0 + t0) * 3 * H + c;
   float z[SEG], f[SEG], o[SEG], cs[SEG], g[SEG];
 #pragma unroll
   for (int i = 0; i < SEG; ++i) {
@@ -281,7 +240,7 @@ qrnn_scan_bwd_seg_kernel(const float* __restrict__ Y, const float* __restrict__ 
     cs[i] = ok ? cp[(long)i * H] : 0.f;
     g[i] = ok ? dhp[(long)i * lddh] : 0.f;
   }
-  const float cm0 = (live && t0 > 0) ? cp[-(long)H] : 0.f;       // c_{t0-1}
+  const float cm0 = (live && t0 > 0 && len > 0) ? cp[-(long)H] : 0.f;       // c_{t0-1}
   // right-to-left local scan with zero incoming carry; z[] / f[] are overwritten by the
   // coefficients of the correction pass (dz = dc kz, df = dc kf), cs[] / o[] by (local dc, Q)
   float carry = 0.f, Q = 1.f;
@@ -316,6 +275,18 @@ qrnn_scan_bwd_seg_kernel(const float* __restrict__ Y, const float* __restrict__ 
       dy[(long)i * 3 * H + H] = dc * f[i];
     }
   }
+}
+
+template <int NSEG_MAX>
+__global__ void __launch_bounds__(32 * NSEG_MAX, 1)
+qrnn_scan_bwd_seg_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
+                         const float* __restrict__ dh, long lddh, float* __restrict__ dY, int T,
+                         int H) {
+  pdl_wait();
+  __shared__ float sA[MAX_SEGS][33], sB[MAX_SEGS][33];
+  const int n = blockIdx.y;
+  const long row0 = (long)n * T;
+  qrnn_bwd_seg(Y, Cst, dh, lddh, dY, row0, row0, T, H, sA, sB);
 }
 
 // Segments per block of the time-segmented kernels for T time steps (the template width: 16,
@@ -353,8 +324,8 @@ qrnn_scan_fwd_seq_var_kernel(const float* __restrict__ Y, float* __restrict__ h,
 // Packed variable-length backward: blockIdx.y = utterance, tab row {row0, T, drow0}: rows row0 ..
 // row0+T-1 of Y / Cst / dh are one utterance, its gate gradients go to rows drow0 .. drow0+T-1
 // of dY and row drow0+T of dY is written zero (the QRNN input's rows, one separator row per
-// utterance: DESIGN.md section 18).  As in the forward, each utterance runs the kernel its own T
-// selects, with the arithmetic of qrnn_scan_bwd_seg_kernel / qrnn_scan_bwd_kernel.
+// utterance: DESIGN.md section 18).  As in the forward, each utterance runs the body its own T
+// selects (qrnn_bwd_seg or qrnn_bwd_seq).
 __global__ void __launch_bounds__(32 * MAX_SEGS, 1)
 qrnn_scan_bwd_seg_var_kernel(const float* __restrict__ Y, const float* __restrict__ Cst,
                              const float* __restrict__ dh, long lddh, float* __restrict__ dY,
@@ -365,63 +336,12 @@ qrnn_scan_bwd_seg_var_kernel(const float* __restrict__ Y, const float* __restric
   const int T = __ldg(r + 1);
   if (T > SEG * MAX_SEGS) return;
   const long row0 = __ldg(r), drow0 = __ldg(r + 2);
-  const int lane = threadIdx.x, seg = threadIdx.y, nseg = blockDim.y;
-  const int c = blockIdx.x * 32 + lane;
-  const bool live = c < H;
-  if (live && seg == 0) {
+  const int c = blockIdx.x * 32 + threadIdx.x;
+  if (c < H && threadIdx.y == 0) {
     float* zr = dY + (drow0 + T) * 3 * H + c;
     zr[0] = 0.f; zr[H] = 0.f; zr[2 * H] = 0.f;
   }
-  const int t0 = seg * SEG;
-  const int len = (T - t0) < SEG ? (T - t0) : SEG;
-  const float* y = Y + (row0 + t0) * 3 * H + c;
-  const float* cp = Cst + (row0 + t0) * H + c;
-  const float* dhp = dh + (row0 + t0) * lddh + c;
-  float* dy = dY + (drow0 + t0) * 3 * H + c;
-  float z[SEG], f[SEG], o[SEG], cs[SEG], g[SEG];
-#pragma unroll
-  for (int i = 0; i < SEG; ++i) {
-    const bool ok = live && i < len;
-    const float* yr = y + (long)i * 3 * H;
-    z[i] = ok ? yr[0] : 0.f;
-    f[i] = ok ? yr[H] : 0.f;
-    o[i] = ok ? yr[2 * H] : 0.f;
-    cs[i] = ok ? cp[(long)i * H] : 0.f;
-    g[i] = ok ? dhp[(long)i * lddh] : 0.f;
-  }
-  const float cm0 = (live && t0 > 0 && len > 0) ? cp[-(long)H] : 0.f;
-  float carry = 0.f, Q = 1.f;
-#pragma unroll
-  for (int i = SEG - 1; i >= 0; --i) {
-    const float zz = tanhf(z[i]), ff = sigmoidf_(f[i]), oo = sigmoidf_(o[i]);
-    const float cm = i > 0 ? cs[i - 1] : cm0;
-    const float ct = cs[i];
-    const bool in = i < len;
-    const float dc = in ? fmaf(g[i], oo, carry) : 0.f;
-    if (live && in) dy[(long)i * 3 * H + 2 * H] = g[i] * ct * oo * (1.f - oo);
-    z[i] = ff * (1.f - zz * zz);
-    f[i] = (zz - cm) * ff * (1.f - ff);
-    cs[i] = dc;
-    o[i] = Q;
-    if (in) {
-      carry = dc * (1.f - ff);
-      Q *= (1.f - ff);
-    }
-  }
-  sA[seg][lane] = Q;
-  sB[seg][lane] = carry;
-  __syncthreads();
-  float kin = 0.f;
-  for (int s2 = nseg - 1; s2 > seg; --s2) kin = sA[s2][lane] * kin + sB[s2][lane];
-  if (!live) return;
-#pragma unroll
-  for (int i = 0; i < SEG; ++i) {
-    if (i < len) {
-      const float dc = fmaf(o[i], kin, cs[i]);
-      dy[(long)i * 3 * H] = dc * z[i];
-      dy[(long)i * 3 * H + H] = dc * f[i];
-    }
-  }
+  qrnn_bwd_seg(Y, Cst, dh, lddh, dY, row0, drow0, T, H, sA, sB);
 }
 
 __global__ void __launch_bounds__(128)
@@ -434,49 +354,10 @@ qrnn_scan_bwd_seq_var_kernel(const float* __restrict__ Y, const float* __restric
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (T <= SEG * MAX_SEGS || c >= H) return;
   const long row0 = __ldg(r), drow0 = __ldg(r + 2);
-  const float* y = Y + row0 * 3 * H + c;
-  const float* cp = Cst + row0 * H + c;
-  const float* dhp = dh + row0 * lddh + c;
   float* dy = dY + drow0 * 3 * H + c;
+  qrnn_bwd_seq(Y + row0 * 3 * H + c, Cst + row0 * H + c, dh + row0 * lddh + c, lddh, dy, T, H,
+               0.f, 0.f);
   dy[(long)T * 3 * H] = 0.f; dy[(long)T * 3 * H + H] = 0.f; dy[(long)T * 3 * H + 2 * H] = 0.f;
-  float carry = 0.f;
-  int t = T - 1;
-  for (; t - (UNROLL - 1) >= 0; t -= UNROLL) {
-    float z[UNROLL], f[UNROLL], o[UNROLL], c[UNROLL], cm[UNROLL], g[UNROLL];
-#pragma unroll
-    for (int i = 0; i < UNROLL; ++i) {
-      const int tt = t - i;
-      const float* yr = y + (long)tt * 3 * H;
-      z[i] = yr[0]; f[i] = yr[H]; o[i] = yr[2 * H];
-      c[i] = cp[(long)tt * H];
-      cm[i] = tt > 0 ? cp[(long)(tt - 1) * H] : 0.f;
-      g[i] = dhp[(long)tt * lddh];
-    }
-#pragma unroll
-    for (int i = 0; i < UNROLL; ++i) {
-      const int tt = t - i;
-      const float zz = tanhf(z[i]), ff = sigmoidf_(f[i]), oo = sigmoidf_(o[i]);
-      const float dc = g[i] * oo + carry;
-      carry = dc * (1.f - ff);
-      float* dr = dy + (long)tt * 3 * H;
-      dr[0] = dc * ff * (1.f - zz * zz);
-      dr[H] = dc * (zz - cm[i]) * ff * (1.f - ff);
-      dr[2 * H] = g[i] * c[i] * oo * (1.f - oo);
-    }
-  }
-  for (; t >= 0; --t) {
-    const float* yr = y + (long)t * 3 * H;
-    const float zz = tanhf(yr[0]), ff = sigmoidf_(yr[H]), oo = sigmoidf_(yr[2 * H]);
-    const float ct = cp[(long)t * H];
-    const float cm1 = t > 0 ? cp[(long)(t - 1) * H] : 0.f;
-    const float g = dhp[(long)t * lddh];
-    const float dc = g * oo + carry;
-    carry = dc * (1.f - ff);
-    float* dr = dy + (long)t * 3 * H;
-    dr[0] = dc * ff * (1.f - zz * zz);
-    dr[H] = dc * (zz - cm1) * ff * (1.f - ff);
-    dr[2 * H] = g * ct * oo * (1.f - oo);
-  }
 }
 
 // Backward of one window's carried scan (WaveFe.encode_long): tab row {row0, T, drow0, c0, cn,
@@ -508,6 +389,23 @@ qrnn_scan_bwd_carry_var_kernel(const float* __restrict__ Y, const float* __restr
                      state[slot * H + c], *ds);
 }
 
+// Launches a uniform (N, T) scan: seg16 / seg24 / seg32, the time-segmented kernel of the width
+// seg_width(T) selects, with one (32, ceil(T/SEG)) block per 32 hidden units and sample, or seq,
+// the sequential kernel, with one thread per hidden unit and sample when T is longer.
+template <typename... KArgs, typename... Args>
+int launch_scan(const char* name, void (*seg16)(KArgs...), void (*seg24)(KArgs...),
+                void (*seg32)(KArgs...), void (*seq)(KArgs...), int N, int T, int H,
+                cudaStream_t st, Args... args) {
+  const int width = seg_width(T);
+  if (width)
+    PASE_LAUNCH(width == 16 ? seg16 : width == 24 ? seg24 : seg32, dim3((H + 31) / 32, N),
+                dim3(32, (T + SEG - 1) / SEG), 0, st, args...);
+  else
+    PASE_LAUNCH(seq, dim3((H + 127) / 128, N), 128, 0, st, args...);
+  PASE_LAUNCH_CHECK(name);
+  return PASE_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -532,24 +430,9 @@ int pase_qrnn_scan_fwd(const float* Y, float* h, long ldh, float* Cst, int N, in
   PASE_CHECK_ARG(Y && h && Cst, "pase_qrnn_scan_fwd: null pointer");
   PASE_CHECK_ARG(N > 0 && T > 0 && H > 0, "pase_qrnn_scan_fwd: N=%d T=%d H=%d", N, T, H);
   PASE_CHECK_ARG(ldh >= H, "pase_qrnn_scan_fwd: ldh=%ld < H=%d", ldh, H);
-  const int nseg = (T + SEG - 1) / SEG, width = seg_width(T);
-  if (width) {
-    if (width == 16)
-      PASE_LAUNCH((qrnn_scan_fwd_seg_kernel<16>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
-                  (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
-    else if (width == 24)
-      PASE_LAUNCH((qrnn_scan_fwd_seg_kernel<24>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
-                  (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
-    else
-      PASE_LAUNCH((qrnn_scan_fwd_seg_kernel<MAX_SEGS>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
-                  (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
-    PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd");
-    return PASE_OK;
-  }
-  dim3 grid((H + 127) / 128, N);
-  PASE_LAUNCH((qrnn_scan_fwd_kernel), grid, 128, 0, (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
-  PASE_LAUNCH_CHECK("pase_qrnn_scan_fwd");
-  return PASE_OK;
+  return launch_scan("pase_qrnn_scan_fwd", qrnn_scan_fwd_seg_kernel<16>,
+                     qrnn_scan_fwd_seg_kernel<24>, qrnn_scan_fwd_seg_kernel<MAX_SEGS>,
+                     qrnn_scan_fwd_kernel, N, T, H, (cudaStream_t)stream, Y, h, ldh, Cst, T, H);
 }
 
 int pase_qrnn_scan_fwd_carry_var(const float* Y, float* h, long ldh, float* Cst, float* state,
@@ -568,24 +451,10 @@ int pase_qrnn_scan_bwd(const float* Y, const float* Cst, const float* dh, long l
   PASE_CHECK_ARG(Y && Cst && dh && dY, "pase_qrnn_scan_bwd: null pointer");
   PASE_CHECK_ARG(N > 0 && T > 0 && H > 0, "pase_qrnn_scan_bwd: N=%d T=%d H=%d", N, T, H);
   PASE_CHECK_ARG(lddh >= H, "pase_qrnn_scan_bwd: lddh=%ld < H=%d", lddh, H);
-  const int nseg = (T + SEG - 1) / SEG, width = seg_width(T);
-  if (width) {
-    if (width == 16)
-      PASE_LAUNCH((qrnn_scan_bwd_seg_kernel<16>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
-                  (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
-    else if (width == 24)
-      PASE_LAUNCH((qrnn_scan_bwd_seg_kernel<24>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
-                  (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
-    else
-      PASE_LAUNCH((qrnn_scan_bwd_seg_kernel<MAX_SEGS>), dim3((H + 31) / 32, N), dim3(32, nseg), 0,
-                  (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
-    PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd");
-    return PASE_OK;
-  }
-  dim3 grid((H + 127) / 128, N);
-  PASE_LAUNCH((qrnn_scan_bwd_kernel), grid, 128, 0, (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T, H);
-  PASE_LAUNCH_CHECK("pase_qrnn_scan_bwd");
-  return PASE_OK;
+  return launch_scan("pase_qrnn_scan_bwd", qrnn_scan_bwd_seg_kernel<16>,
+                     qrnn_scan_bwd_seg_kernel<24>, qrnn_scan_bwd_seg_kernel<MAX_SEGS>,
+                     qrnn_scan_bwd_kernel, N, T, H, (cudaStream_t)stream, Y, Cst, dh, lddh, dY, T,
+                     H);
 }
 
 int pase_qrnn_scan_bwd_var(const float* Y, const float* Cst, const float* dh, long lddh, float* dY,
