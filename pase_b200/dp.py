@@ -25,9 +25,21 @@ def broadcast_parameters_and_buffers(module, src=0, group=None):
     (BatchNorm running statistics, step counters) of rank `src` overwrite the others'.
     Afterwards BatchNorm buffers evolve per rank (exactly N independent reference runs, the
     reference has no SyncBN); checkpoint rank 0's."""
+    _broadcast_in_place([p.data for p in module.parameters()] +
+                        [b.data for b in module.buffers()], src, group)
+
+
+def broadcast_buffers(module, src=0, group=None):
+    """Rank `src`'s buffers (BatchNorm running statistics, step counters) into every rank's, in
+    place: CUDA graphs that read them by address see the new values (what DDP's
+    ``broadcast_buffers`` gives before a forward)."""
+    _broadcast_in_place([b.data for b in module.buffers()], src, group)
+
+
+def _broadcast_in_place(tensors, src, group):
+    """One broadcast per (dtype, device) of the concatenated tensors, copied back into them."""
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
         return
-    tensors = [p.data for p in module.parameters()] + [b.data for b in module.buffers()]
     by_dtype = {}
     for t in tensors:
         by_dtype.setdefault((t.dtype, t.device), []).append(t)

@@ -181,6 +181,25 @@ class TrainPlanner(object):
         return plan, np.concatenate([plan.table, np.asarray(frames, dtype=np.int64)])
 
 
+def _world(group):
+    """Ranks of `group` (None: no data parallelism, 1)."""
+    if group is None:
+        return 1
+    import torch.distributed as dist
+    return dist.get_world_size(group)
+
+
+def _all_gather(t, group, device):
+    """Every rank's CPU tensor `t` (one shape on all ranks), in rank order, as CPU tensors.  It
+    travels on `device` unless the group's backend is gloo alone."""
+    import torch.distributed as dist
+    if dist.get_backend(group) != "gloo":
+        t = t.to(device)
+    parts = [torch.empty_like(t) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(parts, t.contiguous(), group=group)
+    return [p.cpu() for p in parts]
+
+
 class GraphedTrainStep(object):
     """One PASE/PASE+ training step from a resident corpus as one CUDA-graph replay: batch
     assembly (``DeviceBatcher``), the encoder, every worker head and its loss, the summed
@@ -201,9 +220,21 @@ class GraphedTrainStep(object):
     take effect at the next step.  The step runs on its own stream; each call orders the caller's
     current stream after it (and the step after the caller's earlier work), so eager work the
     caller queues between calls, such as a validation pass or a checkpoint, sees the finished
-    step without a host synchronise."""
+    step without a host synchronise.
 
-    def __init__(self, model, engine, batcher, batch_size, warmup=3, stream=None):
+    Data parallelism (``group``: a ``torch.distributed`` process group of W > 1 ranks, one
+    process per GPU of one node): each rank builds its own step over its own replica, engine,
+    batcher and batches of B, and a step on rank r is the step above on rank r's batch with the
+    update on the mean over ranks of the flat gradient.  With ``FlatAdam(peer_dp=True)`` over
+    the same group the step stays one replay: ``pase_adam_flat_dp`` averages the gradients and
+    stores the same new parameters into every rank's buffer inside it.  With a plain
+    ``FlatAdam`` the step is two replays, [batch, forward, losses, backward] and [update, loss
+    copy], with ``engine.reduce_grads(group)`` run eagerly on the step stream between them; no
+    collective is captured.  Every rank must be built with the same ``warmup`` and called in
+    lockstep, the same number of times: a rank that skips a step leaves its peers waiting in
+    the update.  ``losses()`` is then collective too."""
+
+    def __init__(self, model, engine, batcher, batch_size, warmup=3, stream=None, group=None):
         from .optim import FlatAdam
         if int(warmup) < 1:
             raise ValueError("GraphedTrainStep: warmup=%d; at least one eager step builds the "
@@ -214,8 +245,16 @@ class GraphedTrainStep(object):
             raise TypeError("GraphedTrainStep: the engine must be a FlatAdam, got %s"
                             % type(engine).__name__)
         if engine.peer_dp:
-            raise NotImplementedError("GraphedTrainStep: FlatAdam(peer_dp=True) is not supported; "
-                                      "data-parallel steps are not captured here")
+            if group is None:
+                raise NotImplementedError("GraphedTrainStep: a FlatAdam(peer_dp=True) engine "
+                                          "needs group=, the process group it was built over")
+            import torch.distributed as dist
+
+            def resolved(g):
+                return dist.group.WORLD if g is None else g
+            if resolved(engine._group) is not resolved(group):
+                raise ValueError("GraphedTrainStep: the FlatAdam(peer_dp=True) engine was built "
+                                 "over another process group than `group`")
         sunk = {id(p) for _, p in model.frontend.named_parameters() if p.requires_grad}
         if getattr(model.frontend, "grad_sink", None) is None or engine._sunk != sunk:
             raise ValueError("GraphedTrainStep: call engine.bind_encoder(model.frontend) first")
@@ -228,6 +267,9 @@ class GraphedTrainStep(object):
         self.model, self.engine, self.batcher = model, engine, batcher
         self.B, self.warmup = int(batch_size), int(warmup)
         self.device = params[0].device
+        self.group, self.world = group, _world(group)
+        # a plain engine averages the gradients with a collective between two graphs
+        self.split = self.world > 1 and engine._peer is None
         # total_loss's order: classification workers, then regression workers
         self.names = ["total"] + [w.name for w in list(model.classification_workers) +
                                   list(model.regression_workers)]
@@ -235,7 +277,8 @@ class GraphedTrainStep(object):
         self.loss_host = torch.zeros(len(self.names), dtype=torch.float32).pin_memory()
         self.done = torch.cuda.Event()
         self.table = None                 # the graph's static plan table, sized by the first plan
-        self.graph = None
+        self.graph = self.graph_b = None
+        self._vec = None
         self._plans = []
         self.calls = 0
         self._k = 0
@@ -246,8 +289,8 @@ class GraphedTrainStep(object):
         self._stage = [torch.zeros(n, dtype=torch.int64).pin_memory() for _ in (0, 1)]
         self._staged = [torch.cuda.Event(), torch.cuda.Event()]
 
-    def _run(self):
-        """The step as it is captured: everything reads the static table."""
+    def _forward_backward(self):
+        """The step's first part as it is captured: everything reads the static table."""
         from .pase import total_loss
         eng, model = self.engine, self.model
         nb = self.table.numel() - 3 * len(self.planner.spc)
@@ -261,10 +304,43 @@ class GraphedTrainStep(object):
             for m in self.planner.spc:
                 m.frame_table = None
         tot, losses = total_loss(model, preds, labels)
-        vec = torch.stack([tot.detach()] + [losses[n].detach() for n in self.names[1:]])
+        self._vec = torch.stack([tot.detach()] + [losses[n].detach() for n in self.names[1:]])
         tot.backward()
-        eng.step()
-        self.loss_host.copy_(vec, non_blocking=True)
+        if self.split:
+            # the heads' gradients into the flat buffer inside the graph, so the eager
+            # all-reduce after it reads this replay's gradients
+            eng.pack_grads()
+
+    def _update(self):
+        self.engine.step()
+        self.loss_host.copy_(self._vec, non_blocking=True)
+
+    def _run(self):
+        self._forward_backward()
+        if self.split:
+            self.engine.reduce_grads(self.group)
+        self._update()
+
+    def _capture(self):
+        # "thread_local": a process group's watchdog thread may query CUDA during the capture
+        mode = "thread_local" if self.world > 1 else "global"
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=self.stream, capture_error_mode=mode):
+            if self.split:
+                self._forward_backward()
+            else:
+                self._run()
+        if self.split:
+            gb = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(gb, stream=self.stream, pool=g.pool(), capture_error_mode=mode):
+                self._update()
+            self.graph_b = gb
+        self.graph = g
+        # the graph holds raw addresses of the encoder's and decoders' plan buffers; keep those
+        # plans alive when their caches evict them (other shapes run eagerly between replays,
+        # e.g. validation batches)
+        self._plans = [p for m in self.model.modules()
+                       for p in getattr(m, "_plans", {}).values()]
 
     def __call__(self, indices, rng=None):
         indices = [int(i) for i in indices]
@@ -289,16 +365,11 @@ class GraphedTrainStep(object):
                 self._run()
             else:
                 if self.graph is None:
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, stream=self.stream):
-                        self._run()
-                    self.graph = g
-                    # the graph holds raw addresses of the encoder's and decoders' plan buffers;
-                    # keep those plans alive when their caches evict them (other shapes run
-                    # eagerly between replays, e.g. validation batches)
-                    self._plans = [p for m in self.model.modules()
-                                   for p in getattr(m, "_plans", {}).values()]
+                    self._capture()
                 self.graph.replay()
+                if self.split:
+                    self.engine.reduce_grads(self.group)
+                    self.graph_b.replay()
             self.done.record(self.stream)
         # work the caller queues next (an eager validation pass, reading or saving parameters)
         # runs after this step on the device; the host does not wait
@@ -308,11 +379,17 @@ class GraphedTrainStep(object):
 
     def losses(self):
         """{'total': ..., worker name: ...} (python floats, each worker's loss times its
-        loss_weight) of the last step issued; waits for that step only."""
+        loss_weight) of the last step issued; waits for that step only.  With a process group,
+        each entry is the mean over ranks (summed in rank order), i.e. the loss of the global
+        batch; collective: every rank calls it after the same steps."""
         if self.calls == 0:
             raise RuntimeError("GraphedTrainStep.losses: no step has run yet")
         self.done.synchronize()
-        return dict(zip(self.names, self.loss_host.tolist()))
+        vals = self.loss_host.tolist()
+        if self.world > 1:
+            rows = [r.tolist() for r in _all_gather(self.loss_host, self.group, self.device)]
+            vals = [sum(r[j] for r in rows) / self.world for j in range(len(vals))]
+        return dict(zip(self.names, vals))
 
 
 class GraphedEvalStep(object):
@@ -345,9 +422,16 @@ class GraphedEvalStep(object):
     capture.  A ``GraphedTrainStep`` at the same batch size shares the (3B, T) encoder plan
     with it: both graphs write its buffers, which is safe because each call is ordered after
     the caller's earlier work and the caller after it, so the two never run at once.  The first
-    `warmup` calls run eagerly through the code that is captured."""
+    `warmup` calls run eagerly through the code that is captured.
 
-    def __init__(self, model, batcher, batch_size, max_batches=None, warmup=3, stream=None):
+    Data parallelism (``group``: a process group of W > 1 ranks, as for ``GraphedTrainStep``):
+    each rank replays its own shard of the validation batches.  The first call of a pass (after
+    construction or ``reset()``) first broadcasts rank 0's buffers, the BatchNorm running
+    statistics, in place into every rank's, so every rank evaluates the model rank 0 would
+    save.  ``losses()`` is collective and returns every rank's rows, rank-major."""
+
+    def __init__(self, model, batcher, batch_size, max_batches=None, warmup=3, stream=None,
+                 group=None):
         if int(warmup) < 1:
             raise ValueError("GraphedEvalStep: warmup=%d; at least one eager batch builds the "
                              "constants and buffers the capture reads" % warmup)
@@ -365,6 +449,7 @@ class GraphedEvalStep(object):
         self.model, self.batcher = model, batcher
         self.max_batches = int(max_batches)
         self.device = params[0].device
+        self.group, self.world = group, _world(group)
         # running_loss's order (trainer.py:306-326)
         self.names = [w.name for w in list(model.classification_workers) +
                       list(model.regression_workers)] + ["total"]
@@ -425,6 +510,12 @@ class GraphedEvalStep(object):
         elif table.size != self.table.numel():
             raise RuntimeError("GraphedEvalStep: the plan has %d entries, the captured pass %d"
                                % (table.size, self.table.numel()))
+        if self.world > 1 and self.k == 0:
+            # on the caller's stream, which the replay below waits for
+            from .dp import broadcast_buffers
+            import torch.distributed as dist
+            broadcast_buffers(self.model, src=dist.get_global_rank(self.group, 0),
+                              group=self.group)
         k = self._k
         self._staged[k].synchronize()          # the copy that last read this buffer has run
         self._stage[k].numpy()[:] = table
@@ -437,7 +528,8 @@ class GraphedEvalStep(object):
             else:
                 if self.graph is None:
                     g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, stream=self.stream):
+                    mode = "thread_local" if self.world > 1 else "global"
+                    with torch.cuda.graph(g, stream=self.stream, capture_error_mode=mode):
                         self._run()
                     self.graph = g
                     self._plans = [p for m in self.model.modules()
@@ -451,7 +543,9 @@ class GraphedEvalStep(object):
 
     def losses(self):
         """{worker name: [loss of batch 0, 1, ...], ..., 'total': [...]} (python floats) of the
-        batches of the current pass; one device-to-host copy, waits for the pass only."""
+        batches of the current pass; one device-to-host copy, waits for the pass only.  With a
+        process group: rank 0's batches, then rank 1's, ...; collective, and it raises on every
+        rank when the ranks ran different numbers of batches in the pass."""
         n = self.k
         self.stream.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(self.stream):
@@ -459,6 +553,15 @@ class GraphedEvalStep(object):
             self.done.record(self.stream)
         self.done.synchronize()
         rows = self.out_host[:n].tolist()
+        if self.world > 1:
+            counts = [int(c) for c in _all_gather(torch.tensor([n], dtype=torch.int64),
+                                                  self.group, self.device)]
+            if len(set(counts)) > 1:
+                raise RuntimeError("GraphedEvalStep.losses: the ranks ran %s batches in this "
+                                   "pass; every rank must run the same number" % counts)
+            if n:
+                rows = [r for part in _all_gather(self.out_host[:n].clone(), self.group,
+                                                  self.device) for r in part.tolist()]
         return {name: [r[j] for r in rows] for j, name in enumerate(self.names)}
 
     def reset(self):

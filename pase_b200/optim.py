@@ -80,6 +80,7 @@ class FlatAdam(torch.optim.Optimizer):
         f32 = dict(dtype=torch.float32, device=dev)
         self.peer_dp = bool(peer_dp)
         self._peer = None
+        self._group = group
         if peer_dp:
             import torch.distributed as dist
             if not (dist.is_available() and dist.is_initialized()):
@@ -94,7 +95,6 @@ class FlatAdam(torch.optim.Optimizer):
                           "flag": PeerAlloc(2 * world, torch.int32, dev)}
                 self._peer = PeerGroup(allocs, group)
                 self._peer_sync = torch.zeros(2, dtype=torch.int32, device=dev)   # epoch, done
-                self._group = group
         if self._peer is not None:
             self.flat_param = self._peer.allocs["param"].tensor
             self.flat_grad = self._peer.allocs["grad"].tensor
