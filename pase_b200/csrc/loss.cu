@@ -103,8 +103,9 @@ bce_pairs_fwd_kernel(const float* __restrict__ x, long n, long n_pos, double* ac
        i += (long)gridDim.x * blockDim.x) {
     const float v = x[i];
     const float y = i < n_pos ? 1.f : 0.f;
-    const float mx = fmaxf(-v, 0.f);
-    s += (double)((1.f - y) * v + mx + logf(expf(-mx) + expf(-v - mx)));
+    // max(v, 0) - v y + log(1 + e^-|v|): for a confident logit the first two terms cancel
+    // exactly and log1pf keeps the e^-|v| that log(1 + e^-|v|) rounds away above |v| ~ 17
+    s += (double)(fmaxf(v, 0.f) - v * y + log1pf(expf(-fabsf(v))));
   }
   block_acc(s, acc);
 }

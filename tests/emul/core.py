@@ -448,9 +448,11 @@ def pase_l1_bwd(pred, target, n, coef, gscale, dpred):
 
 
 def pase_bce_pairs_fwd(logit, n, n_pos, acc):
+    # the kernel's stable element loss max(v, 0) - v y + log1p(e^-|v|) in fp32 (torch's
+    # binary_cross_entropy_with_logits returns 0 for a confident y = 0 logit)
+    v = logit[:n]
     y = (torch.arange(n) < n_pos).float()
-    acc[0] += torch.nn.functional.binary_cross_entropy_with_logits(
-        logit[:n], y, reduction="sum").double()
+    acc[0] += (v.clamp_min(0.0) - v * y + torch.log1p(torch.exp(-v.abs()))).double().sum()
 
 
 def pase_bce_pairs_bwd(logit, n, n_pos, coef, gscale, dlogit):
